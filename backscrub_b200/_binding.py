@@ -31,6 +31,7 @@ SYMBOLS = [
     "bsb_calcmask_frames_done", "bsb_calcmask_mask_serial",
     "bsb_background_new_still", "bsb_background_new_video", "bsb_background_delete", "bsb_background_grab", "bsb_background_grab_into",
     "bsb_background_thumbnail", "bsb_background_frame", "bsb_background_running",
+    "bsb_set_sources", "bsb_reset_source", "bsb_set_source_background", "bsb_composite_sources", "bsb_composite_sources_yuyv_device",
 ]
 
 
@@ -119,4 +120,11 @@ def bind(path: str) -> C.CDLL:
     L.bsb_background_thumbnail.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, i32p, i32p]
     L.bsb_background_frame.argtypes = [C.c_void_p]
     L.bsb_background_running.argtypes = [C.c_void_p]
+    L.bsb_set_sources.argtypes = [C.c_void_p, C.c_int]
+    L.bsb_reset_source.argtypes = [C.c_void_p, C.c_int]
+    L.bsb_set_source_background.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_size_t]
+    L.bsb_composite_sources.argtypes = [C.c_void_p, C.c_int, i32p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t,
+                                        C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
+    L.bsb_composite_sources_yuyv_device.argtypes = [C.c_void_p, C.c_int, i32p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
+                                                    C.c_void_p, C.c_size_t, C.c_int]
     return L

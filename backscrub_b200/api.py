@@ -201,6 +201,61 @@ class MaskGen:
                                                    d_mask or None, npx, int(sync)):
             self._fail("bsb_composite_yuyv_device")
 
+    # -- independent sources: one frame from each of several cameras per call
+    @staticmethod
+    def _ids(ids):
+        ids = [int(i) for i in ids]
+        return len(ids), (C.c_int * max(1, len(ids)))(*ids)
+
+    def set_sources(self, n_sources: int):
+        """n_sources zeroed smoother states + per-source background slots (again: everything reset)."""
+        if not self._lib.bsb_set_sources(self._h, int(n_sources)):
+            self._fail("bsb_set_sources")
+
+    def reset_source(self, source: int):
+        """start `source` over as a new camera (its smoother state is zeroed)"""
+        if not self._lib.bsb_reset_source(self._h, int(source)):
+            self._fail("bsb_reset_source")
+
+    def set_source_background(self, source: int, bg_raw=None):
+        """background of one source (resized like set_background); None = blend the context background again."""
+        if bg_raw is None:
+            ok = self._lib.bsb_set_source_background(self._h, int(source), None, 0, 0, 0)
+        else:
+            bg_raw = np.ascontiguousarray(bg_raw, np.uint8)
+            ok = self._lib.bsb_set_source_background(self._h, int(source), _ptr(bg_raw), bg_raw.shape[1], bg_raw.shape[0], bg_raw.shape[1] * 3)
+        if not ok:
+            self._fail("bsb_set_source_background")
+
+    def composite_sources(self, frames: np.ndarray, ids, want_out=True, want_yuyv=True, want_mask=True):
+        """HOST buffers: frames [n, H, W, 3], frame b the next frame of source ids[b] (distinct ids) -> (out, yuyv, mask)."""
+        frames = np.ascontiguousarray(frames, np.uint8)
+        n, tab = self._ids(ids)
+        if frames.shape != (n, self.height, self.width, 3):
+            raise BackscrubError(f"frames shape {frames.shape} != {(n, self.height, self.width, 3)}")
+        fb, npx = self.height * self.width * 3, self.height * self.width
+        ow, oh = self.out_width, self.out_height
+        out = np.empty((n, oh, ow, 3), np.uint8) if want_out else None
+        yuyv = np.empty((n, oh, ow, 2), np.uint8) if want_yuyv else None
+        mask = np.empty((n, self.height, self.width), np.uint8) if want_mask else None
+        ok = self._lib.bsb_composite_sources(self._h, n, tab, _ptr(frames), self.width * 3, fb,
+                                             _ptr(out) if want_out else None, ow * oh * 3,
+                                             _ptr(yuyv) if want_yuyv else None, ow * oh * 2,
+                                             _ptr(mask) if want_mask else None, npx)
+        if not ok:
+            self._fail("bsb_composite_sources")
+        return out, yuyv, mask
+
+    def composite_sources_yuyv_device(self, n, ids, d_yuyv_in, d_out=0, d_yuyv=0, d_mask=0, sync=False):
+        """DEVICE-resident camera YUYV frames (tightly packed), frame b of source ids[b]; asynchronous unless `sync`."""
+        m, tab = self._ids(ids)
+        if m != n:
+            raise BackscrubError(f"{m} source ids for {n} frames")
+        npx, opx = self.height * self.width, self.out_width * self.out_height
+        if not self._lib.bsb_composite_sources_yuyv_device(self._h, n, tab, d_yuyv_in, d_out or None, opx * 3, d_yuyv or None, opx * 2,
+                                                           d_mask or None, npx, int(sync)):
+            self._fail("bsb_composite_sources_yuyv_device")
+
     def synchronize(self):
         if not self._lib.bsb_synchronize(self._h):
             self._fail("bsb_synchronize")

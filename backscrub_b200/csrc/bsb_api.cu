@@ -432,6 +432,77 @@ int bsb_composite_yuyv_device(bsb_ctx* ctx, int n_frames, const uint8_t* d_yuyv_
   return 1;
 }
 
+// ---- independent sources ---------------------------------------------------------
+int bsb_set_sources(bsb_ctx* ctx, int n_sources) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_sources(n_sources, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
+int bsb_reset_source(bsb_ctx* ctx, int source) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->reset_source(source, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
+int bsb_set_source_background(bsb_ctx* ctx, int source, const uint8_t* bg_raw, int w, int h, size_t pitch) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_source_background(source, bg_raw, w, h, pitch, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
+int bsb_composite_sources(bsb_ctx* ctx, int n, const int* source_ids, const uint8_t* frames, size_t frame_pitch, size_t frame_stride,
+                          uint8_t* out, size_t out_stride, uint8_t* out_yuyv, size_t yuyv_stride, uint8_t* out_mask, size_t mask_stride) {
+  if (!check_ctx(ctx)) return 0;
+  const bsb::Callbacks* cbp = &ctx->cb;
+  Engine* e = ctx->eng;
+  const size_t row = (size_t)e->W() * 3, fbytes = row * e->H(), npix = (size_t)e->W() * e->H();
+  const size_t orow = (size_t)e->out_w() * 3, obytes = orow * e->out_h(), opix = (size_t)e->out_w() * e->out_h();
+  if (n < 1 || n > e->max_batch()) { report(cbp, "error: n_frames out of range (1..max_batch)"); return 0; }
+  if (!frames || frame_pitch < row) { report(cbp, "error: invalid frame"); return 0; }
+  if (out_yuyv && (e->out_w() & 1)) { report(cbp, "error: YUYV output needs an even width"); return 0; }
+  API_CUDA(cudaSetDevice(e->device()));
+  if (frame_pitch == row && frame_stride == fbytes) {
+    API_CUDA(cudaMemcpyAsync(e->d_frames(), frames, fbytes * n, cudaMemcpyHostToDevice, e->stream()));
+  } else {
+    for (int b = 0; b < n; ++b)
+      API_CUDA(cudaMemcpy2DAsync(e->d_frames() + b * fbytes, row, frames + (size_t)b * frame_stride, frame_pitch, row, (size_t)e->H(),
+                                 cudaMemcpyHostToDevice, e->stream()));
+  }
+  std::string err;
+  if (!e->run_sources(n, source_ids, e->d_frames(), row, fbytes, out ? e->d_out() : nullptr, obytes, out_yuyv ? e->d_yuyv() : nullptr, opix * 2,
+                      out_mask ? e->d_mask() : nullptr, npix, &err)) {
+    report(cbp, "error: " + err); return 0;
+  }
+  if (out) for (int b = 0; b < n; ++b)
+    API_CUDA(cudaMemcpyAsync(out + (size_t)b * out_stride, e->d_out() + b * obytes, obytes, cudaMemcpyDeviceToHost, e->stream()));
+  if (out_yuyv) for (int b = 0; b < n; ++b)
+    API_CUDA(cudaMemcpyAsync(out_yuyv + (size_t)b * yuyv_stride, e->d_yuyv() + b * opix * 2, opix * 2, cudaMemcpyDeviceToHost, e->stream()));
+  if (out_mask) for (int b = 0; b < n; ++b)
+    API_CUDA(cudaMemcpyAsync(out_mask + (size_t)b * mask_stride, e->d_mask() + b * npix, npix, cudaMemcpyDeviceToHost, e->stream()));
+  API_CUDA(cudaStreamSynchronize(e->stream()));
+  API_CUDA(cudaGetLastError());
+  return 1;
+}
+
+int bsb_composite_sources_yuyv_device(bsb_ctx* ctx, int n, const int* source_ids, const uint8_t* d_yuyv_frames, uint8_t* d_out, size_t out_stride,
+                                      uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, int sync) {
+  if (!check_ctx(ctx)) return 0;
+  const bsb::Callbacks* cbp = &ctx->cb;
+  Engine* e = ctx->eng;
+  if (!d_yuyv_frames) { report(cbp, "error: invalid frame"); return 0; }
+  if (d_yuyv && (e->out_w() & 1)) { report(cbp, "error: YUYV output needs an even width"); return 0; }
+  std::string err;
+  if (!e->run_sources_yuyv(n, source_ids, d_yuyv_frames, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, &err)) {
+    report(cbp, "error: " + err); return 0;
+  }
+  if (sync) { API_CUDA(cudaStreamSynchronize(e->stream())); API_CUDA(cudaGetLastError()); }
+  return 1;
+}
+
 int bsb_synchronize(bsb_ctx* ctx) {
   if (!check_ctx(ctx)) return 0;
   std::string err;

@@ -869,6 +869,8 @@ Engine::~Engine() {
                   (void*)d_gauss_tmp_, (void*)d_stage_a_, (void*)d_stage_b_, (void*)d_stage_c_, (void*)d_bg_yuyv_, (void*)pool_counters_, (void*)d_tile_geo_})
     if (p) cudaFree(p);
   for (ChainPlan& cp : chains_) if (cp.d_ops) cudaFree(cp.d_ops);
+  free_sources();
+  for (void* p : {(void*)d_src_tab_, (void*)d_src_raw_, tab_src_.blob}) if (p) cudaFree(p);
   if (h_mask_) cudaFreeHost(h_mask_);
   if (stream_) cudaStreamDestroy(stream_);
 }
@@ -1067,13 +1069,19 @@ void Engine::run_step(size_t si, int n, bool from_u8, bool* first_p, bool* skip_
 }
 
 void Engine::enqueue_decision(int n) {
+  const bool sources = call_mode_ != CALL_PLAIN;      // per-source states, looked up through the id table
   if (dec_up_step_ >= 0) {
     const Step& st = steps_[dec_up_step_];
     const TensorInfo& I = tinfo_[st.in];
-    launch_decision_up_iir(stream_, n, tptr(st.in), I.h, I.w, I.ld, st.align_corners, st.half_pixel, oh_, ow_, state_, ofinal_, opitch_);
+    if (sources)
+      launch_decision_up_sources(stream_, n, tptr(st.in), I.h, I.w, I.ld, st.align_corners, st.half_pixel, oh_, ow_, src_state_, d_src_tab_,
+                                 ofinal_, opitch_);
+    else
+      launch_decision_up_iir(stream_, n, tptr(st.in), I.h, I.w, I.ld, st.align_corners, st.half_pixel, oh_, ow_, state_, ofinal_, opitch_);
     return;
   }
-  launch_decision_iir(stream_, model_type_, n, tptr(g_.output), oh_, ow_, oc_, state_, ofinal_, opitch_);
+  if (sources) launch_decision_sources(stream_, model_type_, n, tptr(g_.output), oh_, ow_, oc_, src_state_, d_src_tab_, ofinal_, opitch_);
+  else launch_decision_iir(stream_, model_type_, n, tptr(g_.output), oh_, ow_, oc_, state_, ofinal_, opitch_);
 }
 
 // PostArgs of one call.  `yuyv_native` (optional out): the frames can stay in camera YUYV format for the post kernel.
@@ -1094,6 +1102,13 @@ PostArgs Engine::post_args(int n, const uint8_t* d_frames, size_t pitch, size_t 
     a.bg = d_bg_frames_; a.bg_stride = fbytes;            // the blurred camera frame itself (filled by enqueue_post)
   }
   if (bg_yuyv_valid_ && !(bgblur_k_ && !has_bg_)) a.bg_yuyv = d_bg_yuyv_;
+  if (call_mode_ != CALL_PLAIN) {
+    // sources: frame b blends bank slot bg_index[b]; the bank's YUYV holds no camera-blur slots, so a call with such a
+    // frame converts every tile (what a plain context in camera-blur mode does)
+    a.bg = d_bank_; a.bg_stride = fbytes; a.bg_cursor = nullptr; a.bg_advance = 0;
+    a.bg_index = d_src_tab_ + max_batch_; a.bg_count = bank_slots();
+    a.bg_yuyv = (call_mode_ == CALL_SOURCES && !(W_ & 1)) ? d_bank_yuyv_ : nullptr;
+  }
   a.ofinal = ofinal_; a.ow = ow_; a.oh = oh_; a.opitch = opitch_;
   a.out_x = out_roidim_[0]; a.out_y = out_roidim_[1]; a.out_w = out_roidim_[2]; a.out_h = out_roidim_[3];
   a.roi_x = roidim_[0]; a.roi_y = roidim_[1]; a.roi_w = roidim_[2]; a.roi_h = roidim_[3];
@@ -1116,9 +1131,12 @@ void Engine::enqueue_post(int n, const uint8_t* d_frames, size_t pitch, size_t s
   const size_t fbytes = (size_t)W_ * H_ * 3;
   const bool flip = flip_h_ || flip_v_, resized = out_w_ != W_ || out_h_ != H_, tail = flip || resized;
   const bool want_rgb = d_out || d_yuyv;
-  const bool ring = has_bg_ && bg_count_ > 1;
-  // app/deepseg.cc:652-658: no background source => the background is the blurred camera frame itself
-  if (!has_bg_ && bgblur_k_ && want_rgb)
+  const bool ring = call_mode_ == CALL_PLAIN && has_bg_ && bg_count_ > 1;
+  // app/deepseg.cc:652-658: no background source => the background is the blurred camera frame itself (sources: into the
+  // bank's camera-blur slots, slot b = frame b)
+  if (call_mode_ == CALL_SOURCES_CAMBLUR && want_rgb)
+    launch_gauss_blur(stream_, n, d_frames, pitch, stride, d_gauss_tmp_, d_bank_, (size_t)W_ * 3, fbytes, W_, H_, taps_);
+  else if (call_mode_ == CALL_PLAIN && !has_bg_ && bgblur_k_ && want_rgb)
     launch_gauss_blur(stream_, n, d_frames, pitch, stride, d_gauss_tmp_, d_bg_frames_, (size_t)W_ * 3, fbytes, W_, H_, taps_);
   const PostArgs a = post_args(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in);
   launch_post(stream_, a);
@@ -1147,7 +1165,8 @@ void Engine::enqueue_post(int n, const uint8_t* d_frames, size_t pitch, size_t s
 // the blur-my-background mode, whose Gaussian runs on the BGR frame.
 bool Engine::yuyv_native(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
                          uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in) const {
-  if (!d_yuyv_in || (bgblur_k_ && !has_bg_)) return false;
+  const bool camblur = call_mode_ == CALL_PLAIN ? (bgblur_k_ && !has_bg_) : call_mode_ == CALL_SOURCES_CAMBLUR;
+  if (!d_yuyv_in || camblur) return false;
   return post_tma_eligible(post_args(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in));
 }
 
@@ -1186,7 +1205,7 @@ bool Engine::run(int n, const uint8_t* d_frames, size_t pitch, size_t stride, ui
   }
 #ifndef BSB_EMU
   const GraphKey key{n, d_frames, pitch, stride, d_out, d_yuyv, d_mask, d_yuyv_in, d_out ? out_stride : 0, d_yuyv ? yuyv_stride : 0,
-                     d_mask ? mask_stride : 0};
+                     d_mask ? mask_stride : 0, call_mode_};
   auto it = graphs_.find(key);
   if (it == graphs_.end()) {
     if (graphs_.size() >= 64) drop_graphs();
@@ -1275,6 +1294,7 @@ bool Engine::set_background_ring(const uint8_t* frames, int count, int bw, int b
   has_bg_ = true;
   if (!refresh_bg_blur(err)) return false;
   if (!refresh_bg_yuyv(err)) return false;
+  if (!refresh_bank_ctx(err)) return false;
   CUDA_OK(cudaStreamSynchronize(stream_));
   CUDA_OK(cudaGetLastError());
   return true;
@@ -1327,6 +1347,9 @@ bool Engine::set_bgblur(int k, std::string* err) {
   bgblur_k_ = k; taps_ = t;
   if (!refresh_bg_blur(err)) return false;
   if (!refresh_bg_yuyv(err)) return false;
+  if (!refresh_bank_ctx(err)) return false;
+  for (int s = 0; s < n_sources_; ++s)
+    if (!refresh_bank_source(s, err)) return false;
   CUDA_OK(cudaStreamSynchronize(stream_));
   return true;
 }
@@ -1365,6 +1388,146 @@ bool Engine::reset_state(std::string* err) {
   CUDA_OK(cudaMemsetAsync(state_, 0, (size_t)oh_ * ow_, stream_));
   CUDA_OK(cudaStreamSynchronize(stream_));
   return true;
+}
+
+// ---------------------------------------------------------------------------
+// independent sources
+// ---------------------------------------------------------------------------
+void Engine::free_sources() {
+  for (void* p : {(void*)src_state_, (void*)d_bank_, (void*)d_bank_yuyv_, (void*)d_src_bg_}) if (p) cudaFree(p);
+  src_state_ = nullptr; d_bank_ = nullptr; d_bank_yuyv_ = nullptr; d_src_bg_ = nullptr;
+  n_sources_ = 0;
+  src_has_bg_.clear();
+}
+
+bool Engine::set_sources(int n_sources, std::string* err) {
+  if (n_sources < 1 || n_sources > 65536) { *err = "n_sources out of range (1..65536)"; return false; }
+  CUDA_OK(cudaSetDevice(device_));
+  CUDA_OK(cudaStreamSynchronize(stream_));
+  drop_graphs();                                  // captured launches hold the old state / bank pointers
+  free_sources();
+  const size_t fbytes = (size_t)W_ * H_ * 3, npix = (size_t)W_ * H_, opx = (size_t)oh_ * ow_;
+  const size_t slots = (size_t)max_batch_ + 1 + (size_t)n_sources;
+  if (!d_src_tab_) {
+    CUDA_OK(cudaMalloc((void**)&d_src_tab_, 2 * (size_t)max_batch_ * sizeof(int)));
+    CUDA_OK(cudaMemset(d_src_tab_, 0, 2 * (size_t)max_batch_ * sizeof(int)));
+  }
+  CUDA_OK(cudaMalloc((void**)&src_state_, (size_t)n_sources * opx));
+  CUDA_OK(cudaMemset(src_state_, 0, (size_t)n_sources * opx));
+  CUDA_OK(cudaMalloc((void**)&d_bank_, slots * fbytes));
+  CUDA_OK(cudaMemset(d_bank_, 0, slots * fbytes));
+  if (!(W_ & 1)) {
+    CUDA_OK(cudaMalloc((void**)&d_bank_yuyv_, slots * npix * 2));
+    CUDA_OK(cudaMemset(d_bank_yuyv_, 0, slots * npix * 2));
+  }
+  CUDA_OK(cudaMalloc((void**)&d_src_bg_, (size_t)n_sources * fbytes));
+  n_sources_ = n_sources;
+  src_has_bg_.assign((size_t)n_sources, 0);
+  if (!refresh_bank_ctx(err)) return false;
+  CUDA_OK(cudaStreamSynchronize(stream_));
+  return true;
+}
+
+bool Engine::reset_source(int source, std::string* err) {
+  if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
+  if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
+  CUDA_OK(cudaSetDevice(device_));
+  const size_t opx = (size_t)oh_ * ow_;
+  CUDA_OK(cudaMemsetAsync(src_state_ + (size_t)source * opx, 0, opx, stream_));
+  CUDA_OK(cudaStreamSynchronize(stream_));
+  return true;
+}
+
+// bank slot of the context's effective background: the still background (blurred when bgblur is on), or plain green
+bool Engine::refresh_bank_ctx(std::string* err) {
+  if (!d_bank_ || bg_count_ > 1) return true;     // a ring of several images cannot serve sources calls (they reject it)
+  const size_t fbytes = (size_t)W_ * H_ * 3, npix = (size_t)W_ * H_;
+  uint8_t* slot = d_bank_ + (size_t)max_batch_ * fbytes;
+  CUDA_OK(cudaMemcpyAsync(slot, (has_bg_ && bgblur_k_) ? d_bg_eff_ : d_bg_, fbytes, cudaMemcpyDeviceToDevice, stream_));
+  if (d_bank_yuyv_) launch_rgb_to_yuyv(stream_, slot, d_bank_yuyv_ + (size_t)max_batch_ * npix * 2, npix);
+  CUDA_OK(cudaGetLastError());
+  return true;
+}
+
+// bank slot of source s from its resized background: blurred once when bgblur is on, then its YUYV
+bool Engine::refresh_bank_source(int s, std::string* err) {
+  if (!src_has_bg_[s]) return true;
+  const size_t fbytes = (size_t)W_ * H_ * 3, npix = (size_t)W_ * H_, k = (size_t)max_batch_ + 1 + (size_t)s;
+  const uint8_t* src = d_src_bg_ + (size_t)s * fbytes;
+  uint8_t* slot = d_bank_ + k * fbytes;
+  if (bgblur_k_) launch_gauss_blur(stream_, 1, src, (size_t)W_ * 3, fbytes, d_gauss_tmp_, slot, (size_t)W_ * 3, fbytes, W_, H_, taps_);
+  else CUDA_OK(cudaMemcpyAsync(slot, src, fbytes, cudaMemcpyDeviceToDevice, stream_));
+  if (d_bank_yuyv_) launch_rgb_to_yuyv(stream_, slot, d_bank_yuyv_ + k * npix * 2, npix);
+  CUDA_OK(cudaGetLastError());
+  return true;
+}
+
+bool Engine::set_source_background(int source, const uint8_t* bg_raw, int bw, int bh, size_t pitch, std::string* err) {
+  if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
+  if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
+  if (!bg_raw) { src_has_bg_[source] = 0; return true; }     // later calls blend the context background again
+  if (bw <= 0 || bh <= 0 || pitch < (size_t)bw * 3) { *err = "invalid background"; return false; }
+  CUDA_OK(cudaSetDevice(device_));
+  const size_t raw = (size_t)bw * bh * 3, fbytes = (size_t)W_ * H_ * 3;
+  if (raw > src_raw_cap_) {
+    CUDA_OK(cudaStreamSynchronize(stream_));
+    if (d_src_raw_) cudaFree(d_src_raw_);
+    d_src_raw_ = nullptr; src_raw_cap_ = 0;
+    CUDA_OK(cudaMalloc((void**)&d_src_raw_, raw));
+    src_raw_cap_ = raw;
+  }
+  if (bw != src_bg_w_ || bh != src_bg_h_) {
+    CUDA_OK(cudaStreamSynchronize(stream_));
+    if (!upload_resize_tab(build_resize_tab(bw, bh, W_, H_), &tab_src_, err)) return false;
+    src_bg_w_ = bw; src_bg_h_ = bh;
+  }
+  CUDA_OK(cudaMemcpy2DAsync(d_src_raw_, (size_t)bw * 3, bg_raw, pitch, (size_t)bw * 3, (size_t)bh, cudaMemcpyHostToDevice, stream_));
+  // app/background.cc:178-194: cv::resize(raw, out, Size(width, height))
+  launch_resize_u8c3(stream_, d_src_raw_, bw, bh, (size_t)bw * 3, d_src_bg_ + (size_t)source * fbytes, W_, H_, (size_t)W_ * 3, tab_src_.tab,
+                     tab_src_.area2x2);
+  src_has_bg_[source] = 1;
+  if (!refresh_bank_source(source, err)) return false;
+  CUDA_OK(cudaStreamSynchronize(stream_));
+  CUDA_OK(cudaGetLastError());
+  return true;
+}
+
+bool Engine::run_sources(int n, const int* ids, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
+                         uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, std::string* err,
+                         const uint8_t* d_yuyv_in) {
+  if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
+  if (n < 1 || n > max_batch_) { *err = "n_frames out of range (1..max_batch)"; return false; }
+  if (!ids) { *err = "null source id table"; return false; }
+  if (has_bg_ && bg_count_ > 1) { *err = "sources calls need a still context background (animate a source with bsb_set_source_background)"; return false; }
+  // frame b: state of source ids[b]; background = the source's own, else the context's, else (bgblur, no background
+  // at all) the blurred camera frame in camera-blur slot b
+  const bool ctx_camblur = bgblur_k_ && !has_bg_;
+  std::vector<int> tab(2 * (size_t)max_batch_, 0);
+  bool camblur = false;
+  for (int b = 0; b < n; ++b) {
+    const int id = ids[b];
+    if (id < 0 || id >= n_sources_) { *err = "source id out of range"; return false; }
+    for (int c = 0; c < b; ++c)
+      if (ids[c] == id) { *err = "source ids must be distinct within one call"; return false; }
+    tab[b] = id;
+    int slot = max_batch_;
+    if (src_has_bg_[id]) slot = max_batch_ + 1 + id;
+    else if (ctx_camblur) { slot = b; camblur = true; }
+    tab[(size_t)max_batch_ + b] = slot;
+  }
+  CUDA_OK(cudaSetDevice(device_));
+  // outside the graph, before its launch: stream order keeps the previous launch's reads ahead of this write
+  CUDA_OK(cudaMemcpyAsync(d_src_tab_, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, stream_));
+  call_mode_ = camblur ? CALL_SOURCES_CAMBLUR : CALL_SOURCES;
+  const bool ok = run(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, false, err, d_yuyv_in);
+  call_mode_ = CALL_PLAIN;
+  return ok;
+}
+
+bool Engine::run_sources_yuyv(int n, const int* ids, const uint8_t* d_yuyv_in, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv,
+                              size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, std::string* err) {
+  const size_t row = (size_t)W_ * 3;
+  return run_sources(n, ids, d_frames_, row, row * H_, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, err, d_yuyv_in);
 }
 
 double Engine::time_stage(int stage, int n, int iters, std::string* err) {

@@ -101,6 +101,20 @@ class Engine {
   bool set_output(bool flip_h, bool flip_v, int out_w, int out_h, std::string* err);
   bool sync(std::string* err);
   bool reset_state(std::string* err);
+
+  // Independent sources (camera streams) batched one frame each into a call.  set_sources allocates n zeroed smoother
+  // states and the per-source background bank (again: everything reallocated and zeroed, graphs dropped).
+  bool set_sources(int n_sources, std::string* err);
+  bool reset_source(int source, std::string* err);
+  // cv::resize(raw -> W x H) into the source's bank slot (+ bgblur, + its YUYV); bg_raw == nullptr clears the slot
+  bool set_source_background(int source, const uint8_t* bg_raw, int bw, int bh, size_t pitch, std::string* err);
+  // frame b belongs to source ids[b] (HOST array of n distinct ids); same buffers / layout as run()
+  bool run_sources(int n, const int* ids, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
+                   uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, std::string* err,
+                   const uint8_t* d_yuyv_in = nullptr);
+  bool run_sources_yuyv(int n, const int* ids, const uint8_t* d_yuyv_in, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv, size_t yuyv_stride,
+                        uint8_t* d_mask, size_t mask_stride, std::string* err);
+  int n_sources() const { return n_sources_; }
   double time_stage(int stage, int n, int iters, std::string* err);
 
   // accessors
@@ -257,13 +271,36 @@ class Engine {
   int last_call_launches_ = 0;
   size_t stage_a_cap_ = 0, stage_b_cap_ = 0, stage_c_cap_ = 0, out_cap_ = 0, yuyv_cap_ = 0;
 
+  // ---- independent sources (run_sources) ----
+  // Kind of the call being enqueued: plain (one stream, state_), sources, or sources with at least one frame that blends
+  // its own blurred camera frame (bgblur on, no background of either kind).
+  enum CallMode { CALL_PLAIN = 0, CALL_SOURCES = 1, CALL_SOURCES_CAMBLUR = 2 };
+  int call_mode_ = CALL_PLAIN;
+  int n_sources_ = 0;
+  uint8_t* src_state_ = nullptr;     // [n_sources][oh*ow] smoother state per source
+  int* d_src_tab_ = nullptr;         // [2][max_batch]: source id of frame b | background-bank slot of frame b (written before each launch)
+  // background bank, one base + one stride for the post kernel: [max_batch] camera-blur slots | [1] the context's effective
+  // background | [n_sources] source slots; d_bank_yuyv_ is its YUYV (valid for the context and source slots)
+  uint8_t* d_bank_ = nullptr, *d_bank_yuyv_ = nullptr;
+  uint8_t* d_src_bg_ = nullptr;      // [n_sources] resized, unblurred source backgrounds (re-blurred when bgblur changes)
+  uint8_t* d_src_raw_ = nullptr;     // staging of one decoded source background
+  size_t src_raw_cap_ = 0;
+  DevResizeTab tab_src_;
+  int src_bg_w_ = 0, src_bg_h_ = 0;
+  std::vector<char> src_has_bg_;
+  int bank_slots() const { return max_batch_ + 1 + n_sources_; }
+  bool refresh_bank_ctx(std::string* err);
+  bool refresh_bank_source(int s, std::string* err);
+  void free_sources();
+
   // everything a captured launch sequence bakes into its kernel arguments
   struct GraphKey {
     int n; const void* f; size_t pitch, stride; const void* o; const void* y; const void* m; const void* yin;
     size_t ostride, ystride, mstride;
+    int mode;                        // CallMode: a plain and a sources graph over the same buffers are different graphs
     bool operator<(const GraphKey& r) const {
-      return std::tie(n, f, pitch, stride, o, y, m, yin, ostride, ystride, mstride) <
-             std::tie(r.n, r.f, r.pitch, r.stride, r.o, r.y, r.m, r.yin, r.ostride, r.ystride, r.mstride);
+      return std::tie(n, f, pitch, stride, o, y, m, yin, ostride, ystride, mstride, mode) <
+             std::tie(r.n, r.f, r.pitch, r.stride, r.o, r.y, r.m, r.yin, r.ostride, r.ystride, r.mstride, r.mode);
     }
   };
 #ifndef BSB_EMU

@@ -179,6 +179,13 @@ void launch_decision_iir(cudaStream_t s, int model_type, int B, const float* mod
 // kernel) instead of writing and re-reading the 5.5 MB-per-frame tensor.
 void launch_decision_up_iir(cudaStream_t s, int B, const float* low, int ih, int iw, int ld, bool align_corners, bool half_pixel,
                             int oh, int ow, uint8_t* state, uint8_t* ofinal, int opitch);
+// Independent sources: frame b of the batch belongs to source src[b] (DEVICE table [B], ids distinct within the call) and
+// advances that source's state, states: [n_sources][oh*ow].  One step of the IIR per frame, every frame in parallel.
+void launch_decision_sources(cudaStream_t s, int model_type, int B, const float* model_out, int oh, int ow, int oc,
+                             uint8_t* states, const int* src, uint8_t* ofinal, int opitch);
+// DeepLab form with the final 33 -> 257 resize folded in (as launch_decision_up_iir)
+void launch_decision_up_sources(cudaStream_t s, int B, const float* low, int ih, int iw, int ld, bool align_corners, bool half_pixel,
+                                int oh, int ow, uint8_t* states, const int* src, uint8_t* ofinal, int opitch);
 // source coordinate / neighbours of RESIZE_BILINEAR (TF/lite/kernels/internal/reference/resize_bilinear.h:29-57)
 BSB_D void bsb_resize_interp(float value, float scale, bool half_pixel, int in_size, float* scaled, int* lo, int* hi) {
   *scaled = half_pixel ? (value + 0.5f) * scale - 0.5f : value * scale;
@@ -196,6 +203,7 @@ struct PostArgs {
   const uint8_t* frames; size_t frame_pitch, frame_stride;   // row pitch / per-frame stride (bytes)
   const uint8_t* bg; size_t bg_pitch, bg_stride;             // bg_stride 0 => one static background
   const int* bg_cursor; int bg_count, bg_advance;             // non-null: frame b blends ring image (*cursor + b*advance) % count
+  const int* bg_index;                                         // non-null (DEVICE [B]): frame b blends image bg_index[b] of bg_count (wins over bg_cursor)
   const uint8_t* ofinal; int ow, oh, opitch;                  // [B][oh][opitch]
   int out_x, out_y, out_w, out_h;                              // out_roidim inside ofinal
   int roi_x, roi_y, roi_w, roi_h;                              // roidim inside the frame

@@ -23,9 +23,11 @@ BSB_D uint8_t lin_v(int h0, int h1, int b0, int b1) {
 }
 
 // background of batch frame b: one static image (bg_stride 0), one image per frame, or a ring of
-// bg_count images entered at the device-side cursor (animated backgrounds, app/background.cc:126-176)
+// bg_count images entered at the device-side cursor (animated backgrounds, app/background.cc:126-176), or the image a
+// per-frame table names (independent sources)
 BSB_D size_t bg_frame_offset(const PostArgs& a, int b) {
-  if (a.bg_cursor) b = (int)(((unsigned)__ldg(a.bg_cursor) + (unsigned)b * (unsigned)a.bg_advance) % (unsigned)a.bg_count);
+  if (a.bg_index) b = __ldg(a.bg_index + b);
+  else if (a.bg_cursor) b = (int)(((unsigned)__ldg(a.bg_cursor) + (unsigned)b * (unsigned)a.bg_advance) % (unsigned)a.bg_count);
   return (size_t)b * a.bg_stride;
 }
 
@@ -271,32 +273,44 @@ void launch_decision_iir(cudaStream_t s, int model_type, int B, const float* mod
 // DeepLab: RESIZE_BILINEAR (33x33x21 -> 257x257x21) + argmax + IIR in one pass.  One thread = one output pixel; the four
 // neighbours and weights are those of k_resize_bilinear, the value of class i is formed with the same expression
 // (-fmad=false: every product and sum rounds separately), the argmax scans the classes in order with a strict >.
+struct UpTap { int o00, o10, o01, o11; float dy, dx, wy0, wx0; };
+
+BSB_D UpTap up_tap(int y, int x, int ih, int iw, int ld, float hs, float ws, bool half_pixel) {
+  float fy, fx; int y0, y1, x0, x1;
+  bsb_resize_interp((float)y, hs, half_pixel, ih, &fy, &y0, &y1);
+  bsb_resize_interp((float)x, ws, half_pixel, iw, &fx, &x0, &x1);
+  UpTap t;
+  t.dy = fy - (float)y0; t.dx = fx - (float)x0;
+  t.wy0 = 1.f - t.dy; t.wx0 = 1.f - t.dx;
+  t.o00 = (y0 * iw + x0) * ld; t.o10 = (y1 * iw + x0) * ld; t.o01 = (y0 * iw + x1) * ld; t.o11 = (y1 * iw + x1) * ld;
+  return t;
+}
+
+// the decision of one output pixel of one frame (`f`: that frame's 33x33x21 tensor): 1 = background (argmax != person)
+BSB_D unsigned up_decide(const float* f, const UpTap& t) {
+  float maxval = -10000.f; int maxpos = 0;
+#pragma unroll 7
+  for (int i = 0; i < 21; ++i) {
+    const float a = __ldg(f + t.o00 + i) * t.wy0 * t.wx0;
+    const float bb = __ldg(f + t.o10 + i) * t.dy * t.wx0;
+    const float d = __ldg(f + t.o01 + i) * t.wy0 * t.dx;
+    const float e = __ldg(f + t.o11 + i) * t.dy * t.dx;
+    const float v = ((a + bb) + d) + e;
+    if (v > maxval) { maxval = v; maxpos = i; }
+  }
+  return (maxpos == 15) ? 0u : 1u;
+}
+
 __global__ void __launch_bounds__(128) k_decision_up_iir(int B, const float* low, int ih, int iw, int ld, float hs, float ws, bool half_pixel,
                                                          int oh, int ow, uint8_t* state, uint8_t* ofinal, int opitch, int oframe) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= oh * ow) return;
   const int y = n / ow, x = n - y * ow;
-  float fy, fx; int y0, y1, x0, x1;
-  bsb_resize_interp((float)y, hs, half_pixel, ih, &fy, &y0, &y1);
-  bsb_resize_interp((float)x, ws, half_pixel, iw, &fx, &x0, &x1);
-  const float dy = fy - (float)y0, dx = fx - (float)x0;
-  const float wy0 = 1.f - dy, wx0 = 1.f - dx;
-  const int o00 = (y0 * iw + x0) * ld, o10 = (y1 * iw + x0) * ld, o01 = (y0 * iw + x1) * ld, o11 = (y1 * iw + x1) * ld;
+  const UpTap t = up_tap(y, x, ih, iw, ld, hs, ws, half_pixel);
   const int opos = y * opitch + x;
   unsigned st = state[n];
   for (int b = 0; b < B; ++b) {
-    const float* f = low + (size_t)b * ih * iw * ld;
-    float maxval = -10000.f; int maxpos = 0;
-#pragma unroll 7
-    for (int i = 0; i < 21; ++i) {
-      const float a = __ldg(f + o00 + i) * wy0 * wx0;
-      const float bb = __ldg(f + o10 + i) * dy * wx0;
-      const float d = __ldg(f + o01 + i) * wy0 * dx;
-      const float e = __ldg(f + o11 + i) * dy * dx;
-      const float v = ((a + bb) + d) + e;
-      if (v > maxval) { maxval = v; maxpos = i; }
-    }
-    const unsigned val = (maxpos == 15) ? 0u : 255u;
+    const unsigned val = up_decide(low + (size_t)b * ih * iw * ld, t) ? 255u : 0u;
     st = (val & 0xE0u) | (st >> 3);
     ofinal[(size_t)b * oframe + opos] = (uint8_t)st;
   }
@@ -314,26 +328,8 @@ __global__ void __launch_bounds__(DEC_PX * DEC_WARPS) k_decision_up_par(int B, c
   const unsigned s_in = valid ? state[n] : 0u;
   const int y = valid ? n / ow : 0, x = valid ? n - y * ow : 0;
   if (valid) {
-    float fy, fx; int y0, y1, x0, x1;
-    bsb_resize_interp((float)y, hs, half_pixel, ih, &fy, &y0, &y1);
-    bsb_resize_interp((float)x, ws, half_pixel, iw, &fx, &x0, &x1);
-    const float dy = fy - (float)y0, dx = fx - (float)x0;
-    const float wy0 = 1.f - dy, wx0 = 1.f - dx;
-    const int o00 = (y0 * iw + x0) * ld, o10 = (y1 * iw + x0) * ld, o01 = (y0 * iw + x1) * ld, o11 = (y1 * iw + x1) * ld;
-    for (int b = ty; b < B; b += DEC_WARPS) {
-      const float* f = low + (size_t)b * ih * iw * ld;
-      float maxval = -10000.f; int maxpos = 0;
-#pragma unroll 7
-      for (int i = 0; i < 21; ++i) {
-        const float a = __ldg(f + o00 + i) * wy0 * wx0;
-        const float bb = __ldg(f + o10 + i) * dy * wx0;
-        const float dd = __ldg(f + o01 + i) * wy0 * dx;
-        const float e = __ldg(f + o11 + i) * dy * dx;
-        const float v = ((a + bb) + dd) + e;
-        if (v > maxval) { maxval = v; maxpos = i; }
-      }
-      d[b * DEC_PX + tx] = (maxpos == 15) ? 0 : 1;
-    }
+    const UpTap t = up_tap(y, x, ih, iw, ld, hs, ws, half_pixel);
+    for (int b = ty; b < B; b += DEC_WARPS) d[b * DEC_PX + tx] = (uint8_t)up_decide(low + (size_t)b * ih * iw * ld, t);
   }
   __syncthreads();
   if (!valid) return;
@@ -353,6 +349,55 @@ void launch_decision_up_iir(cudaStream_t s, int B, const float* low, int ih, int
   }
   BSB_LAUNCH(k_decision_up_iir, dim3((unsigned)ceil_div(oh * ow, 128)), dim3(128), 0, s, B, low, ih, iw, ld, hs, ws, half_pixel, oh, ow, state,
              ofinal, opitch, oh * opitch);
+  count_launch();
+}
+
+// ---------------------------------------------------------------------------
+// Independent sources (one frame per source and call): frame b advances the state of source src[b] by exactly one IIR
+// step, st = (d ? 0xE0 : 0) | (state >> 3).  Ids are distinct within a call, so no two frames share a state byte and
+// every (pixel, frame) is independent: one thread each, blockIdx.y = frame, threads along pixels (coalesced state,
+// ofinal and model-output loads).
+// ---------------------------------------------------------------------------
+constexpr int DEC_SRC_T = 128;
+
+__global__ void __launch_bounds__(DEC_SRC_T) k_decision_sources(int model_type, const float* out_f, int npix, int oc, uint8_t* states,
+                                                                const int* src, uint8_t* ofinal, int ow, int opitch, int oframe) {
+  const int n = blockIdx.x * DEC_SRC_T + threadIdx.x, b = blockIdx.y;
+  if (n >= npix) return;
+  uint8_t* sp = states + (size_t)__ldg(src + b) * npix + n;
+  const unsigned st = (decide(model_type, out_f + ((size_t)b * npix + n) * oc) ? 0xE0u : 0u) | ((unsigned)*sp >> 3);
+  ofinal[(size_t)b * oframe + (n / ow) * opitch + (n % ow)] = (uint8_t)st;
+  *sp = (uint8_t)st;
+}
+
+__global__ void __launch_bounds__(DEC_SRC_T) k_decision_up_sources(const float* low, int ih, int iw, int ld, float hs, float ws, bool half_pixel,
+                                                                   int oh, int ow, uint8_t* states, const int* src, uint8_t* ofinal, int opitch,
+                                                                   int oframe) {
+  const int n = blockIdx.x * DEC_SRC_T + threadIdx.x, b = blockIdx.y;
+  if (n >= oh * ow) return;
+  const int y = n / ow, x = n - y * ow;
+  uint8_t* sp = states + (size_t)__ldg(src + b) * oh * ow + n;
+  const unsigned d = up_decide(low + (size_t)b * ih * iw * ld, up_tap(y, x, ih, iw, ld, hs, ws, half_pixel));
+  const unsigned st = (d ? 0xE0u : 0u) | ((unsigned)*sp >> 3);
+  ofinal[(size_t)b * oframe + y * opitch + x] = (uint8_t)st;
+  *sp = (uint8_t)st;
+}
+
+void launch_decision_sources(cudaStream_t s, int model_type, int B, const float* model_out, int oh, int ow, int oc,
+                             uint8_t* states, const int* src, uint8_t* ofinal, int opitch) {
+  const int npix = oh * ow;
+  BSB_LAUNCH(k_decision_sources, dim3((unsigned)ceil_div(npix, DEC_SRC_T), (unsigned)B), dim3(DEC_SRC_T), 0, s, model_type, model_out, npix, oc,
+             states, src, ofinal, ow, opitch, oh * opitch);
+  count_launch();
+}
+
+void launch_decision_up_sources(cudaStream_t s, int B, const float* low, int ih, int iw, int ld, bool align_corners, bool half_pixel,
+                                int oh, int ow, uint8_t* states, const int* src, uint8_t* ofinal, int opitch) {
+  float hs = (float)ih / (float)oh, ws = (float)iw / (float)ow;
+  if (align_corners && oh > 1) hs = (float)(ih - 1) / (float)(oh - 1);
+  if (align_corners && ow > 1) ws = (float)(iw - 1) / (float)(ow - 1);
+  BSB_LAUNCH(k_decision_up_sources, dim3((unsigned)ceil_div(oh * ow, DEC_SRC_T), (unsigned)B), dim3(DEC_SRC_T), 0, s, low, ih, iw, ld, hs, ws,
+             half_pixel, oh, ow, states, src, ofinal, opitch, oh * opitch);
   count_launch();
 }
 

@@ -131,7 +131,8 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
     // ... then the big tiles: the background tile (L2-resident for a still image) and its cached YUYV (a background
     // tile needs nothing else, a mixed tile has its second operand early) ...
     int bgi = 0;
-    if (a.bg_cursor) bgi = (int)(((unsigned)__ldg(a.bg_cursor) + (unsigned)b * (unsigned)a.bg_advance) % (unsigned)a.bg_count);
+    if (a.bg_index) bgi = __ldg(a.bg_index + b);
+    else if (a.bg_cursor) bgi = (int)(((unsigned)__ldg(a.bg_cursor) + (unsigned)b * (unsigned)a.bg_advance) % (unsigned)a.bg_count);
     else if (a.bg_stride) bgi = b;
     tma::mbar_expect_tx(barB, (unsigned)L::F_BYTES + (cfg.has_bgy ? (unsigned)L::Y_BYTES : 0u));
     tma::load_3d(sB, &tm.bg, blockIdx.x * (TW * 3 / 4), ty0, bgi, barB);
@@ -352,7 +353,7 @@ static bool make_map(CUtensorMap* m, const void* base, bool words, size_t row_by
 static bool build_post_maps(const PostArgs& a, PostMaps* tm, int TW) {
   const unsigned bw3 = (unsigned)TW * 3, bw2 = (unsigned)TW * 2, pw = TW == 128 ? (unsigned)PtL<128>::PW : (unsigned)PtL<64>::PW;
   const size_t W = (size_t)a.W, H = (size_t)a.H, B = (size_t)a.B;
-  const size_t nbg = a.bg_cursor ? (size_t)a.bg_count : (a.bg_stride ? B : 1);
+  const size_t nbg = (a.bg_index || a.bg_cursor) ? (size_t)a.bg_count : (a.bg_stride ? B : 1);
   bool ok = true;
   if (a.yuyv_in) ok = ok && make_map(&tm->frame, a.yuyv_in, true, W * 2, H, B, W * 2, a.yuyv_in_stride, bw2, PF_H);
   else ok = ok && make_map(&tm->frame, a.frames, true, W * 3, H, B, a.frame_pitch, a.frame_stride, bw3, PF_H);

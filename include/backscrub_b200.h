@@ -68,7 +68,8 @@ BSB_API bsb_ctx* bsb_maskgen_new(const char* modelname, size_t threads, size_t w
                                  bsb_stage_cb onmask, void* caller_ctx);
 
 /* Same, with the GPU-side knobs: CUDA device ordinal, maximum frames per launch
- * (consecutive frames of ONE stream; the IIR advances in order), flags above. */
+ * (consecutive frames of ONE stream, the IIR advancing in order — or, through the sources
+ * calls below, one frame each of up to max_batch independent cameras), flags above. */
 BSB_API bsb_ctx* bsb_maskgen_new_ex(const char* modelname, size_t width, size_t height, int device,
                                     int max_batch, unsigned flags, bsb_debug_cb ondebug, bsb_stage_cb onprep,
                                     bsb_stage_cb oninfer, bsb_stage_cb onmask, void* caller_ctx);
@@ -146,6 +147,38 @@ BSB_API int bsb_decode_mjpg(bsb_ctx* ctx, const uint8_t* jpeg, size_t jpeg_size,
 BSB_API int bsb_composite_yuyv_device(bsb_ctx* ctx, int n_frames, const uint8_t* d_yuyv_frames,
                                       uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv, size_t yuyv_stride,
                                       uint8_t* d_mask, size_t mask_stride, int sync);
+
+/* ---- independent sources: one frame from each of several cameras in one launch ----------
+ * A "source" is one camera stream with its own temporal smoother state (what one
+ * bs_maskgen_new context holds in the reference, lib/libbackscrub.cc:161-259).  A sources call
+ * composites frame b as the next frame of source source_ids[b]; source_ids is a HOST array of
+ * n_frames ids, all distinct, each in [0, n_sources), 1 <= n_frames <= max_batch.  Frame b blends,
+ * in this order: the source's own background (bsb_set_source_background); else the context
+ * background (bsb_set_background, or the green default), blurred when bgblur is on; else, with
+ * bgblur on and no background of either kind, its own blurred camera frame (app/deepseg.cc:652-658).
+ * bsb_set_bgblur and bsb_set_output apply to every frame; callbacks do not fire; the context
+ * background must not be a ring of more than one image.  Plain calls never touch the per-source
+ * states and sources calls never touch the plain smoother state, so both can be mixed on one
+ * context.  A violated rule returns 0 with a bsb_last_error() message and leaves the context usable. */
+/* Allocates n_sources zeroed smoother states and the per-source background bank (n_sources may
+ * exceed max_batch).  Calling it again reallocates and zeroes everything. */
+BSB_API int bsb_set_sources(bsb_ctx* ctx, int n_sources);
+/* Zeroes one source's smoother state: the source starts over as a new camera. */
+BSB_API int bsb_reset_source(bsb_ctx* ctx, int source);
+/* bsb_set_background for one source: cv::resize(raw -> W x H) on the GPU (app/background.cc:178-194) into
+ * the source's slot, blurred once if bgblur is on.  bg_raw NULL clears the slot (the source blends the
+ * context background again).  Video backgrounds: call again for each decoded frame. */
+BSB_API int bsb_set_source_background(bsb_ctx* ctx, int source, const uint8_t* bg_raw, int bg_w, int bg_h, size_t bg_pitch);
+/* HOST buffers, BGR frames, laid out as in bsb_composite (out rows tightly packed, `out_stride` bytes
+ * per frame).  Any of out / out_yuyv / out_mask may be NULL. */
+BSB_API int bsb_composite_sources(bsb_ctx* ctx, int n_frames, const int* source_ids, const uint8_t* frames, size_t frame_pitch,
+                                  size_t frame_stride, uint8_t* out, size_t out_stride, uint8_t* out_yuyv, size_t yuyv_stride,
+                                  uint8_t* out_mask, size_t mask_stride);
+/* DEVICE pointers, camera YUYV frames, laid out as in bsb_composite_yuyv_device; asynchronous unless
+ * `sync`.  The id table is copied before the call returns, so it may be reused at once. */
+BSB_API int bsb_composite_sources_yuyv_device(bsb_ctx* ctx, int n_frames, const int* source_ids, const uint8_t* d_yuyv_frames,
+                                              uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv, size_t yuyv_stride,
+                                              uint8_t* d_mask, size_t mask_stride, int sync);
 /* ---- asynchronous mask front-end: the reference's CalcMask (app/deepseg.cc:159-286) ----
  * A worker thread owns the mask-generation context.  set_input_frame clones the frame and wakes the worker (a
  * frame that arrives while the worker is busy replaces the pending one: latest frame wins); get_output_mask copies
