@@ -86,13 +86,14 @@ void launch_mb_block(cudaStream_t s, int B, const MbBlockArgs& a);
 // Low-resolution chain (the MobileNetV3 "middle" of the Meet / MLKit graphs: every tensor has P = h*w <= 256 pixels and
 // <= 128 channels): ONE kernel, one CTA per frame, walks a list of ops with every activation resident in shared
 // memory —  X [P][32] (the narrow block input / output), D [P][128] (the expanded tensor after its depthwise conv),
-// E [P][32] (one 32-channel slice of the expanded tensor).  Each op accumulates in the order of the stand-alone kernel it
+// E (one zero-haloed 16- or 32-channel slice of the expanded tensor: 16 where that fits two CTAs on an SM, i.e. Meet's
+// 9x16 and 6x10; 32 for MLKit's 16x16).  Each op accumulates in the order of the stand-alone kernel it
 // replaces (k ascending fmaf, taps in (fy, fx) order, pool rows-then-columns), so results are bit-identical.
 enum ChainOpType : int {
   CH_DWG = 0,         // depthwise k x k (stride s) from a GLOBAL tensor [ih*iw][ld] into D            (block entry)
   CH_SE = 1,          // global average pool of D or X -> FC (-> FC) -> channel scale vector sv
   CH_PW = 2,          // 1x1 conv: src (D or X, optionally * sv) -> dst (X or D), optional in-place residual
-  CH_EXPAND_DW = 3,   // X -> 1x1 expand (+act) -> depthwise k x k stride 1 (+act) -> D, 32 channels at a time
+  CH_EXPAND_DW = 3,   // X -> 1x1 expand (+act) -> depthwise k x k stride 1 (+act) -> D, one E slice at a time
   CH_SCALE_STORE = 4  // global out[p][c] = D[p][c] * sv[c]                                             (chain exit)
 };
 struct ChainOp {

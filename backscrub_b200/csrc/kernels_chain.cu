@@ -5,12 +5,16 @@
 // (reference kernels: depthwiseconv_float.h:25-96, pooling.h:26-79, fully_connected.h:27-61, conv.h:25-99; delegated to
 // XNNPACK by the reference, xnnpack_delegate.cc:1840-2497).  None of those launches can fill the GPU, and the SE
 // reductions serialise them.  Here one CTA owns one frame and keeps every activation of the chain in shared memory
-// (see kernels.h: X / D / E); the batch x streams dimension provides the parallelism (one frame per SM at a time).
+// (see kernels.h: X / D / E); the batch x streams dimension provides the parallelism.  For the Meet geometries the
+// expanded tensor goes through E 16 channels at a time, which brings the CTA under half an SM's shared memory and
+// registers: two frames share an SM and cover each other's barrier and L2 waits.  MLKit (16x16) cannot fit two at any
+// slice width and keeps 32-channel slices, one frame per SM.
 //
 // Arithmetic contract: identical to the stand-alone kernels (kernels_nn.cu) and therefore to the oracle —
 // every output accumulates fmaf in ascending k / (fy, fx) order, the pool sums each row left to right and then the
 // rows top to bottom, the SE scale multiplies the operand (one rounding) before the fmaf.
 #include <algorithm>
+#include <mutex>
 
 #include "kernels.h"
 
@@ -20,27 +24,32 @@ void count_launch();
 
 namespace {
 
-constexpr int CH_T = 512;            // threads per CTA
+constexpr int CH_T = 512;            // threads per CTA of the one-frame-per-SM instantiation
+constexpr int CH_T2 = 384;           // threads per CTA of the two-frames-per-SM instantiation
 constexpr int CH_XLD = 32;           // X row stride (floats): block inputs / outputs have <= 32 channels
 constexpr int CH_DLD = 128;          // D row stride: expanded tensors have <= 128 channels
-constexpr int CH_ELD = 32;           // E slice width
 
 constexpr int CH_PAD = 2;            // zero halo of the E slice (covers 3x3 and 5x5 stride-1 windows)
+// pixel row stride of the haloed E grid.  With 16-channel slices a warp reads two pixel rows at once (one per
+// half-warp); an odd stride puts them 16 banks apart.  With 32-channel slices a warp reads one pixel, any stride is free.
+BSB_HD int chain_estride(int w, int eld) { return eld < 32 ? (w + 2 * CH_PAD) | 1 : w + 2 * CH_PAD; }
 struct ChainLayout { int off_x, off_d, off_e, e_floats, off_w1, off_wd, off_vec, total; };   // float offsets
-BSB_HD ChainLayout chain_layout(int h, int w) {
+// eld: E slice width (16 or 32 channels)
+BSB_HD ChainLayout chain_layout(int h, int w, int eld) {
+  // the fixed-size pieces first: their addresses are compile-time constants in the kernel and cost no registers
   ChainLayout L;
   const int P = h * w;
-  L.off_x = 0;
+  L.off_vec = 0;                                  // v0 | v1 | sv
+  L.off_wd = L.off_vec + 3 * 128;                 // depthwise taps of one slice [k*k <= 25][eld]
+  L.off_w1 = L.off_wd + 25 * eld;                 // expand weights of one slice [cin <= 32][eld]
+  L.off_x = L.off_w1 + 32 * eld;
   L.off_d = L.off_x + P * CH_XLD;
   L.off_e = L.off_d + P * CH_DLD;                 // zero-haloed E slice; PW / FC weight staging and the pool row sums alias it
-  int e_floats = (h + 2 * CH_PAD) * (w + 2 * CH_PAD) * CH_ELD;
-  if (e_floats < 4096) e_floats = 4096;
+  int e_floats = (h + 2 * CH_PAD) * chain_estride(w, eld) * eld;
+  if (e_floats < 4096) e_floats = 4096;           // PW staging: K * n4 <= 4096 (Engine::detect_chain)
   if (e_floats < h * CH_DLD) e_floats = h * CH_DLD;
   L.e_floats = e_floats;
-  L.off_w1 = L.off_e + e_floats;
-  L.off_wd = L.off_w1 + 32 * 32;                  // expand weights of one slice [cin <= 32][32]
-  L.off_vec = L.off_wd + 25 * 32;                 // depthwise taps of one slice [k*k <= 25][32]
-  L.total = L.off_vec + 3 * 128;                  // v0 | v1 | sv
+  L.total = L.off_e + e_floats;
   return L;
 }
 
@@ -49,11 +58,11 @@ BSB_D float chain_act2(float v, int a1, int a2) { return bsb_act(bsb_act(v, a1),
 // dst[p][n] = act(sum_k A[p][k] (* sv[k]) * Ws[k][n] + bias) (+ residual), R rows x 4 columns per thread, k ascending.
 // A: shared [P][lda]; Ws: shared [K][n4] (zero padded); dst: shared, row p at dst + drow(p) * ldd (may be the residual
 // source: each element is read and then written by the same thread).  pw > 0: dst is the zero-haloed E slice
-// (row p = pixel (p / pw, p % pw) of a (h + 4) x (pw + 4) grid).  ACT2 >= 0 fixes the second activation at compile time
-// (the first one must then be ACT_NONE); ACT2 < 0 is the generic path.
+// (row p = pixel (p / pw, p % pw) of a (h + 4) x (pw + 4) grid of row stride es).  ACT2 >= 0 fixes the second
+// activation at compile time (the first one must then be ACT_NONE); ACT2 < 0 is the generic path.
 template <int R, int ACT2>
 BSB_D void chain_gemm_t(const float* A, int lda, int K, const float* sv, const float* Ws, int n4, int N, const float* bias,
-                        int a1, int a2, bool residual, int a3, float* dst, int ldd, int P, int pw) {
+                        int a1, int a2, bool residual, int a3, float* dst, int ldd, int P, int pw, int es) {
   const int cg = n4 / 4, rg = (P + R - 1) / R;
   for (int t = threadIdx.x; t < cg * rg; t += blockDim.x) {
     const int tx = t % cg, ty = t / cg;
@@ -91,7 +100,7 @@ BSB_D void chain_gemm_t(const float* A, int lda, int K, const float* sv, const f
     for (int i = 0; i < R; ++i) {
       const int p = p0 + i;
       if (p >= P) break;
-      const int drow = pw > 0 ? ((p / pw + CH_PAD) * (pw + 2 * CH_PAD) + (p % pw) + CH_PAD) : p;
+      const int drow = pw > 0 ? ((p / pw + CH_PAD) * es + (p % pw) + CH_PAD) : p;
       float* dp = dst + (size_t)drow * ldd + n0;
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
@@ -107,13 +116,13 @@ BSB_D void chain_gemm_t(const float* A, int lda, int K, const float* sv, const f
 
 template <int R>
 BSB_D void chain_gemm(const float* A, int lda, int K, const float* sv, const float* Ws, int n4, int N, const float* bias,
-                      int a1, int a2, bool residual, int a3, float* dst, int ldd, int P, int pw) {
+                      int a1, int a2, bool residual, int a3, float* dst, int ldd, int P, int pw, int es) {
   // the activation combinations of the MobileNetV3-style graphs get their own instantiation (no per-element switch)
-  if (a1 == ACT_NONE && a2 == ACT_NONE) chain_gemm_t<R, ACT_NONE>(A, lda, K, sv, Ws, n4, N, bias, a1, a2, residual, a3, dst, ldd, P, pw);
-  else if (a1 == ACT_NONE && a2 == ACT_HARD_SWISH) chain_gemm_t<R, ACT_HARD_SWISH>(A, lda, K, sv, Ws, n4, N, bias, a1, a2, residual, a3, dst, ldd, P, pw);
-  else if (a1 == ACT_NONE && a2 == ACT_RELU6) chain_gemm_t<R, ACT_RELU6>(A, lda, K, sv, Ws, n4, N, bias, a1, a2, residual, a3, dst, ldd, P, pw);
-  else if (a1 == ACT_NONE && a2 == ACT_RELU) chain_gemm_t<R, ACT_RELU>(A, lda, K, sv, Ws, n4, N, bias, a1, a2, residual, a3, dst, ldd, P, pw);
-  else chain_gemm_t<R, -1>(A, lda, K, sv, Ws, n4, N, bias, a1, a2, residual, a3, dst, ldd, P, pw);
+  if (a1 == ACT_NONE && a2 == ACT_NONE) chain_gemm_t<R, ACT_NONE>(A, lda, K, sv, Ws, n4, N, bias, a1, a2, residual, a3, dst, ldd, P, pw, es);
+  else if (a1 == ACT_NONE && a2 == ACT_HARD_SWISH) chain_gemm_t<R, ACT_HARD_SWISH>(A, lda, K, sv, Ws, n4, N, bias, a1, a2, residual, a3, dst, ldd, P, pw, es);
+  else if (a1 == ACT_NONE && a2 == ACT_RELU6) chain_gemm_t<R, ACT_RELU6>(A, lda, K, sv, Ws, n4, N, bias, a1, a2, residual, a3, dst, ldd, P, pw, es);
+  else if (a1 == ACT_NONE && a2 == ACT_RELU) chain_gemm_t<R, ACT_RELU>(A, lda, K, sv, Ws, n4, N, bias, a1, a2, residual, a3, dst, ldd, P, pw, es);
+  else chain_gemm_t<R, -1>(A, lda, K, sv, Ws, n4, N, bias, a1, a2, residual, a3, dst, ldd, P, pw, es);
 }
 
 // global [K][n4] -> shared, all loads in flight
@@ -139,34 +148,38 @@ BSB_D void chain_fc(const float* in, const FcLayer& f, float* out, float* stage,
   if (n < f.N) out[n] = chain_act2(acc + (f.bias ? __ldg(f.bias + n) : 0.f), f.act1, f.act2);
 }
 
-// depthwise KS x KS, stride 1, SAME, of one 32-channel slice: E (zero-haloed (h+4) x (w+4) grid of [32]) -> D[:, c0 : c0 + cw].
-// A lane keeps its channel, so its KS*KS taps live in registers; a thread produces 4 consecutive pixels of a row from
-// KS x (KS + 3) loads.  Out-of-image taps read the halo's zeros: fmaf(+0, w, acc) leaves acc unchanged bit for bit (an
-// accumulator that starts at +0 can never become -0 by adding zeros), so skipping them as the oracle does gives the same bits.
-template <int KS, int ACT2>
-BSB_D void chain_dw_slice_t(const float* E, const float* wds, const ChainOp& op, int c0, int cw, int h, int w, float* D) {
-  const int j = threadIdx.x & 31;
+// depthwise KS x KS, stride 1, SAME, of one ELD-channel slice: E (zero-haloed (h+4) x (w+4) grid of [ELD], row stride
+// chain_estride) -> D[:, c0 : c0 + cw].  A lane keeps its channel, so its KS*KS taps live in registers; a thread produces
+// 4 consecutive pixels of a row from KS x (KS + 3) loads.  With 16-channel slices the two half-warps take the same strip
+// of two consecutive rows (an odd row stride apart: no bank conflict).  Out-of-image taps read the halo's zeros:
+// fmaf(+0, w, acc) leaves acc unchanged bit for bit (an accumulator that starts at +0 can never become -0 by adding
+// zeros), so skipping them as the oracle does gives the same bits.
+template <int KS, int ACT2, int ELD>
+BSB_D void chain_dw_slice_t(const float* E, const float* wds, const ChainOp& op, int c0, int cw, int h, int w, int es, float* D) {
+  constexpr int ROWS = 32 / ELD;                  // output rows per warp
+  const int j = threadIdx.x % ELD, half = (threadIdx.x & 31) / ELD;
   if (j >= cw) return;
   float wr[KS * KS];
 #pragma unroll
-  for (int t = 0; t < KS * KS; ++t) wr[t] = wds[t * 32 + j];
+  for (int t = 0; t < KS * KS; ++t) wr[t] = wds[t * ELD + j];
   const float bias = op.bd ? __ldg(op.bd + c0 + j) : 0.f;
-  const int ew = w + 2 * CH_PAD, strips = (w + 3) / 4;
+  const int ew = w + 2 * CH_PAD, strips = (w + 3) / 4, row_groups = (h + ROWS - 1) / ROWS;
   const bool full = (w & 3) == 0;                 // every strip has 4 pixels and its KS + 3 columns lie inside the haloed grid
-  for (int sidx = threadIdx.x >> 5; sidx < h * strips; sidx += blockDim.x >> 5) {
-    const int oy = sidx / strips, ox0 = (sidx - oy * strips) * 4;
+  for (int sidx = threadIdx.x >> 5; sidx < row_groups * strips; sidx += blockDim.x >> 5) {
+    const int ry = sidx / strips, oy = ry * ROWS + half, ox0 = (sidx - ry * strips) * 4;
+    if (oy >= h) continue;
     float acc[4] = {0.f, 0.f, 0.f, 0.f};
     // window origin in the haloed grid: (oy - pt + CH_PAD, ox0 - pl + CH_PAD); pt, pl <= CH_PAD
-    const float* e0 = E + ((size_t)(oy - op.pt + CH_PAD) * ew + (ox0 - op.pl + CH_PAD)) * CH_ELD + j;
+    const float* e0 = E + ((size_t)(oy - op.pt + CH_PAD) * es + (ox0 - op.pl + CH_PAD)) * ELD + j;
 #pragma unroll
     for (int fy = 0; fy < KS; ++fy) {
       float v[KS + 3];
       if (full) {
 #pragma unroll
-        for (int c = 0; c < KS + 3; ++c) v[c] = e0[((size_t)fy * ew + c) * CH_ELD];
+        for (int c = 0; c < KS + 3; ++c) v[c] = e0[((size_t)fy * es + c) * ELD];
       } else {
 #pragma unroll
-        for (int c = 0; c < KS + 3; ++c) v[c] = (ox0 - op.pl + CH_PAD + c < ew) ? e0[((size_t)fy * ew + c) * CH_ELD] : 0.f;
+        for (int c = 0; c < KS + 3; ++c) v[c] = (ox0 - op.pl + CH_PAD + c < ew) ? e0[((size_t)fy * es + c) * ELD] : 0.f;
       }
 #pragma unroll
       for (int q = 0; q < 4; ++q)
@@ -182,26 +195,26 @@ BSB_D void chain_dw_slice_t(const float* E, const float* wds, const ChainOp& op,
   }
 }
 
-// depthwise KS x KS, stride 1, SAME, of one 32-channel slice: E (zero-haloed (h+4) x (w+4) grid of [32]) -> D[:, c0 : c0 + cw].
-// A lane keeps its channel, so its KS*KS taps live in registers; a thread produces 4 consecutive pixels of a row from
-// KS x (KS + 3) loads.  Out-of-image taps read the halo's zeros: fmaf(+0, w, acc) leaves acc unchanged bit for bit (an
-// accumulator that starts at +0 can never become -0 by adding zeros), so skipping them as the oracle does gives the same bits.
-template <int KS>
-BSB_D void chain_dw_slice(const float* E, const float* wds, const ChainOp& op, int c0, int cw, int h, int w, float* D) {
-  if (op.dact1 == ACT_NONE && op.dact2 == ACT_HARD_SWISH) chain_dw_slice_t<KS, ACT_HARD_SWISH>(E, wds, op, c0, cw, h, w, D);
-  else if (op.dact1 == ACT_NONE && op.dact2 == ACT_RELU6) chain_dw_slice_t<KS, ACT_RELU6>(E, wds, op, c0, cw, h, w, D);
-  else if (op.dact1 == ACT_NONE && op.dact2 == ACT_RELU) chain_dw_slice_t<KS, ACT_RELU>(E, wds, op, c0, cw, h, w, D);
-  else chain_dw_slice_t<KS, -1>(E, wds, op, c0, cw, h, w, D);
+template <int KS, int ELD>
+BSB_D void chain_dw_slice(const float* E, const float* wds, const ChainOp& op, int c0, int cw, int h, int w, int es, float* D) {
+  if (op.dact1 == ACT_NONE && op.dact2 == ACT_HARD_SWISH) chain_dw_slice_t<KS, ACT_HARD_SWISH, ELD>(E, wds, op, c0, cw, h, w, es, D);
+  else if (op.dact1 == ACT_NONE && op.dact2 == ACT_RELU6) chain_dw_slice_t<KS, ACT_RELU6, ELD>(E, wds, op, c0, cw, h, w, es, D);
+  else if (op.dact1 == ACT_NONE && op.dact2 == ACT_RELU) chain_dw_slice_t<KS, ACT_RELU, ELD>(E, wds, op, c0, cw, h, w, es, D);
+  else chain_dw_slice_t<KS, -1, ELD>(E, wds, op, c0, cw, h, w, es, D);
 }
 
 }  // namespace
 
-template <int R>
-__global__ void __launch_bounds__(CH_T, 1) k_chain(const ChainOp* ops, int n_ops, int h, int w) {
+// R: rows per thread tile of the GEMMs; ELD: E slice width; NT, MIN_CTAS: threads per CTA and CTAs per SM.
+// es = chain_estride(w, ELD) comes in as a parameter: read from the constant bank, it costs no register.
+template <int R, int ELD, int NT, int MIN_CTAS>
+__global__ void __launch_bounds__(NT, MIN_CTAS) k_chain(const ChainOp* ops, int n_ops, int h, int w, int es) {
+  // expand GEMM into a 16-column slice: (P / 2) x 4 thread tiles (Meet: 288 of the 384 threads)
+  constexpr int RE = ELD == 16 ? 2 : R;
   BSB_DYN_SMEM(smem_raw);
   float* sm = reinterpret_cast<float*>(smem_raw);
   const int P = h * w;
-  const ChainLayout L = chain_layout(h, w);
+  const ChainLayout L = chain_layout(h, w, ELD);
   float* X = sm + L.off_x; float* D = sm + L.off_d; float* E = sm + L.off_e;
   float* w1s = sm + L.off_w1; float* wds = sm + L.off_wd;
   float* v0 = sm + L.off_vec; float* v1 = v0 + 128; float* sv = v1 + 128;
@@ -240,32 +253,32 @@ __global__ void __launch_bounds__(CH_T, 1) k_chain(const ChainOp* ops, int n_ops
         break;
       }
       case CH_EXPAND_DW: {
-        // X [P][cin] -> expand 1x1 (+act) -> depthwise k x k stride 1 (+act) -> D [P][cout], one 32-channel slice at a time
-        // (E was used as scratch by the ops in between: its zero halo is rebuilt first)
+        // X [P][cin] -> expand 1x1 (+act) -> depthwise k x k stride 1 (+act) -> D [P][cout], one ELD-channel slice at a
+        // time (E was used as scratch by the ops in between: its zero halo is rebuilt first)
         {
-          const int ew = w + 2 * CH_PAD, eh = h + 2 * CH_PAD;
-          for (int i = tid; i < eh * ew * (CH_ELD / 4); i += T) {
-            const int cell = i / (CH_ELD / 4), ey = cell / ew, ex = cell - ey * ew;
+          const int eh = h + 2 * CH_PAD;
+          for (int i = tid; i < eh * es * (ELD / 4); i += T) {
+            const int cell = i / (ELD / 4), ey = cell / es, ex = cell - ey * es;
             if (ey < CH_PAD || ey >= h + CH_PAD || ex < CH_PAD || ex >= w + CH_PAD)
-              *reinterpret_cast<float4*>(E + (size_t)cell * CH_ELD + 4 * (i % (CH_ELD / 4))) = make_float4(0.f, 0.f, 0.f, 0.f);
+              *reinterpret_cast<float4*>(E + (size_t)cell * ELD + 4 * (i % (ELD / 4))) = make_float4(0.f, 0.f, 0.f, 0.f);
           }
         }
-        for (int c0 = 0; c0 < op.cout; c0 += 32) {
-          const int cw = min(32, op.cout - c0);
+        for (int c0 = 0; c0 < op.cout; c0 += ELD) {
+          const int cw = min(ELD, op.cout - c0);
           if (c0) __syncthreads();                        // the previous slice's E / w1s / wds are fully consumed
-          for (int i = tid; i < op.cin * 32; i += T) {
-            const int kk = i >> 5, j = i & 31;
+          for (int i = tid; i < op.cin * ELD; i += T) {
+            const int kk = i / ELD, j = i % ELD;
             w1s[i] = j < cw ? __ldg(op.w + (size_t)kk * op.n4 + c0 + j) : 0.f;
           }
-          for (int i = tid; i < op.k * op.k * 32; i += T) {
-            const int tp = i >> 5, j = i & 31;
+          for (int i = tid; i < op.k * op.k * ELD; i += T) {
+            const int tp = i / ELD, j = i % ELD;
             wds[i] = j < cw ? __ldg(op.wd + (size_t)tp * op.cout + c0 + j) : 0.f;
           }
           __syncthreads();
-          chain_gemm<R>(X, CH_XLD, op.cin, nullptr, w1s, 32, cw, op.b ? op.b + c0 : nullptr, op.act1, op.act2, false, 0, E, CH_ELD, P, w);
+          chain_gemm<RE>(X, CH_XLD, op.cin, nullptr, w1s, ELD, cw, op.b ? op.b + c0 : nullptr, op.act1, op.act2, false, 0, E, ELD, P, w, es);
           __syncthreads();
-          if (op.k == 5) chain_dw_slice<5>(E, wds, op, c0, cw, h, w, D);
-          else chain_dw_slice<3>(E, wds, op, c0, cw, h, w, D);
+          if (op.k == 5) chain_dw_slice<5, ELD>(E, wds, op, c0, cw, h, w, es, D);
+          else chain_dw_slice<3, ELD>(E, wds, op, c0, cw, h, w, es, D);
         }
         break;
       }
@@ -303,7 +316,7 @@ __global__ void __launch_bounds__(CH_T, 1) k_chain(const ChainOp* ops, int n_ops
         float* Ws = E;                                    // [K][n4] staging (E is dead outside EXPAND_DW)
         chain_stage(Ws, op.w, op.cin * op.n4);
         __syncthreads();
-        chain_gemm<R>(A, lda, op.cin, op.use_scale ? sv : nullptr, Ws, op.n4, op.cout, op.b, op.act1, op.act2, op.residual != 0, op.act3, dst, ldd, P, 0);
+        chain_gemm<R>(A, lda, op.cin, op.use_scale ? sv : nullptr, Ws, op.n4, op.cout, op.b, op.act1, op.act2, op.residual != 0, op.act3, dst, ldd, P, 0, 0);
         break;
       }
       case CH_SCALE_STORE: {
@@ -323,24 +336,61 @@ __global__ void __launch_bounds__(CH_T, 1) k_chain(const ChainOp* ops, int n_ops
   }
 }
 
+namespace {
+
+// Which instantiation runs a chain over h x w pixels.  The 384-thread one (GEMM tiles of 3 rows: (P / 3) x 8 = 384 tiles
+// for Meet's 9x16) uses 16-channel E slices so that two CTAs fit on one SM; it is chosen when the geometry allows that on
+// the current device (Meet full 9x16: 114 816 B, Meet lite 6x10).  Everything else (MLKit's 16x16: 512 threads, 4-row
+// tiles, 219 KiB) runs one CTA per SM with 32-channel slices.
+struct ChainConfig { bool two_per_sm; size_t smem; };
+
+ChainConfig chain_config(int h, int w) {
+  const int P = h * w;
+  if (P % 3 == 0 && (P / 3) * 8 <= CH_T2) {
+    const size_t bytes = (size_t)chain_layout(h, w, 16).total * sizeof(float);
+    int per_sm = 228 * 1024, reserved = 1024;     // H100
+#ifndef BSB_EMU
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev) != cudaSuccess) {
+      cudaGetLastError();
+      per_sm = 0;
+    }
+#endif
+    if (2 * (bytes + (size_t)reserved) <= (size_t)per_sm) return {true, bytes};
+  }
+  return {false, (size_t)chain_layout(h, w, 32).total * sizeof(float)};
+}
+
+}  // namespace
+
 size_t chain_smem_bytes(int h, int w) {
   const int P = h * w;
   if (P < 1 || P > 256 || h > 64) return 0;
-  const size_t bytes = (size_t)chain_layout(h, w).total * sizeof(float);
+  const size_t bytes = chain_config(h, w).smem;
   return bytes <= 226 * 1024 ? bytes : 0;
 }
 
 void launch_chain(cudaStream_t s, int B, int h, int w, const ChainOp* d_ops, int n_ops) {
-  const size_t smem = chain_smem_bytes(h, w);
-  // threads and row tile so that the narrow GEMMs ((P / R) x 8 thread tiles) fill the CTA exactly once:
-  // 9x16 (Meet): 48 x 8 = 384 tiles of 3 rows; 16x16 (MLKit): 64 x 8 = 512 tiles of 4 rows
-  const int P = h * w;
-  if (P % 3 == 0 && (P / 3) * 8 <= 384) {
-    ensure_dyn_smem(reinterpret_cast<const void*>(k_chain<3>), smem);
-    BSB_LAUNCH(k_chain<3>, dim3((unsigned)B), dim3(384), smem, s, d_ops, n_ops, h, w);
+  const ChainConfig cfg = chain_config(h, w);
+  if (cfg.two_per_sm) {
+    auto k = k_chain<3, 16, CH_T2, 2>;
+    ensure_dyn_smem(reinterpret_cast<const void*>(k), cfg.smem);
+#ifndef BSB_EMU
+    // the whole unified L1 / shared array as shared memory: room for the two CTAs (set once per device)
+    static std::once_flag carveout[64];
+    int dev = 0;
+    if (cudaGetDevice(&dev) == cudaSuccess && dev < 64)
+      std::call_once(carveout[dev], [&] {
+        if (cudaFuncSetAttribute(reinterpret_cast<const void*>(k), cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess)
+          cudaGetLastError();
+      });
+#endif
+    BSB_LAUNCH(k, dim3((unsigned)B), dim3(CH_T2), cfg.smem, s, d_ops, n_ops, h, w, chain_estride(w, 16));
   } else {
-    ensure_dyn_smem(reinterpret_cast<const void*>(k_chain<4>), smem);
-    BSB_LAUNCH(k_chain<4>, dim3((unsigned)B), dim3(CH_T), smem, s, d_ops, n_ops, h, w);
+    auto k = k_chain<4, 32, CH_T, 1>;
+    ensure_dyn_smem(reinterpret_cast<const void*>(k), cfg.smem);
+    BSB_LAUNCH(k, dim3((unsigned)B), dim3(CH_T), cfg.smem, s, d_ops, n_ops, h, w, chain_estride(w, 32));
   }
   count_launch();
 }
