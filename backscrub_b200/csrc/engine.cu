@@ -445,6 +445,8 @@ bool Engine::plan(std::string* err) {
   if (tuning().head && !(flags_ & (1u | 8u))) detect_heads();
   // ---- encoder entry (16 -> 16 1x1 -> depthwise 3x3 stride 2) as one kernel ----
   if (tuning().pw_dws2 && !tuning().stem_pw && !(flags_ & (1u | 8u))) detect_pw_dws2();
+  // ---- the two inverted-residual blocks between the encoder entry and the chain as two kernels ----
+  if (!(flags_ & (1u | 8u))) detect_enc_blocks();
   find_segments();
   dec_up_step_ = -1;
   if (tuning().dec_up && model_type_ == MODEL_DEEPLAB && !(flags_ & 1u) && !steps_.empty()) {
@@ -460,11 +462,14 @@ bool Engine::plan(std::string* err) {
   for (int s = 0; s < ns; ++s) {
     const Step& st = steps_[s];
     use(st.in, s); use(st.in2, s); use(st.scale, s); use(st.in_add, s); use(st.residual, s);
-    tinfo_[st.out].materialized = true;
-    const int r = root(st.out);
-    tinfo_[r].materialized = true;
-    tinfo_[r].first_def = std::min(tinfo_[r].first_def, s);
-    use(st.out, s);
+    for (int o : {st.out, st.out2}) {
+      if (o < 0) continue;
+      tinfo_[o].materialized = true;
+      const int r = root(o);
+      tinfo_[r].materialized = true;
+      tinfo_[r].first_def = std::min(tinfo_[r].first_def, s);
+      use(o, s);
+    }
   }
   // a sub-batched segment runs its steps once per frame group: every tensor it touches must stay allocated from the
   // segment's first step to its last (a buffer recycled inside the segment would be overwritten by group g while group
@@ -474,7 +479,7 @@ bool Engine::plan(std::string* err) {
     const int s1 = s0 + seg_len_[s0] - 1;
     for (int s = s0; s <= s1; ++s) {
       const Step& st = steps_[s];
-      for (int t : {st.in, st.in2, st.scale, st.in_add, st.residual, st.up_from, st.out}) {
+      for (int t : {st.in, st.in2, st.scale, st.in_add, st.residual, st.up_from, st.out, st.out2}) {
         if (t < 0) continue;
         const int r = root(t);
         tinfo_[r].last_use = std::max(tinfo_[r].last_use, s1);
@@ -515,8 +520,11 @@ bool Engine::plan(std::string* err) {
   std::vector<char> allocated(nt, 0);
   tinfo_[g_.input].offset = alloc(tinfo_[g_.input].frame_elems * max_batch_); allocated[g_.input] = 1;
   for (int s = 0; s < ns; ++s) {
-    const int o = root(steps_[s].out);
-    if (!allocated[o]) { tinfo_[o].offset = alloc(tinfo_[o].frame_elems * max_batch_); allocated[o] = 1; }
+    for (int t : {steps_[s].out, steps_[s].out2}) {
+      if (t < 0) continue;
+      const int o = root(t);
+      if (!allocated[o]) { tinfo_[o].offset = alloc(tinfo_[o].frame_elems * max_batch_); allocated[o] = 1; }
+    }
     if (keep) continue;
     for (int t = 0; t < nt; ++t)
       if (allocated[t] == 1 && tinfo_[t].alias_parent < 0 && tinfo_[t].materialized && tinfo_[t].last_use == s) {
@@ -598,6 +606,63 @@ void Engine::detect_pw_dws2() {
     tinfo_[P.out].materialized = false;
     steps_.erase(steps_.begin() + i, steps_.begin() + i + 2);
     steps_.insert(steps_.begin() + i, h);
+  }
+}
+
+// Find   PW(scaled, no act) -> PW(expand, act) -> DW 3x3 s2 (act) -> PW(project)                    = block A
+//        -> PW(expand, act) -> DW 3x3 s1 (act) -> PW(project + residual of A's output) -> PW(hswish) = block B
+// with act RELU6 or RELU throughout, the channel counts the kernels are compiled for, and the four expanded tensors
+// read only inside the run; replace the eight steps by ENC_A (outputs: the project, and the scaled 1x1 as out2) and
+// ENC_B (outputs: the hswish 1x1, and the residual sum as out2).  Same arithmetic per output element.
+void Engine::detect_enc_blocks() {
+  auto reads = [&](const Step& r, int t) { return r.in == t || r.in2 == t || r.scale == t || r.in_add == t || r.residual == t; };
+  auto one = [](const Step& s, int want) { return (s.act1 == ACT_NONE && s.act2 == want) || (s.act1 == want && s.act2 == ACT_NONE); };
+  auto pw = [&](const Step& s, int in, int act) {
+    return s.kind == Step::PW && s.in == in && !s.use_tc && s.up_from < 0 && s.in_add < 0 && s.n4 == s.N && one(s, act);
+  };
+  auto dw3 = [&](const Step& s, int in, int stride, int act) {
+    return s.kind == Step::DW && s.in == in && s.residual < 0 && s.kh == 3 && s.kw == 3 && s.sh == stride && s.sw == stride &&
+           s.dh == 1 && s.dw == 1 && one(s, act) && tinfo_[s.out].c == tinfo_[in].c;
+  };
+  for (size_t i = 0; i + 8 <= steps_.size(); ++i) {
+    const Step* s = &steps_[i];
+    const int act = s[1].act1 != ACT_NONE ? s[1].act1 : s[1].act2;
+    if (act != ACT_RELU6 && act != ACT_RELU) continue;
+    if (!(pw(s[0], s[0].in, ACT_NONE) && s[0].scale >= 0 && s[0].residual < 0 &&
+          pw(s[1], s[0].out, act) && s[1].scale < 0 && s[1].residual < 0 &&
+          dw3(s[2], s[1].out, 2, act) &&
+          pw(s[3], s[2].out, ACT_NONE) && s[3].scale < 0 && s[3].residual < 0 &&
+          pw(s[4], s[3].out, act) && s[4].scale < 0 && s[4].residual < 0 &&
+          dw3(s[5], s[4].out, 1, act) &&
+          pw(s[6], s[5].out, ACT_NONE) && s[6].scale < 0 && s[6].residual == s[3].out && s[6].act3 == ACT_NONE &&
+          pw(s[7], s[6].out, ACT_HARD_SWISH) && s[7].scale < 0 && s[7].residual < 0))
+      continue;
+    const TensorInfo& X = tinfo_[s[0].in]; const TensorInfo& T25 = tinfo_[s[0].out]; const TensorInfo& T36 = tinfo_[s[3].out];
+    const TensorInfo& T48 = tinfo_[s[6].out]; const TensorInfo& T52 = tinfo_[s[7].out];
+    // SAME padding of the stride-2 depthwise: its window of the 1x1 output covers every pixel a tile owns
+    if (s[2].pt > 1 || s[2].pl > 1 || T36.h != (T25.h + 1) / 2 || T36.w != (T25.w + 1) / 2 || s[5].pt != 1 || s[5].pl != 1) continue;
+    if (T25.h != X.h || T25.w != X.w || T48.h != T36.h || T48.w != T36.w || T52.h != T36.h || T52.w != T36.w) continue;
+    if (!enc_blocks_supported(device_, X.c, s[0].N, s[1].N, s[3].N, s[4].N, s[7].N, X.ld, T25.ld, T36.ld, T48.ld, T52.ld) ||
+        s[0].K != X.c || s[6].N != s[3].N)
+      continue;
+    // the expanded tensors are private to the run; the four outputs are materialised
+    bool contained = true;
+    for (int k : {1, 2, 4, 5}) {
+      if (s[k].out == g_.output) contained = false;
+      for (size_t r = 0; r < steps_.size() && contained; ++r)
+        if ((r < i || r >= i + 8 || (int)(r - i) != k + 1) && reads(steps_[r], s[k].out)) contained = false;
+    }
+    if (!contained) continue;
+    EncPlan ep; ep.act = act;
+    for (int k = 0; k < 8; ++k) ep.s[k] = s[k];
+    Step a; a.kind = Step::ENC_A; a.op_index = s[0].op_index; a.in = s[0].in; a.scale = s[0].scale; a.out = s[3].out; a.out2 = s[0].out;
+    Step b; b.kind = Step::ENC_B; b.op_index = s[4].op_index; b.in = s[3].out; b.out = s[7].out; b.out2 = s[6].out;
+    a.block = b.block = (int)encs_.size();
+    encs_.push_back(ep);
+    for (int k : {1, 2, 4, 5}) tinfo_[s[k].out].materialized = false;
+    steps_.erase(steps_.begin() + i, steps_.begin() + i + 8);
+    steps_.insert(steps_.begin() + i, {a, b});
+    ++i;
   }
 }
 
@@ -1054,6 +1119,24 @@ void Engine::run_step(size_t si, int n, bool from_u8, bool* first_p, bool* skip_
                     wblob_ + D.w_off, D.has_bias ? wblob_ + D.b_off : nullptr, D.act1, D.act2, D.act3,
                     hp.has_t ? wblob_ + T.w_off : nullptr, hp.has_t ? wblob_ + T.b_off : nullptr, hp.has_t ? T.N : 0, hp.has_t ? T.act2 : 0,
                     tptr(st.out), O.ld, n, I.h, I.w, D.pt, D.pl);
+        break;
+      }
+      case Step::ENC_A:
+      case Step::ENC_B: {
+        const EncPlan& ep = encs_[st.block];
+        const Step* s = ep.s;
+        EncBlocksArgs a{};
+        a.x = tptr(s[0].in); a.ld_x = tinfo_[s[0].in].ld; a.sv = tptr(s[0].scale);
+        for (int k = 0, pwk = 0; k < 8; ++k) {
+          if (s[k].kind != Step::PW) continue;
+          a.w[pwk] = wblob_ + s[k].w_off; a.b[pwk] = s[k].has_bias ? wblob_ + s[k].b_off : nullptr; ++pwk;
+        }
+        for (int d = 0; d < 2; ++d) { const Step& D = s[d ? 5 : 2]; a.wd[d] = wblob_ + D.w_off; a.bd[d] = D.has_bias ? wblob_ + D.b_off : nullptr; }
+        a.t25 = tptr(s[0].out); a.ld25 = tinfo_[s[0].out].ld; a.t36 = tptr(s[3].out); a.ld36 = tinfo_[s[3].out].ld;
+        a.t48 = tptr(s[6].out); a.ld48 = tinfo_[s[6].out].ld; a.t52 = tptr(s[7].out); a.ld52 = tinfo_[s[7].out].ld;
+        a.ih = tinfo_[s[0].out].h; a.iw = tinfo_[s[0].out].w; a.oh = tinfo_[s[3].out].h; a.ow = tinfo_[s[3].out].w;
+        a.pt_a = s[2].pt; a.pl_a = s[2].pl; a.act = ep.act;
+        launch_enc_blocks(stream_, n, a, st.kind == Step::ENC_B);
         break;
       }
       case Step::CHAIN: {

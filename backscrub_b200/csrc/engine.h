@@ -30,10 +30,12 @@ struct TensorInfo {
 };
 
 struct Step {
-  enum Kind { CONV, PW, DW, POOL, RESIZE, TCONV, ELT, COPY, BLOCK, CHAIN, HEAD } kind = ELT;
-  int block = -1;             // BLOCK: index into Engine::blocks_ (the four fused sub-steps); CHAIN: index into Engine::chains_
+  enum Kind { CONV, PW, DW, POOL, RESIZE, TCONV, ELT, COPY, BLOCK, CHAIN, HEAD, ENC_A, ENC_B } kind = ELT;
+  int block = -1;             // BLOCK: index into Engine::blocks_ (the four fused sub-steps); CHAIN: index into Engine::chains_;
+                              // ENC_A / ENC_B: index into Engine::encs_
   int op_index = -1;
   int in = -1, in2 = -1, out = -1, scale = -1, in_add = -1, residual = -1;
+  int out2 = -1;               // ENC_A / ENC_B: the block's second output (a decoder skip)
   size_t w_off = 0, b_off = 0; bool has_bias = false;
   int act1 = 0, act2 = 0, act3 = 0;
   int K = 0, N = 0, n4 = 0;
@@ -219,6 +221,11 @@ class Engine {
   std::vector<HeadPlan> heads_;
   void detect_heads();
   void detect_pw_dws2();
+  // the two inverted-residual blocks between the encoder entry and the chain (kernels_nn.cu, k_enc_block_s2 / _res):
+  // the eight original steps (scaled 1x1, expand, depthwise s2, project | expand, depthwise, project + residual, expand)
+  struct EncPlan { Step s[8]; int act = 0; };
+  std::vector<EncPlan> encs_;
+  void detect_enc_blocks();
   std::vector<float> wblob_h_;
   size_t arena_elems_ = 0;
   bool tc_enabled_ = false, uses_tc_ = false;   // tensor-core 1x1 convs allowed / actually planned for at least one layer

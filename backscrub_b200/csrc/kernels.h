@@ -136,6 +136,22 @@ void launch_head(cudaStream_t s, int C, const float* x, int ld_x, const float* s
                  const float* wp, const float* bp, int actp1, int actp2, const float* wd, const float* bd, int actd1, int actd2, int actr,
                  const float* wt, const float* bt, int oc, int actt, float* out, int ld_out, int B, int h, int w, int pt, int pl);
 
+// The two MobileNetV3 inverted-residual blocks between the encoder entry and the chain (Meet / MLKit), as two kernels;
+// the expanded tensors are never materialised.  Same arithmetic per output as the stand-alone kernels.
+//   A: t25 = (x * sv) . W0 + b0;  t36 = act(dw3x3 s2 (act(t25 . W1 + b1)) + bd) . W2 + b2          (16 -> 72 -> 24)
+//   B: t48 = act(dw3x3 (act(t36 . W3 + b3)) + bd) . W4 + b4 + t36;  t52 = hswish(t48 . W5 + b5)      (24 -> 88 -> 24 -> 96)
+// act = RELU6 or RELU (the expand and the depthwise of both blocks); the weights are [K][N] with N a multiple of 4.
+struct EncBlocksArgs {
+  const float* x; int ld_x; const float* sv;                 // [B][ih][iw][ld_x] (16 channels), SE scale [B][16]
+  const float* w[6]; const float* b[6];                       // 1x1 convs W0, W1, W2, W3, W4, W5 (b: null -> 0)
+  const float* wd[2]; const float* bd[2];                     // depthwise [3][3][C] of block A, block B
+  float* t25; int ld25; float* t36; int ld36; float* t48; int ld48; float* t52; int ld52;
+  int ih, iw, oh, ow, pt_a, pl_a, act;                        // act: ACT_RELU6 or ACT_RELU
+};
+// the channel counts (16, 16, 72, 24, 88, 96) the kernels are compiled for, the strides, and the shared memory of this device
+bool enc_blocks_supported(int device, int c_in, int c_25, int c_e1, int c_36, int c_e2, int c_52, int ld_x, int ld25, int ld36, int ld48, int ld52);
+void launch_enc_blocks(cudaStream_t s, int B, const EncBlocksArgs& a, bool block_b);
+
 // Convolution2DTransposeBias k2x2 s2 (lib/transpose_conv_bias.cc:37-114).  w: OHWI [oc][2][2][ic].
 void launch_tconv2x2(cudaStream_t s, int B, const float* in, int ih, int iw, int ic, int ld_in,
                      const float* w, const float* bias, int oc, float* out, int oh, int ow, int ld_out, int act2);

@@ -1905,6 +1905,321 @@ void launch_head(cudaStream_t s, int C, const float* x, int ld_x, const float* s
 }
 
 // ---------------------------------------------------------------------------
+// The two inverted-residual blocks between the encoder entry and the chain of the Meet / MLKit graphs, one kernel each
+// (kernels.h, EncBlocksArgs).  One CTA = a 4 x 16 tile of the block's output; everything it needs from the block's
+// input window is recomputed in shared memory, so the expanded tensors (t29 .. t44, 72 / 88 channels) never reach
+// global memory.  Pixels shared with neighbouring tiles are computed twice; each value is still the one chain of the
+// stand-alone kernels (1x1: fmaf over k ascending from +0, operand scaled first, bias last, then the activation, then
+// the residual; depthwise: taps in (fy, fx) order, out-of-image taps skipped, bias last).
+//   A (k_enc_block_s2): window (2 TH + 1) x (2 TW + 1) of the input; t25 on the window (written to global only for
+//     the pixels this tile owns, so each t25 pixel has one writer), then the 72 expanded channels in slices of 24:
+//     expand -> stride-2 depthwise -> project, the project's accumulators persisting across the slices.
+//   B (k_enc_block_res): window (TH + 2) x (TW + 2) of t36; expand all 88 channels -> depthwise -> project + t36
+//     (from the window centre) = t48, then t52 = hswish(t48 . W5 + b5) from the tile's t48 in shared memory.
+// Thread maps: the lanes of a warp take consecutive pixels and one channel group, so every weight read is a broadcast;
+// the pixel-major buffers read by pixel have an odd stride and the depthwise results are stored channel-major [c][64],
+// so those reads are free of bank conflicts.  Projects: thread = tile pixel (tid % 64) x 6 of the 24 output channels.
+// ---------------------------------------------------------------------------
+constexpr int EB_TH = 4, EB_TW = 16, EB_NP = EB_TH * EB_TW;
+constexpr int EB_C0 = 16, EB_E1 = 72, EB_C1 = 24, EB_E2 = 88, EB_C2 = 96;
+constexpr int eb_r4(int x) { return (x + 3) / 4 * 4; }
+// A: shared memory in floats (every region starts on 16 bytes)
+constexpr int EA_WH = 2 * EB_TH + 1, EA_WW = 2 * EB_TW + 1, EA_WP = EA_WH * EA_WW, EA_S = 24, EA_Q = 12;
+constexpr int EA_P25 = EB_C0 + 1, EA_PE = EA_S + 4;                       // pixel strides of t25 (odd), of the slice
+constexpr int EA_W0 = 0, EA_B0 = EA_W0 + EB_C0 * EB_C0, EA_SV = EA_B0 + EB_C0, EA_W1 = EA_SV + EB_C0, EA_B1 = EA_W1 + EB_C0 * EB_E1,
+              EA_WD = EA_B1 + EB_E1, EA_BD = EA_WD + 9 * EB_E1, EA_W2 = EA_BD + EB_E1, EA_B2 = EA_W2 + EB_E1 * EB_C1,
+              EA_T25 = EA_B2 + EB_C1, EA_E = EA_T25 + eb_r4(EA_WP * EA_P25), EA_D = EA_E + EA_WP * EA_PE, EA_END = EA_D + EA_S * EB_NP;
+// B
+constexpr int EB_WH = EB_TH + 2, EB_WW = EB_TW + 2, EB_WP = EB_WH * EB_WW, EB_Q = 8;
+constexpr int EB_PX = EB_C1 + 1, EB_PE = EB_E2 + 4;                       // pixel strides of t36 (odd), of the expanded tensor
+constexpr int EB_W3 = 0, EB_B3 = EB_W3 + EB_C1 * EB_E2, EB_WD = EB_B3 + EB_E2, EB_BD = EB_WD + 9 * EB_E2, EB_W4 = EB_BD + EB_E2,
+              EB_B4 = EB_W4 + EB_E2 * EB_C1, EB_W5 = EB_B4 + EB_C1, EB_B5 = EB_W5 + EB_C1 * EB_C2, EB_X = EB_B5 + EB_C2,
+              EB_E = EB_X + eb_r4(EB_WP * EB_PX), EB_D = EB_E + EB_WP * EB_PE, EB_END = EB_D + EB_E2 * EB_NP;
+constexpr size_t EA_SMEM = sizeof(float) * EA_END, EB_SMEM = sizeof(float) * EB_END;
+static_assert(EA_W1 % 4 == 0 && EA_WD % 4 == 0 && EA_W2 % 4 == 0 && EA_E % 4 == 0 && EA_D % 4 == 0, "16-byte rows");
+static_assert(EB_WD % 4 == 0 && EB_W4 % 4 == 0 && EB_W5 % 4 == 0 && EB_E % 4 == 0 && EB_D % 4 == 0, "16-byte rows");
+static_assert(EB_C1 * EB_NP <= EB_WP * EB_PE, "t48 of the tile reuses the expanded tensor's buffer");
+
+BSB_D void eb_copy(float* dst, const float* src, int n) {            // n % 4 == 0, src 16-byte aligned
+  for (int i = threadIdx.x * 4; i < n; i += 256 * 4) *reinterpret_cast<float4*>(dst + i) = __ldg(reinterpret_cast<const float4*>(src + i));
+}
+BSB_D void eb_bias(float* dst, const float* src, int n) {
+  for (int i = threadIdx.x; i < n; i += 256) dst[i] = src ? __ldg(src + i) : 0.f;
+}
+BSB_D void fma4s(float4& acc, float v, const float4& w) {
+  acc.x = fmaf(v, w.x, acc.x); acc.y = fmaf(v, w.y, acc.y); acc.z = fmaf(v, w.z, acc.z); acc.w = fmaf(v, w.w, acc.w);
+}
+template <int ACT> BSB_D float4 bias_act4(const float4& u, const float* b) {
+  return make_float4(bsb_act(u.x + b[0], ACT), bsb_act(u.y + b[1], ACT), bsb_act(u.z + b[2], ACT), bsb_act(u.w + b[3], ACT));
+}
+// act(x . W + b) for N consecutive columns of W ([K][ldw] in shared memory) from x (K values in shared memory)
+template <int K, int N, int ACT>
+BSB_D void eb_expand(const float* x, const float* w, int ldw, const float* b, float* out) {
+  float4 u[N / 4];
+#pragma unroll
+  for (int q = 0; q < N / 4; ++q) u[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    const float v = x[k];
+#pragma unroll
+    for (int q = 0; q < N / 4; ++q) fma4s(u[q], v, *reinterpret_cast<const float4*>(w + k * ldw + 4 * q));
+  }
+#pragma unroll
+  for (int q = 0; q < N / 4; ++q) *reinterpret_cast<float4*>(out + 4 * q) = bias_act4<ACT>(u[q], b + 4 * q);
+}
+// depthwise result of 4 channels of one tile pixel into the channel-major buffer d[c][EB_NP]
+template <int ACT> BSB_D void eb_store_dw(float* d, int pp, const float4& u, const float* b) {
+  const float4 r = bias_act4<ACT>(u, b);
+  d[pp] = r.x; d[EB_NP + pp] = r.y; d[2 * EB_NP + pp] = r.z; d[3 * EB_NP + pp] = r.w;
+}
+// acc[j] += d[k][p] * w[k][j], k ascending, for 6 output channels (w: row stride EB_C1, 8-byte aligned)
+template <int K> BSB_D void eb_project6(const float* d, int p, const float* w, float* acc) {
+#pragma unroll 4
+  for (int k = 0; k < K; ++k) {
+    const float v = d[k * EB_NP + p];
+    const float2 w0 = *reinterpret_cast<const float2*>(w + k * EB_C1), w1 = *reinterpret_cast<const float2*>(w + k * EB_C1 + 2),
+                 w2 = *reinterpret_cast<const float2*>(w + k * EB_C1 + 4);
+    acc[0] = fmaf(v, w0.x, acc[0]); acc[1] = fmaf(v, w0.y, acc[1]); acc[2] = fmaf(v, w1.x, acc[2]);
+    acc[3] = fmaf(v, w1.y, acc[3]); acc[4] = fmaf(v, w2.x, acc[4]); acc[5] = fmaf(v, w2.y, acc[5]);
+  }
+}
+
+template <int ACT>
+__global__ void __launch_bounds__(256, 2) k_enc_block_s2(EncBlocksArgs a) {
+  BSB_DYN_SMEM(smem_raw);
+  float* sm = reinterpret_cast<float*>(smem_raw);
+  float* s25 = sm + EA_T25; float* se = sm + EA_E; float* sd = sm + EA_D;
+  const int tid = threadIdx.x;
+  const int ox0 = blockIdx.x * EB_TW, oy0 = blockIdx.y * EB_TH, b = blockIdx.z;
+  const int ix0 = 2 * ox0 - a.pl_a, iy0 = 2 * oy0 - a.pt_a;          // input pixel of the window's origin
+  eb_copy(sm + EA_W0, a.w[0], EB_C0 * EB_C0); eb_copy(sm + EA_W1, a.w[1], EB_C0 * EB_E1);
+  eb_copy(sm + EA_WD, a.wd[0], 9 * EB_E1); eb_copy(sm + EA_W2, a.w[2], EB_E1 * EB_C1);
+  eb_bias(sm + EA_B0, a.b[0], EB_C0); eb_bias(sm + EA_B1, a.b[1], EB_E1); eb_bias(sm + EA_BD, a.bd[0], EB_E1); eb_bias(sm + EA_B2, a.b[2], EB_C1);
+  if (tid < EB_C0) sm[EA_SV + tid] = __ldg(a.sv + (size_t)b * EB_C0 + tid);
+  __syncthreads();
+  // ---- t25 on the window.  This tile writes the t25 rows [2 TH by, 2 TH (by + 1)) and columns [2 TW bx, 2 TW (bx + 1))
+  // (the last tile row / column: up to the image edge); with SAME padding (pt, pl <= 1, oh = ceil(ih / 2)) they lie in
+  // its window ----
+  const int r0 = 2 * oy0, r1 = blockIdx.y + 1 == gridDim.y ? a.ih : 2 * (oy0 + EB_TH);
+  const int q0 = 2 * ox0, q1 = blockIdx.x + 1 == gridDim.x ? a.iw : 2 * (ox0 + EB_TW);
+  const float* xb = a.x + (size_t)b * a.ih * a.iw * a.ld_x;
+  float* t25b = a.t25 + (size_t)b * a.ih * a.iw * a.ld25;
+  for (int i = tid; i < EA_WP; i += 256) {
+    const int sy = i / EA_WW, sx = i - sy * EA_WW;
+    const int gy = iy0 + sy, gx = ix0 + sx;
+    if (gy < 0 || gy >= a.ih || gx < 0 || gx >= a.iw) continue;          // never read: the depthwise skips out-of-image taps
+    const size_t pix = (size_t)gy * a.iw + gx;
+    float xv[EB_C0];
+#pragma unroll
+    for (int k = 0; k < EB_C0 / 4; ++k) {
+      const float4 t = __ldg(reinterpret_cast<const float4*>(xb + pix * a.ld_x + 4 * k));
+      xv[4 * k] = t.x * sm[EA_SV + 4 * k]; xv[4 * k + 1] = t.y * sm[EA_SV + 4 * k + 1];
+      xv[4 * k + 2] = t.z * sm[EA_SV + 4 * k + 2]; xv[4 * k + 3] = t.w * sm[EA_SV + 4 * k + 3];
+    }
+    float4 acc[EB_C0 / 4];
+#pragma unroll
+    for (int q = 0; q < EB_C0 / 4; ++q) acc[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int k = 0; k < EB_C0; ++k)
+#pragma unroll
+      for (int q = 0; q < EB_C0 / 4; ++q) fma4s(acc[q], xv[k], *reinterpret_cast<const float4*>(sm + EA_W0 + k * EB_C0 + 4 * q));
+    const bool own = gy >= r0 && gy < r1 && gx >= q0 && gx < q1;
+    float* tp = s25 + i * EA_P25;
+#pragma unroll
+    for (int q = 0; q < EB_C0 / 4; ++q) {
+      const float4 r = bias_act4<ACT_NONE>(acc[q], sm + EA_B0 + 4 * q);
+      tp[4 * q] = r.x; tp[4 * q + 1] = r.y; tp[4 * q + 2] = r.z; tp[4 * q + 3] = r.w;
+      if (own) *reinterpret_cast<float4*>(t25b + pix * a.ld25 + 4 * q) = r;
+    }
+  }
+  __syncthreads();
+  const int g = tid / EB_NP, p = tid % EB_NP;                         // project: tile pixel p, output channels 6g .. 6g + 5
+  const int py = oy0 + p / EB_TW, px = ox0 + p % EB_TW;
+  const bool p_ok = py < a.oh && px < a.ow;
+  float acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  for (int s0 = 0; s0 < EB_E1; s0 += EA_S) {
+    // ---- expand: channels s0 .. s0 + 23 on the window, 12 per item ----
+    for (int it = tid; it < EA_WP * (EA_S / EA_Q); it += 256) {
+      const int q = it / EA_WP, i = it - q * EA_WP;
+      const int sy = i / EA_WW, sx = i - sy * EA_WW;
+      const int gy = iy0 + sy, gx = ix0 + sx;
+      if (gy < 0 || gy >= a.ih || gx < 0 || gx >= a.iw) continue;
+      eb_expand<EB_C0, EA_Q, ACT>(s25 + i * EA_P25, sm + EA_W1 + s0 + EA_Q * q, EB_E1, sm + EA_B1 + s0 + EA_Q * q, se + i * EA_PE + EA_Q * q);
+    }
+    __syncthreads();
+    // ---- depthwise 3x3 stride 2 on the tile, 4 channels per item ----
+    for (int it = tid; it < EB_NP * (EA_S / 4); it += 256) {
+      const int q = it / EB_NP, pp = it - q * EB_NP;
+      const int ly = pp / EB_TW, lx = pp % EB_TW;
+      const int oy = oy0 + ly, ox = ox0 + lx;
+      if (oy >= a.oh || ox >= a.ow) continue;
+      float4 u = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+      for (int fy = 0; fy < 3; ++fy) {
+        const int iy = 2 * oy - a.pt_a + fy;
+        if (iy < 0 || iy >= a.ih) continue;
+#pragma unroll
+        for (int fx = 0; fx < 3; ++fx) {
+          const int ix = 2 * ox - a.pl_a + fx;
+          if (ix < 0 || ix >= a.iw) continue;
+          fma4(u, *reinterpret_cast<const float4*>(se + ((2 * ly + fy) * EA_WW + 2 * lx + fx) * EA_PE + 4 * q),
+               *reinterpret_cast<const float4*>(sm + EA_WD + (fy * 3 + fx) * EB_E1 + s0 + 4 * q));
+        }
+      }
+      eb_store_dw<ACT>(sd + 4 * q * EB_NP, pp, u, sm + EA_BD + s0 + 4 * q);
+    }
+    __syncthreads();
+    // ---- project: k ascending across the slices (the next slice's expand only writes the window buffer; the barrier
+    // after it orders this read of sd before the next depthwise) ----
+    if (p_ok) eb_project6<EA_S>(sd, p, sm + EA_W2 + s0 * EB_C1 + 6 * g, acc);
+  }
+  if (!p_ok) return;
+  float* op = a.t36 + (((size_t)b * a.oh + py) * a.ow + px) * a.ld36 + 6 * g;
+#pragma unroll
+  for (int j = 0; j < 6; j += 2)
+    *reinterpret_cast<float2*>(op + j) = make_float2(acc[j] + sm[EA_B2 + 6 * g + j], acc[j + 1] + sm[EA_B2 + 6 * g + j + 1]);
+}
+
+template <int ACT>
+__global__ void __launch_bounds__(256, 2) k_enc_block_res(EncBlocksArgs a) {
+  BSB_DYN_SMEM(smem_raw);
+  float* sm = reinterpret_cast<float*>(smem_raw);
+  float* sx = sm + EB_X; float* se = sm + EB_E; float* sd = sm + EB_D;
+  float* s48 = se;                                                   // the tile's t48 [24][64], once the expanded tensor is consumed
+  const int tid = threadIdx.x;
+  const int h = a.oh, w = a.ow;
+  const int ox0 = blockIdx.x * EB_TW, oy0 = blockIdx.y * EB_TH, b = blockIdx.z;
+  const int ix0 = ox0 - 1, iy0 = oy0 - 1;                            // SAME 3x3: one pixel of halo
+  eb_copy(sm + EB_W3, a.w[3], EB_C1 * EB_E2); eb_copy(sm + EB_WD, a.wd[1], 9 * EB_E2);
+  eb_copy(sm + EB_W4, a.w[4], EB_E2 * EB_C1); eb_copy(sm + EB_W5, a.w[5], EB_C1 * EB_C2);
+  eb_bias(sm + EB_B3, a.b[3], EB_E2); eb_bias(sm + EB_BD, a.bd[1], EB_E2); eb_bias(sm + EB_B4, a.b[4], EB_C1); eb_bias(sm + EB_B5, a.b[5], EB_C2);
+  const float* xb = a.t36 + (size_t)b * h * w * a.ld36;
+  for (int it = tid; it < EB_WP * (EB_C1 / 4); it += 256) {
+    const int i = it / (EB_C1 / 4), q = it - i * (EB_C1 / 4);
+    const int gy = iy0 + i / EB_WW, gx = ix0 + i % EB_WW;
+    if (gy < 0 || gy >= h || gx < 0 || gx >= w) continue;
+    const float4 v = __ldg(reinterpret_cast<const float4*>(xb + ((size_t)gy * w + gx) * a.ld36 + 4 * q));
+    float* xp = sx + i * EB_PX + 4 * q;
+    xp[0] = v.x; xp[1] = v.y; xp[2] = v.z; xp[3] = v.w;
+  }
+  __syncthreads();
+  // ---- expand 24 -> 88 on the window, 8 channels per item ----
+  for (int it = tid; it < EB_WP * (EB_E2 / EB_Q); it += 256) {
+    const int q = it / EB_WP, i = it - q * EB_WP;
+    const int gy = iy0 + i / EB_WW, gx = ix0 + i % EB_WW;
+    if (gy < 0 || gy >= h || gx < 0 || gx >= w) continue;
+    eb_expand<EB_C1, EB_Q, ACT>(sx + i * EB_PX, sm + EB_W3 + EB_Q * q, EB_E2, sm + EB_B3 + EB_Q * q, se + i * EB_PE + EB_Q * q);
+  }
+  __syncthreads();
+  // ---- depthwise 3x3 stride 1 on the tile, 4 channels per item ----
+  for (int it = tid; it < EB_NP * (EB_E2 / 4); it += 256) {
+    const int q = it / EB_NP, pp = it - q * EB_NP;
+    const int ly = pp / EB_TW, lx = pp % EB_TW;
+    const int oy = oy0 + ly, ox = ox0 + lx;
+    if (oy >= h || ox >= w) continue;
+    float4 u = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int fy = 0; fy < 3; ++fy) {
+      const int iy = oy - 1 + fy;
+      if (iy < 0 || iy >= h) continue;
+#pragma unroll
+      for (int fx = 0; fx < 3; ++fx) {
+        const int ix = ox - 1 + fx;
+        if (ix < 0 || ix >= w) continue;
+        fma4(u, *reinterpret_cast<const float4*>(se + ((ly + fy) * EB_WW + lx + fx) * EB_PE + 4 * q),
+             *reinterpret_cast<const float4*>(sm + EB_WD + (fy * 3 + fx) * EB_E2 + 4 * q));
+      }
+    }
+    eb_store_dw<ACT>(sd + 4 * q * EB_NP, pp, u, sm + EB_BD + 4 * q);
+  }
+  __syncthreads();
+  // ---- project 88 -> 24 + t36 = t48 ----
+  const int g = tid / EB_NP, p = tid % EB_NP;
+  const int ly = p / EB_TW, lx = p % EB_TW;
+  const int py = oy0 + ly, px = ox0 + lx;
+  const bool p_ok = py < h && px < w;
+  const size_t pix = ((size_t)b * h + py) * w + px;
+  if (p_ok) {
+    float acc[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+    eb_project6<EB_E2>(sd, p, sm + EB_W4 + 6 * g, acc);
+    const float* res = sx + ((ly + 1) * EB_WW + lx + 1) * EB_PX + 6 * g;
+    float r[6];
+#pragma unroll
+    for (int j = 0; j < 6; ++j) {
+      r[j] = (acc[j] + sm[EB_B4 + 6 * g + j]) + res[j];
+      s48[(6 * g + j) * EB_NP + p] = r[j];
+    }
+    float* op = a.t48 + pix * a.ld48 + 6 * g;
+#pragma unroll
+    for (int j = 0; j < 6; j += 2) *reinterpret_cast<float2*>(op + j) = make_float2(r[j], r[j + 1]);
+  }
+  __syncthreads();
+  // ---- t52 = hswish(t48 . W5 + b5): channels 24g .. 24g + 23 ----
+  if (!p_ok) return;
+  float4 u[6];
+#pragma unroll
+  for (int q = 0; q < 6; ++q) u[q] = make_float4(0.f, 0.f, 0.f, 0.f);
+  const float* wp = sm + EB_W5 + 24 * g;
+#pragma unroll 4
+  for (int k = 0; k < EB_C1; ++k) {
+    const float v = s48[k * EB_NP + p];
+#pragma unroll
+    for (int q = 0; q < 6; ++q) fma4s(u[q], v, *reinterpret_cast<const float4*>(wp + k * EB_C2 + 4 * q));
+  }
+  float* op = a.t52 + pix * a.ld52 + 24 * g;
+#pragma unroll
+  for (int q = 0; q < 6; ++q) *reinterpret_cast<float4*>(op + 4 * q) = bias_act4<ACT_HARD_SWISH>(u[q], sm + EB_B5 + 24 * g + 4 * q);
+}
+
+bool enc_blocks_supported(int device, int c_in, int c_25, int c_e1, int c_36, int c_e2, int c_52, int ld_x, int ld25, int ld36, int ld48, int ld52) {
+  if (c_in != EB_C0 || c_25 != EB_C0 || c_e1 != EB_E1 || c_36 != EB_C1 || c_e2 != EB_E2 || c_52 != EB_C2) return false;
+  if (ld_x % 4 || ld25 % 4 || ld36 % 4 || ld48 % 4 || ld52 % 4) return false;
+#ifdef BSB_EMU
+  (void)device;
+#else
+  int optin = 0;
+  if (cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, device) != cudaSuccess) { cudaGetLastError(); return false; }
+  if ((size_t)optin < std::max(EA_SMEM, EB_SMEM)) return false;
+#endif
+  return true;
+}
+
+// dynamic shared memory and, for two co-resident CTAs, the whole unified L1 / shared array as shared memory
+static void enc_prepare(const void* k, size_t smem) {
+  ensure_dyn_smem(k, smem);
+#ifndef BSB_EMU
+  static std::mutex mu;
+  static std::map<std::pair<int, const void*>, bool> done;
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) { cudaGetLastError(); return; }
+  std::lock_guard<std::mutex> lock(mu);
+  if (done[std::make_pair(dev, k)]) return;
+  if (cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess) cudaGetLastError();
+  done[std::make_pair(dev, k)] = true;
+#endif
+}
+
+template <int ACT>
+static void launch_enc_blocks_t(cudaStream_t s, dim3 grid, const EncBlocksArgs& a, bool block_b) {
+  if (!block_b) {
+    auto k = k_enc_block_s2<ACT>;
+    enc_prepare(reinterpret_cast<const void*>(k), EA_SMEM);
+    BSB_LAUNCH(k, grid, dim3(256), EA_SMEM, s, a);
+  } else {
+    auto k = k_enc_block_res<ACT>;
+    enc_prepare(reinterpret_cast<const void*>(k), EB_SMEM);
+    BSB_LAUNCH(k, grid, dim3(256), EB_SMEM, s, a);
+  }
+}
+
+void launch_enc_blocks(cudaStream_t s, int B, const EncBlocksArgs& a, bool block_b) {
+  const dim3 grid((unsigned)ceil_div(a.ow, EB_TW), (unsigned)ceil_div(a.oh, EB_TH), (unsigned)B);
+  if (a.act == ACT_RELU) launch_enc_blocks_t<ACT_RELU>(s, grid, a, block_b);
+  else launch_enc_blocks_t<ACT_RELU6>(s, grid, a, block_b);
+  count_launch();
+}
+
+// ---------------------------------------------------------------------------
 // Convolution2DTransposeBias, k = 2x2, stride 2, SAME (even output): no overlap, so
 // out[2y+fy][2x+fx][o] = bias[o] + sum_ic in[y][x][ic] * w[o][fy][fx][ic], ic ascending
 // (the order in which lib/transpose_conv_bias.cc:80-108 scatters into one output).
