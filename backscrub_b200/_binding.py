@@ -32,6 +32,7 @@ SYMBOLS = [
     "bsb_background_new_still", "bsb_background_new_video", "bsb_background_delete", "bsb_background_grab", "bsb_background_grab_into",
     "bsb_background_thumbnail", "bsb_background_frame", "bsb_background_running",
     "bsb_set_sources", "bsb_reset_source", "bsb_set_source_background", "bsb_composite_sources", "bsb_composite_sources_yuyv_device",
+    "bsb_composite_nv12", "bsb_composite_nv12_device", "bsb_composite_sources_nv12_device", "bsb_convert_nv12_to_bgr",
 ]
 
 
@@ -127,4 +128,11 @@ def bind(path: str) -> C.CDLL:
                                         C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t]
     L.bsb_composite_sources_yuyv_device.argtypes = [C.c_void_p, C.c_int, i32p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
                                                     C.c_void_p, C.c_size_t, C.c_int]
+    L.bsb_composite_nv12.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t,
+                                     C.c_void_p, C.c_size_t]
+    L.bsb_composite_nv12_device.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t,
+                                            C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int]
+    L.bsb_composite_sources_nv12_device.argtypes = [C.c_void_p, C.c_int, i32p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p,
+                                                    C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int]
+    L.bsb_convert_nv12_to_bgr.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
     return L

@@ -201,6 +201,41 @@ class MaskGen:
                                                    d_mask or None, npx, int(sync)):
             self._fail("bsb_composite_yuyv_device")
 
+    # -- NV12 camera frames in, NV12 composites out (definitions in include/backscrub_b200.h)
+    def _nv12_layout(self, pitch, uv_offset, in_stride):
+        pitch = self.width if pitch is None else int(pitch)
+        uv_offset = pitch * self.height if uv_offset is None else int(uv_offset)
+        in_stride = uv_offset + pitch * (self.height // 2) if in_stride is None else int(in_stride)
+        return pitch, uv_offset, in_stride
+
+    def composite_nv12(self, frames: np.ndarray, want_out=True, want_nv12=True, want_mask=True):
+        """HOST buffers: tightly packed NV12 frames [n, H*3/2, W] -> (out [n, oh, ow, 3], nv12 [n, oh*3/2, ow], mask)."""
+        frames = np.ascontiguousarray(frames, np.uint8)
+        n = frames.shape[0]
+        if frames.shape[1:] != (self.height * 3 // 2, self.width):
+            raise BackscrubError(f"frame shape {frames.shape[1:]} != {(self.height * 3 // 2, self.width)}")
+        npx = self.height * self.width
+        ow, oh = self.out_width, self.out_height
+        out = np.empty((n, oh, ow, 3), np.uint8) if want_out else None
+        nv12 = np.empty((n, oh * 3 // 2, ow), np.uint8) if want_nv12 else None
+        mask = np.empty((n, self.height, self.width), np.uint8) if want_mask else None
+        ok = self._lib.bsb_composite_nv12(self._h, n, _ptr(frames), npx * 3 // 2,
+                                          _ptr(out) if want_out else None, ow * oh * 3,
+                                          _ptr(nv12) if want_nv12 else None, ow * oh * 3 // 2,
+                                          _ptr(mask) if want_mask else None, npx)
+        if not ok:
+            self._fail("bsb_composite_nv12")
+        return out, nv12, mask
+
+    def composite_nv12_device(self, n, d_nv12, d_out=0, d_nv12_out=0, d_mask=0, sync=False, pitch=None, uv_offset=None, in_stride=None):
+        """DEVICE-resident camera NV12 frames (row pitch, UV plane offset and frame stride default to tight packing) ->
+        BGR / tightly packed NV12 / mask on the device; asynchronous unless `sync`."""
+        p, uv, st = self._nv12_layout(pitch, uv_offset, in_stride)
+        npx, opx = self.height * self.width, self.out_width * self.out_height
+        if not self._lib.bsb_composite_nv12_device(self._h, n, d_nv12, p, uv, st, d_out or None, opx * 3, d_nv12_out or None, opx * 3 // 2,
+                                                   d_mask or None, npx, int(sync)):
+            self._fail("bsb_composite_nv12_device")
+
     # -- independent sources: one frame from each of several cameras per call
     @staticmethod
     def _ids(ids):
@@ -256,6 +291,18 @@ class MaskGen:
                                                            d_mask or None, npx, int(sync)):
             self._fail("bsb_composite_sources_yuyv_device")
 
+    def composite_sources_nv12_device(self, n, ids, d_nv12, d_out=0, d_nv12_out=0, d_mask=0, sync=False, pitch=None, uv_offset=None,
+                                      in_stride=None):
+        """DEVICE-resident camera NV12 frames (layout as composite_nv12_device), frame b of source ids[b]."""
+        m, tab = self._ids(ids)
+        if m != n:
+            raise BackscrubError(f"{m} source ids for {n} frames")
+        p, uv, st = self._nv12_layout(pitch, uv_offset, in_stride)
+        npx, opx = self.height * self.width, self.out_width * self.out_height
+        if not self._lib.bsb_composite_sources_nv12_device(self._h, n, tab, d_nv12, p, uv, st, d_out or None, opx * 3, d_nv12_out or None,
+                                                           opx * 3 // 2, d_mask or None, npx, int(sync)):
+            self._fail("bsb_composite_sources_nv12_device")
+
     def synchronize(self):
         if not self._lib.bsb_synchronize(self._h):
             self._fail("bsb_synchronize")
@@ -305,7 +352,7 @@ class MaskGen:
 
     @property
     def yuyv_native(self) -> bool:
-        """the last composite_yuyv call read the camera YUYV frames in place (no BGR frame was materialised)"""
+        """the last call read the camera frames in their wire format (YUYV or NV12) in place (no BGR frame was materialised)"""
         return bool(self._lib.bsb_yuyv_native(self._h))
 
     @property
@@ -387,5 +434,15 @@ def convert_yuyv_to_bgr(lib, yuyv, device=0):
     h, w, _ = yuyv.shape
     out = np.empty((h, w, 3), np.uint8)
     if not lib.bsb_convert_yuyv_to_bgr(device, _ptr(yuyv), _ptr(out), w, h):
+        raise BackscrubError(lib.bsb_last_error().decode())
+    return out
+
+
+def convert_nv12_to_bgr(lib, nv12, device=0):
+    """cv::cvtColor(COLOR_YUV2BGR_NV12): tightly packed NV12 [H*3/2, W] -> BGR [H, W, 3]."""
+    nv12 = np.ascontiguousarray(nv12, np.uint8)
+    h, w = nv12.shape[0] * 2 // 3, nv12.shape[1]
+    out = np.empty((h, w, 3), np.uint8)
+    if not lib.bsb_convert_nv12_to_bgr(device, _ptr(nv12), _ptr(out), w, h):
         raise BackscrubError(lib.bsb_last_error().decode())
     return out

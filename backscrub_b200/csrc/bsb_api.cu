@@ -432,6 +432,54 @@ int bsb_composite_yuyv_device(bsb_ctx* ctx, int n_frames, const uint8_t* d_yuyv_
   return 1;
 }
 
+// ---- NV12 camera frames in, NV12 composites out ------------------------------------
+int bsb_composite_nv12(bsb_ctx* ctx, int n_frames, const uint8_t* nv12, size_t in_stride, uint8_t* out, size_t out_stride,
+                       uint8_t* nv12_out, size_t nv12_stride, uint8_t* out_mask, size_t mask_stride) {
+  if (!check_ctx(ctx)) return 0;
+  const bsb::Callbacks* cbp = &ctx->cb;
+  Engine* e = ctx->eng;
+  const size_t npix = (size_t)e->W() * e->H(), fnv = npix * 3 / 2;
+  const size_t opix = (size_t)e->out_w() * e->out_h(), obytes = opix * 3, onv = opix * 3 / 2;
+  if (n_frames < 1 || n_frames > e->max_batch()) { report(cbp, "error: n_frames out of range (1..max_batch)"); return 0; }
+  if (!nv12 || in_stride < fnv) { report(cbp, "error: invalid frame"); return 0; }
+  if ((e->W() & 1) || (e->H() & 1)) { report(cbp, "error: NV12 needs an even frame width and height"); return 0; }
+  API_CUDA(cudaSetDevice(e->device()));
+  std::string err;
+  uint8_t* d_nv = nullptr;
+  if (nv12_out && !(d_nv = e->nv12_staging(&err))) { report(cbp, "error: " + err); return 0; }
+  // the frames go to the context's camera staging (max_batch * W*H*2 bytes), tightly packed
+  if (in_stride == fnv) API_CUDA(cudaMemcpyAsync(e->d_yuyv_in(), nv12, fnv * n_frames, cudaMemcpyHostToDevice, e->stream()));
+  else for (int b = 0; b < n_frames; ++b)
+    API_CUDA(cudaMemcpyAsync(e->d_yuyv_in() + b * fnv, nv12 + (size_t)b * in_stride, fnv, cudaMemcpyHostToDevice, e->stream()));
+  if (!e->run_nv12(n_frames, nullptr, e->d_yuyv_in(), (size_t)e->W(), npix, fnv, out ? e->d_out() : nullptr, obytes, d_nv, onv,
+                   out_mask ? e->d_mask() : nullptr, npix, &err)) {
+    report(cbp, "error: failed to process video frame: " + err); return 0;
+  }
+  if (out) for (int b = 0; b < n_frames; ++b)
+    API_CUDA(cudaMemcpyAsync(out + (size_t)b * out_stride, e->d_out() + b * obytes, obytes, cudaMemcpyDeviceToHost, e->stream()));
+  if (nv12_out) for (int b = 0; b < n_frames; ++b)
+    API_CUDA(cudaMemcpyAsync(nv12_out + (size_t)b * nv12_stride, d_nv + b * onv, onv, cudaMemcpyDeviceToHost, e->stream()));
+  if (out_mask) for (int b = 0; b < n_frames; ++b)
+    API_CUDA(cudaMemcpyAsync(out_mask + (size_t)b * mask_stride, e->d_mask() + b * npix, npix, cudaMemcpyDeviceToHost, e->stream()));
+  API_CUDA(cudaStreamSynchronize(e->stream()));
+  API_CUDA(cudaGetLastError());
+  return 1;
+}
+
+int bsb_composite_nv12_device(bsb_ctx* ctx, int n_frames, const uint8_t* d_nv12, size_t in_pitch, size_t uv_offset, size_t in_stride,
+                              uint8_t* d_out, size_t out_stride, uint8_t* d_nv12_out, size_t nv12_stride, uint8_t* d_mask, size_t mask_stride,
+                              int sync) {
+  if (!check_ctx(ctx)) return 0;
+  const bsb::Callbacks* cbp = &ctx->cb;
+  Engine* e = ctx->eng;
+  std::string err;
+  if (!e->run_nv12(n_frames, nullptr, d_nv12, in_pitch, uv_offset, in_stride, d_out, out_stride, d_nv12_out, nv12_stride, d_mask, mask_stride, &err)) {
+    report(cbp, "error: " + err); return 0;
+  }
+  if (sync) { API_CUDA(cudaStreamSynchronize(e->stream())); API_CUDA(cudaGetLastError()); }
+  return 1;
+}
+
 // ---- independent sources ---------------------------------------------------------
 int bsb_set_sources(bsb_ctx* ctx, int n_sources) {
   if (!check_ctx(ctx)) return 0;
@@ -497,6 +545,22 @@ int bsb_composite_sources_yuyv_device(bsb_ctx* ctx, int n, const int* source_ids
   if (d_yuyv && (e->out_w() & 1)) { report(cbp, "error: YUYV output needs an even width"); return 0; }
   std::string err;
   if (!e->run_sources_yuyv(n, source_ids, d_yuyv_frames, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, &err)) {
+    report(cbp, "error: " + err); return 0;
+  }
+  if (sync) { API_CUDA(cudaStreamSynchronize(e->stream())); API_CUDA(cudaGetLastError()); }
+  return 1;
+}
+
+int bsb_composite_sources_nv12_device(bsb_ctx* ctx, int n_frames, const int* source_ids, const uint8_t* d_nv12, size_t in_pitch,
+                                      size_t uv_offset, size_t in_stride, uint8_t* d_out, size_t out_stride, uint8_t* d_nv12_out,
+                                      size_t nv12_stride, uint8_t* d_mask, size_t mask_stride, int sync) {
+  if (!check_ctx(ctx)) return 0;
+  const bsb::Callbacks* cbp = &ctx->cb;
+  Engine* e = ctx->eng;
+  if (!source_ids) { report(cbp, "error: null source id table"); return 0; }
+  std::string err;
+  if (!e->run_nv12(n_frames, source_ids, d_nv12, in_pitch, uv_offset, in_stride, d_out, out_stride, d_nv12_out, nv12_stride, d_mask, mask_stride,
+                   &err)) {
     report(cbp, "error: " + err); return 0;
   }
   if (sync) { API_CUDA(cudaStreamSynchronize(e->stream())); API_CUDA(cudaGetLastError()); }
@@ -570,6 +634,20 @@ int bsb_convert_yuyv_to_bgr(int device, const uint8_t* yuyv, uint8_t* bgr, int w
   if (!a.alloc(npix * 2) || !o.alloc(npix * 3)) { g_last_error = "cudaMalloc failed"; return 0; }
   cudaMemcpy(a.p, yuyv, npix * 2, cudaMemcpyHostToDevice);
   if (npix) bsb::launch_yuyv_to_bgr(nullptr, a.u8(), o.u8(), npix);
+  if (!stage_end()) return 0;
+  cudaMemcpy(bgr, o.p, npix * 3, cudaMemcpyDeviceToHost);
+  return 1;
+}
+
+int bsb_convert_nv12_to_bgr(int device, const uint8_t* nv12, uint8_t* bgr, int width, int height) {
+  if (!nv12 || !bgr || width < 0 || height < 0) { g_last_error = "invalid argument"; return 0; }
+  if ((width | height) & 1) { g_last_error = "NV12 needs an even width and height"; return 0; }
+  const size_t npix = (size_t)width * height;
+  if (!stage_begin(device)) return 0;
+  DevBuf a, o;
+  if (!a.alloc(npix * 3 / 2) || !o.alloc(npix * 3)) { g_last_error = "cudaMalloc failed"; return 0; }
+  cudaMemcpy(a.p, nv12, npix * 3 / 2, cudaMemcpyHostToDevice);
+  if (npix) bsb::launch_nv12_to_bgr(nullptr, 1, a.u8(), (size_t)width, npix, npix * 3 / 2, o.u8(), width, height);
   if (!stage_end()) return 0;
   cudaMemcpy(bgr, o.p, npix * 3, cudaMemcpyDeviceToHost);
   return 1;

@@ -931,7 +931,8 @@ Engine::~Engine() {
   for (void* p : {(void*)wblob_, (void*)arena_, (void*)lut_, (void*)rowsum_, (void*)in_u8_, (void*)filt_u8_, (void*)state_, (void*)ofinal_,
                   (void*)d_frames_, (void*)d_out_, (void*)d_yuyv_, (void*)d_mask_, (void*)d_bg_, (void*)d_bg_raw_, (void*)d_yuyv_in_,
                   tab_in_.blob, tab_up_.blob, tab_bg_.blob, tab_out_.blob, (void*)d_bg_cursor_, (void*)d_bg_eff_, (void*)d_bg_frames_,
-                  (void*)d_gauss_tmp_, (void*)d_stage_a_, (void*)d_stage_b_, (void*)d_stage_c_, (void*)d_bg_yuyv_, (void*)pool_counters_, (void*)d_tile_geo_})
+                  (void*)d_gauss_tmp_, (void*)d_stage_a_, (void*)d_stage_b_, (void*)d_stage_c_, (void*)d_bg_yuyv_, (void*)pool_counters_, (void*)d_tile_geo_,
+                  (void*)d_bg_nv12_, (void*)d_nv12_})
     if (p) cudaFree(p);
   for (ChainPlan& cp : chains_) if (cp.d_ops) cudaFree(cp.d_ops);
   free_sources();
@@ -944,10 +945,13 @@ Engine::~Engine() {
 // enqueue: the per-call kernel sequence (captured into a CUDA graph by run())
 // ---------------------------------------------------------------------------
 void Engine::enqueue_pre(int n, const uint8_t* d_frames, size_t pitch, size_t stride, const uint8_t* d_yuyv_in) {
-  // camera YUYV frames are read in place (each bilinear tap converted like cv::COLOR_YUV2BGR_YUYV would have)
-  if (d_yuyv_in)
+  // camera YUYV / NV12 frames are read in place (each bilinear tap converted like cv::COLOR_YUV2BGR_YUYV / _NV12 would have)
+  if (d_yuyv_in && nv12_.on)
+    launch_resize_roi_swap(stream_, n, d_yuyv_in, nv12_.stride, nv12_.pitch, roidim_[0], roidim_[1], roidim_[2], roidim_[3], tab_in_.tab,
+                           in_u8_, mw_, mh_, in_roidim_[0], in_roidim_[1], in_roidim_[2], in_roidim_[3], tab_in_.area2x2, IN_NV12, nv12_.uv);
+  else if (d_yuyv_in)
     launch_resize_roi_swap(stream_, n, d_yuyv_in, (size_t)W_ * H_ * 2, (size_t)W_ * 2, roidim_[0], roidim_[1], roidim_[2], roidim_[3], tab_in_.tab,
-                           in_u8_, mw_, mh_, in_roidim_[0], in_roidim_[1], in_roidim_[2], in_roidim_[3], tab_in_.area2x2, true);
+                           in_u8_, mw_, mh_, in_roidim_[0], in_roidim_[1], in_roidim_[2], in_roidim_[3], tab_in_.area2x2, IN_YUYV);
   else
     launch_resize_roi_swap(stream_, n, d_frames, stride, pitch, roidim_[0], roidim_[1], roidim_[2], roidim_[3], tab_in_.tab,
                            in_u8_, mw_, mh_, in_roidim_[0], in_roidim_[1], in_roidim_[2], in_roidim_[3], tab_in_.area2x2);
@@ -1167,16 +1171,22 @@ void Engine::enqueue_decision(int n) {
   else launch_decision_iir(stream_, model_type_, n, tptr(g_.output), oh_, ow_, oc_, state_, ofinal_, opitch_);
 }
 
-// PostArgs of one call.  `yuyv_native` (optional out): the frames can stay in camera YUYV format for the post kernel.
+// PostArgs of one call.  d_yuyv_in (non-null): the post kernel reads the camera frames in place — YUYV, or NV12 in an NV12
+// call, which then also writes its video output (d_yuyv) as NV12.
 PostArgs Engine::post_args(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
                            uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in) const {
   const size_t fbytes = (size_t)W_ * H_ * 3;
   const bool flip = flip_h_ || flip_v_, resized = out_w_ != W_ || out_h_ != H_, tail = flip || resized;
   const bool want_rgb = d_out || d_yuyv;
+  const bool nv12_in = nv12_.on && d_yuyv_in;
   PostArgs a{};
   a.B = n; a.W = W_; a.H = H_;
   a.frames = d_frames; a.frame_pitch = pitch; a.frame_stride = stride;
-  a.yuyv_in = d_yuyv_in; a.yuyv_in_stride = (size_t)W_ * H_ * 2;
+  if (nv12_in) {
+    a.nv12_in = d_yuyv_in; a.nv12_in_pitch = nv12_.pitch; a.nv12_in_uv = nv12_.uv; a.nv12_in_stride = nv12_.stride;
+  } else {
+    a.yuyv_in = d_yuyv_in; a.yuyv_in_stride = (size_t)W_ * H_ * 2;
+  }
   a.bg = d_bg_; a.bg_pitch = (size_t)W_ * 3; a.bg_stride = 0;
   if (has_bg_) {
     if (bgblur_k_) a.bg = d_bg_eff_;                       // blurred once, when the background / strength was set
@@ -1184,14 +1194,17 @@ PostArgs Engine::post_args(int n, const uint8_t* d_frames, size_t pitch, size_t 
   } else if (bgblur_k_ && want_rgb) {
     a.bg = d_bg_frames_; a.bg_stride = fbytes;            // the blurred camera frame itself (filled by enqueue_post)
   }
-  if (bg_yuyv_valid_ && !(bgblur_k_ && !has_bg_)) a.bg_yuyv = d_bg_yuyv_;
+  if (bg_yuyv_valid_ && !(bgblur_k_ && !has_bg_)) { a.bg_yuyv = d_bg_yuyv_; a.bg_nv12 = bg_nv12_valid_ ? d_bg_nv12_ : nullptr; }
   if (call_mode_ != CALL_PLAIN) {
     // sources: frame b blends bank slot bg_index[b]; the bank's YUYV holds no camera-blur slots, so a call with such a
     // frame converts every tile (what a plain context in camera-blur mode does)
     a.bg = d_bank_; a.bg_stride = fbytes; a.bg_cursor = nullptr; a.bg_advance = 0;
     a.bg_index = d_src_tab_ + max_batch_; a.bg_count = bank_slots();
     a.bg_yuyv = (call_mode_ == CALL_SOURCES && !(W_ & 1)) ? d_bank_yuyv_ : nullptr;
+    a.bg_nv12 = call_mode_ == CALL_SOURCES ? d_bank_nv12_ : nullptr;
   }
+  // the cached background in the call's video format (NV12 where the kernel writes NV12, else YUYV)
+  if (nv12_in) a.bg_yuyv = nullptr; else a.bg_nv12 = nullptr;
   a.ofinal = ofinal_; a.ow = ow_; a.oh = oh_; a.opitch = opitch_;
   a.out_x = out_roidim_[0]; a.out_y = out_roidim_[1]; a.out_w = out_roidim_[2]; a.out_h = out_roidim_[3];
   a.roi_x = roidim_[0]; a.roi_y = roidim_[1]; a.roi_w = roidim_[2]; a.roi_h = roidim_[3];
@@ -1199,7 +1212,8 @@ PostArgs Engine::post_args(int n, const uint8_t* d_frames, size_t pitch, size_t 
   a.out_pitch = (size_t)W_ * 3;
   if (!tail) {
     a.out = d_out; a.out_stride = out_stride;
-    a.yuyv = d_yuyv; a.yuyv_stride = yuyv_stride;
+    if (nv12_in) { a.nv12 = d_yuyv; a.nv12_stride = yuyv_stride; }
+    else { a.yuyv = d_yuyv; a.yuyv_stride = yuyv_stride; }
   } else {
     a.out = want_rgb ? d_stage_a_ : nullptr; a.out_stride = fbytes;
     a.yuyv = nullptr; a.yuyv_stride = 0;
@@ -1243,9 +1257,9 @@ void Engine::enqueue_post(int n, const uint8_t* d_frames, size_t pitch, size_t s
   if (d_yuyv) launch_rgb_to_yuyv(stream_, cur, d_yuyv, (size_t)out_w_ * out_h_, n, cur_stride, yuyv_stride);
 }
 
-// Camera YUYV input: the pre-processing kernel always reads the YUYV frames in place; the BGR frame is materialised
-// (k_yuyv_to_bgr into `d_frames`) only when the post stage cannot read YUYV itself — no TMA path for this geometry, or
-// the blur-my-background mode, whose Gaussian runs on the BGR frame.
+// Camera YUYV / NV12 input: the pre-processing kernel always reads the frames in place; the BGR frame is materialised
+// (k_yuyv_to_bgr / k_nv12_to_bgr into `d_frames`) only when the post stage cannot read the wire format itself — no TMA
+// path for this geometry or layout, or the blur-my-background mode, whose Gaussian runs on the BGR frame.
 bool Engine::yuyv_native(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
                          uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in) const {
   const bool camblur = call_mode_ == CALL_PLAIN ? (bgblur_k_ && !has_bg_) : call_mode_ == CALL_SOURCES_CAMBLUR;
@@ -1257,14 +1271,24 @@ void Engine::enqueue_all(int n, const uint8_t* d_frames, size_t pitch, size_t st
                          uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in,
                          bool native, bool sync_cbs) {
   const long l0 = thread_launch_count();
-  if (d_yuyv_in && !native) launch_yuyv_to_bgr(stream_, d_yuyv_in, const_cast<uint8_t*>(d_frames), (size_t)n * W_ * H_);
+  if (d_yuyv_in && !native) {
+    if (nv12_.on) launch_nv12_to_bgr(stream_, n, d_yuyv_in, nv12_.pitch, nv12_.uv, nv12_.stride, const_cast<uint8_t*>(d_frames), W_, H_);
+    else launch_yuyv_to_bgr(stream_, d_yuyv_in, const_cast<uint8_t*>(d_frames), (size_t)n * W_ * H_);
+  }
   enqueue_pre(n, d_frames, pitch, stride, d_yuyv_in);
   if (sync_cbs && cb_.onprep) { cudaStreamSynchronize(stream_); cb_.onprep(cb_.caller_ctx); }
   enqueue_cnn(n, true);
   if (sync_cbs && cb_.oninfer) { cudaStreamSynchronize(stream_); cb_.oninfer(cb_.caller_ctx); }
   enqueue_decision(n);
   if (sync_cbs && cb_.onmask) { cudaStreamSynchronize(stream_); cb_.onmask(cb_.caller_ctx); }
-  enqueue_post(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, native ? d_yuyv_in : nullptr);
+  // NV12 output: the post kernel writes it when it reads the NV12 frames in place and no flip / resize follows; otherwise
+  // the YUYV output goes to the context staging and k_yuyv_to_nv12 derives the NV12 from it (the definition)
+  const bool tail = flip_h_ || flip_v_ || out_w_ != W_ || out_h_ != H_;
+  const bool nv12_staged = nv12_.on && d_yuyv && !(native && !tail);
+  const size_t opix = (size_t)out_w_ * out_h_;
+  enqueue_post(n, d_frames, pitch, stride, d_out, out_stride, nv12_staged ? d_yuyv_ : d_yuyv, nv12_staged ? opix * 2 : yuyv_stride, d_mask,
+               mask_stride, native ? d_yuyv_in : nullptr);
+  if (nv12_staged) launch_yuyv_to_nv12(stream_, n, d_yuyv_, opix * 2, d_yuyv, yuyv_stride, out_w_, out_h_);
   last_call_launches_ = (int)(thread_launch_count() - l0);
 }
 
@@ -1288,7 +1312,7 @@ bool Engine::run(int n, const uint8_t* d_frames, size_t pitch, size_t stride, ui
   }
 #ifndef BSB_EMU
   const GraphKey key{n, d_frames, pitch, stride, d_out, d_yuyv, d_mask, d_yuyv_in, d_out ? out_stride : 0, d_yuyv ? yuyv_stride : 0,
-                     d_mask ? mask_stride : 0, call_mode_};
+                     d_mask ? mask_stride : 0, call_mode_, nv12_.on, nv12_.pitch, nv12_.uv, nv12_.stride};
   auto it = graphs_.find(key);
   if (it == graphs_.end()) {
     if (graphs_.size() >= 64) drop_graphs();
@@ -1321,6 +1345,27 @@ bool Engine::run_yuyv(int n, const uint8_t* d_yuyv_in, uint8_t* d_out, size_t ou
                       uint8_t* d_mask, size_t mask_stride, std::string* err) {
   const size_t row = (size_t)W_ * 3;
   return run(n, d_frames_, row, row * H_, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, false, err, d_yuyv_in);
+}
+
+bool Engine::run_nv12(int n, const int* ids, const uint8_t* d_nv12, size_t pitch, size_t uv_off, size_t in_stride, uint8_t* d_out,
+                      size_t out_stride, uint8_t* d_nv12_out, size_t nv12_stride, uint8_t* d_mask, size_t mask_stride, std::string* err) {
+  if ((W_ & 1) || (H_ & 1)) { *err = "NV12 needs an even frame width and height"; return false; }
+  if (d_nv12_out && ((out_w_ & 1) || (out_h_ & 1))) { *err = "NV12 output needs an even output width and height"; return false; }
+  if (!d_nv12) { *err = "invalid frame"; return false; }
+  if (pitch < (size_t)W_) { *err = "NV12 row pitch is smaller than the frame width"; return false; }
+  if (uv_off < pitch * H_) { *err = "NV12 UV plane offset lies inside the Y plane"; return false; }
+  if (in_stride < uv_off + pitch * (size_t)(H_ / 2 - 1) + (size_t)W_) { *err = "NV12 frame does not fit in the frame stride"; return false; }
+  const size_t row = (size_t)W_ * 3;
+  nv12_ = Nv12Call{true, pitch, uv_off, in_stride};
+  const bool ok = ids ? run_sources(n, ids, d_frames_, row, row * H_, d_out, out_stride, d_nv12_out, nv12_stride, d_mask, mask_stride, err, d_nv12)
+                      : run(n, d_frames_, row, row * H_, d_out, out_stride, d_nv12_out, nv12_stride, d_mask, mask_stride, false, err, d_nv12);
+  nv12_ = Nv12Call{};
+  return ok;
+}
+
+uint8_t* Engine::nv12_staging(std::string* err) {
+  if (!ensure((void**)&d_nv12_, &nv12_cap_, (size_t)max_batch_ * out_w_ * out_h_ * 3 / 2, err)) return nullptr;
+  return d_nv12_;
 }
 
 bool Engine::infer(int n, const float* h_in, float* h_out, std::string* err) {
@@ -1418,6 +1463,13 @@ bool Engine::refresh_bg_yuyv(std::string* err) {
   launch_rgb_to_yuyv(stream_, src, d_bg_yuyv_, npix, bg_count_, npix * 3, npix * 2);
   CUDA_OK(cudaGetLastError());
   bg_yuyv_valid_ = true;
+  // ... and its NV12 for NV12 calls
+  bg_nv12_valid_ = false;
+  if (H_ & 1) return true;
+  if (!ensure((void**)&d_bg_nv12_, &bg_nv12_cap_, npix * 3 / 2 * (size_t)bg_count_, err)) return false;
+  launch_yuyv_to_nv12(stream_, bg_count_, d_bg_yuyv_, npix * 2, d_bg_nv12_, npix * 3 / 2, W_, H_);
+  CUDA_OK(cudaGetLastError());
+  bg_nv12_valid_ = true;
   return true;
 }
 
@@ -1477,8 +1529,8 @@ bool Engine::reset_state(std::string* err) {
 // independent sources
 // ---------------------------------------------------------------------------
 void Engine::free_sources() {
-  for (void* p : {(void*)src_state_, (void*)d_bank_, (void*)d_bank_yuyv_, (void*)d_src_bg_}) if (p) cudaFree(p);
-  src_state_ = nullptr; d_bank_ = nullptr; d_bank_yuyv_ = nullptr; d_src_bg_ = nullptr;
+  for (void* p : {(void*)src_state_, (void*)d_bank_, (void*)d_bank_yuyv_, (void*)d_bank_nv12_, (void*)d_src_bg_}) if (p) cudaFree(p);
+  src_state_ = nullptr; d_bank_ = nullptr; d_bank_yuyv_ = nullptr; d_bank_nv12_ = nullptr; d_src_bg_ = nullptr;
   n_sources_ = 0;
   src_has_bg_.clear();
 }
@@ -1502,6 +1554,10 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   if (!(W_ & 1)) {
     CUDA_OK(cudaMalloc((void**)&d_bank_yuyv_, slots * npix * 2));
     CUDA_OK(cudaMemset(d_bank_yuyv_, 0, slots * npix * 2));
+    if (!(H_ & 1)) {
+      CUDA_OK(cudaMalloc((void**)&d_bank_nv12_, slots * npix * 3 / 2));
+      CUDA_OK(cudaMemset(d_bank_nv12_, 0, slots * npix * 3 / 2));
+    }
   }
   CUDA_OK(cudaMalloc((void**)&d_src_bg_, (size_t)n_sources * fbytes));
   n_sources_ = n_sources;
@@ -1528,6 +1584,8 @@ bool Engine::refresh_bank_ctx(std::string* err) {
   uint8_t* slot = d_bank_ + (size_t)max_batch_ * fbytes;
   CUDA_OK(cudaMemcpyAsync(slot, (has_bg_ && bgblur_k_) ? d_bg_eff_ : d_bg_, fbytes, cudaMemcpyDeviceToDevice, stream_));
   if (d_bank_yuyv_) launch_rgb_to_yuyv(stream_, slot, d_bank_yuyv_ + (size_t)max_batch_ * npix * 2, npix);
+  if (d_bank_nv12_)
+    launch_yuyv_to_nv12(stream_, 1, d_bank_yuyv_ + (size_t)max_batch_ * npix * 2, 0, d_bank_nv12_ + (size_t)max_batch_ * npix * 3 / 2, 0, W_, H_);
   CUDA_OK(cudaGetLastError());
   return true;
 }
@@ -1541,6 +1599,7 @@ bool Engine::refresh_bank_source(int s, std::string* err) {
   if (bgblur_k_) launch_gauss_blur(stream_, 1, src, (size_t)W_ * 3, fbytes, d_gauss_tmp_, slot, (size_t)W_ * 3, fbytes, W_, H_, taps_);
   else CUDA_OK(cudaMemcpyAsync(slot, src, fbytes, cudaMemcpyDeviceToDevice, stream_));
   if (d_bank_yuyv_) launch_rgb_to_yuyv(stream_, slot, d_bank_yuyv_ + k * npix * 2, npix);
+  if (d_bank_nv12_) launch_yuyv_to_nv12(stream_, 1, d_bank_yuyv_ + k * npix * 2, 0, d_bank_nv12_ + k * npix * 3 / 2, 0, W_, H_);
   CUDA_OK(cudaGetLastError());
   return true;
 }

@@ -116,6 +116,13 @@ class Engine {
                    const uint8_t* d_yuyv_in = nullptr);
   bool run_sources_yuyv(int n, const int* ids, const uint8_t* d_yuyv_in, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv, size_t yuyv_stride,
                         uint8_t* d_mask, size_t mask_stride, std::string* err);
+  // Camera NV12 frames (W, H even): Y rows `pitch` bytes apart, the UV plane at byte `uv_off` of a frame, `in_stride` bytes
+  // per frame.  The video output is tightly packed NV12 (`nv12_stride` bytes per frame).  ids == nullptr: a plain call,
+  // else a sources call as run_sources.
+  bool run_nv12(int n, const int* ids, const uint8_t* d_nv12, size_t pitch, size_t uv_off, size_t in_stride, uint8_t* d_out, size_t out_stride,
+                uint8_t* d_nv12_out, size_t nv12_stride, uint8_t* d_mask, size_t mask_stride, std::string* err);
+  // device staging of max_batch NV12 output frames (host-buffer API), grown on demand; nullptr on error
+  uint8_t* nv12_staging(std::string* err);
   int n_sources() const { return n_sources_; }
   double time_stage(int stage, int n, int iters, std::string* err);
 
@@ -274,7 +281,16 @@ class Engine {
   uint8_t* d_bg_yuyv_ = nullptr;     // YUYV of the effective background (ring): all-background tiles are copies
   size_t bg_yuyv_cap_ = 0;
   bool bg_yuyv_valid_ = false;
-  bool last_native_ = false;         // the last call read camera YUYV in place (no BGR frame was materialised)
+  uint8_t* d_bg_nv12_ = nullptr;     // ... and its NV12 (W*H*3/2 bytes per image; even W and H), for NV12 calls
+  size_t bg_nv12_cap_ = 0;
+  bool bg_nv12_valid_ = false;
+  bool last_native_ = false;         // the last call read the camera frames (YUYV or NV12) in place (no BGR frame was materialised)
+  // Format of the NV12 call being enqueued (set by run_nv12 around run / run_sources, like call_mode_): the camera pointer
+  // (d_yuyv_in) holds NV12 frames with this layout, and the video output pointer (d_yuyv) receives NV12
+  struct Nv12Call { bool on = false; size_t pitch = 0, uv = 0, stride = 0; };
+  Nv12Call nv12_;
+  uint8_t* d_nv12_ = nullptr;        // host-buffer API staging of the NV12 output
+  size_t nv12_cap_ = 0;
   int last_call_launches_ = 0;
   size_t stage_a_cap_ = 0, stage_b_cap_ = 0, stage_c_cap_ = 0, out_cap_ = 0, yuyv_cap_ = 0;
 
@@ -287,8 +303,9 @@ class Engine {
   uint8_t* src_state_ = nullptr;     // [n_sources][oh*ow] smoother state per source
   int* d_src_tab_ = nullptr;         // [2][max_batch]: source id of frame b | background-bank slot of frame b (written before each launch)
   // background bank, one base + one stride for the post kernel: [max_batch] camera-blur slots | [1] the context's effective
-  // background | [n_sources] source slots; d_bank_yuyv_ is its YUYV (valid for the context and source slots)
-  uint8_t* d_bank_ = nullptr, *d_bank_yuyv_ = nullptr;
+  // background | [n_sources] source slots; d_bank_yuyv_ is its YUYV and d_bank_nv12_ its NV12 (valid for the context and
+  // source slots)
+  uint8_t* d_bank_ = nullptr, *d_bank_yuyv_ = nullptr, *d_bank_nv12_ = nullptr;
   uint8_t* d_src_bg_ = nullptr;      // [n_sources] resized, unblurred source backgrounds (re-blurred when bgblur changes)
   uint8_t* d_src_raw_ = nullptr;     // staging of one decoded source background
   size_t src_raw_cap_ = 0;
@@ -305,9 +322,10 @@ class Engine {
     int n; const void* f; size_t pitch, stride; const void* o; const void* y; const void* m; const void* yin;
     size_t ostride, ystride, mstride;
     int mode;                        // CallMode: a plain and a sources graph over the same buffers are different graphs
+    bool nv12; size_t npitch, nuv, nstride;   // NV12 call and its input layout: never confused with a YUYV call
     bool operator<(const GraphKey& r) const {
-      return std::tie(n, f, pitch, stride, o, y, m, yin, ostride, ystride, mstride, mode) <
-             std::tie(r.n, r.f, r.pitch, r.stride, r.o, r.y, r.m, r.yin, r.ostride, r.ystride, r.mstride, r.mode);
+      return std::tie(n, f, pitch, stride, o, y, m, yin, ostride, ystride, mstride, mode, nv12, npitch, nuv, nstride) <
+             std::tie(r.n, r.f, r.pitch, r.stride, r.o, r.y, r.m, r.yin, r.ostride, r.ystride, r.mstride, r.mode, r.nv12, r.npitch, r.nuv, r.nstride);
     }
   };
 #ifndef BSB_EMU

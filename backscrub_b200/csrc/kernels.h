@@ -174,12 +174,16 @@ struct ResizeTab {        // OpenCV INTER_LINEAR 8-bit tables (device pointers)
   const uint2* xcol;      // [dw] packed {sx | sx1 << 16, a0 | a1 << 16} (sx1 = min(sx + 1, sw - 1))
 };
 
+// format of the frames a call reads: BGR, or a camera wire format read in place
+enum InFmt : int { IN_BGR = 0, IN_YUYV = 1, IN_NV12 = 2 };
+
 // lib/libbackscrub.cc:285-290: ROI crop -> cv::resize(INTER_LINEAR) -> BGR2RGB, into the
 // zero-padded model-sized u8 image.  frames: B x (H x W x 3, stride bytes).
 void launch_resize_roi_swap(cudaStream_t s, int B, const uint8_t* frames, size_t frame_stride, size_t frame_pitch,
                             int roi_x, int roi_y, int roi_w, int roi_h, ResizeTab tab,
                             uint8_t* in_u8, int mw, int mh, int in_x, int in_y, int in_w, int in_h, bool area2x2,
-                            bool in_yuyv = false);   // in_yuyv: `frames` are camera YUYV frames (pitch W*2), converted per tap
+                            int in_fmt = IN_BGR,     // IN_YUYV: camera YUYV frames (pitch W*2); IN_NV12: camera NV12 frames
+                            size_t uv_off = 0);      // (Y rows `frame_pitch` apart, UV plane at byte uv_off); converted per tap
 
 // lib/libbackscrub.cc:295-302: bilateralFilter(5,100,100) + convertTo(CV_32F, scale, offset)
 void launch_bilateral_norm(cudaStream_t s, int B, const uint8_t* in_u8, int mw, int mh,
@@ -235,12 +239,18 @@ struct PostArgs {
   // converted to YUYV, same indexing as `bg` with W*2-byte rows, so all-background tiles are pure copies.
   const uint8_t* yuyv_in; size_t yuyv_in_stride;
   const uint8_t* bg_yuyv;
+  // TMA path only, NV12 calls: camera NV12 frames read in place (Y rows `nv12_in_pitch` bytes apart, the UV plane at byte
+  // `nv12_in_uv` of a frame, `nv12_in_stride` bytes per frame), the video output written as tightly packed NV12
+  // (`nv12_stride` bytes per frame; yuyv is null), and the background (ring / bank) as NV12, W*H*3/2 bytes per image
+  const uint8_t* nv12_in; size_t nv12_in_pitch, nv12_in_uv, nv12_in_stride;
+  uint8_t* nv12; size_t nv12_stride;
+  const uint8_t* bg_nv12;
   // per tile row / tile column: the patch of the small mask a (TW + 4) x 36 halo tile touches, {first, count}
   // (precomputed once per context from `tab`: the patch request is the head of every CTA's critical path)
   const int2* geo_rows; const int2* geo_cols64; const int2* geo_cols128;
 };
 void launch_post(cudaStream_t s, const PostArgs& a);
-// true if launch_post will take the TMA kernel for these arguments (the only one that can read a.yuyv_in)
+// true if launch_post will take the TMA kernel for these arguments (the only one that can read a.yuyv_in / a.nv12_in)
 bool post_tma_eligible(const PostArgs& a);
 
 // app/background.cc:178-194: cv::resize(raw -> W x H), 3 channels
@@ -266,6 +276,12 @@ void launch_yuyv_to_bgr(cudaStream_t s, const uint8_t* yuyv, uint8_t* bgr, size_
 void launch_alpha_blend(cudaStream_t s, const uint8_t* a, const uint8_t* b, const uint8_t* mask, uint8_t* out, size_t npix);
 // npix pixels per frame (even), n frames
 void launch_rgb_to_yuyv(cudaStream_t s, const uint8_t* rgb, uint8_t* yuyv, size_t npix, int n = 1, size_t rgb_stride = 0, size_t yuyv_stride = 0);
+// cv::cvtColor(COLOR_YUV2BGR_NV12): n camera NV12 frames (W, H even; Y rows `pitch` apart, UV plane at byte uv_off,
+// `in_stride` bytes per frame) -> tightly packed BGR frames
+void launch_nv12_to_bgr(cudaStream_t s, int n, const uint8_t* nv12, size_t pitch, size_t uv_off, size_t in_stride, uint8_t* bgr, int W, int H);
+// the project's NV12 output from its YUYV output (include/backscrub_b200.h): n frames of W x H (even), tightly packed
+// W*2-byte YUYV rows -> tightly packed NV12 (Y plane, UV plane at byte W*H)
+void launch_yuyv_to_nv12(cudaStream_t s, int n, const uint8_t* yuyv, size_t yuyv_stride, uint8_t* nv12, size_t nv12_stride, int W, int H);
 // *cursor = (*cursor + step) % count, after the frames of a call have been blended
 void launch_advance_cursor(cudaStream_t s, int* cursor, int step, int count);
 

@@ -35,20 +35,40 @@ BSB_D size_t bg_frame_offset(const PostArgs& a, int b) {
 // ROI crop -> resize -> BGR2RGB into the zero-padded model-sized image.
 // One thread = one destination pixel (3 channels).
 // ---------------------------------------------------------------------------
-// IN_YUYV: `frames` are camera YUYV frames (W*2-byte rows); every tap is first converted the way
-// cv::cvtColor(COLOR_YUV2BGR_YUYV) would have (cv::VideoCapture's conversion, app/deepseg.cc:553), so the result
+// FMT (InFmt): IN_BGR frames; IN_YUYV: camera YUYV frames (W*2-byte rows); IN_NV12: camera NV12 frames (Y rows `pitch`
+// bytes apart, the UV plane at byte `uv_off` of the frame).  Every tap of a camera frame is first converted the way
+// cv::cvtColor(COLOR_YUV2BGR_YUYV / _NV12) would have (cv::VideoCapture's conversion, app/deepseg.cc:553), so the result
 // equals converting the whole frame first — without materialising the BGR frame.
-template <bool IN_YUYV>
+template <int FMT>
 __global__ void __launch_bounds__(256) k_resize_roi_swap(int B, const uint8_t* frames, size_t frame_stride, size_t pitch,
                                                          int roi_x, int roi_y, int roi_w, int roi_h, ResizeTab t,
                                                          uint8_t* in_u8, int mw, int mh, int in_x, int in_y, int in_w, int in_h,
-                                                         bool area2x2) {
+                                                         bool area2x2, size_t uv_off) {
   const long total = (long)B * in_w * in_h;
   const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
   const int dx = (int)(idx % in_w), dy = (int)((idx / in_w) % in_h), b = (int)(idx / ((long)in_w * in_h));
   uint8_t px[3];
-  if (IN_YUYV) {
+  if (FMT == IN_NV12) {
+    const uint8_t* img = frames + (size_t)b * frame_stride;
+    int p00[3], p01[3], p10[3], p11[3];
+    if (area2x2) {
+      const int y0 = roi_y + 2 * dy, x0 = roi_x + 2 * dx;
+      nv12_px_to_bgr(img, pitch, uv_off, x0, y0, p00); nv12_px_to_bgr(img, pitch, uv_off, x0 + 1, y0, p01);
+      nv12_px_to_bgr(img, pitch, uv_off, x0, y0 + 1, p10); nv12_px_to_bgr(img, pitch, uv_off, x0 + 1, y0 + 1, p11);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) px[c] = (uint8_t)((p00[c] + p01[c] + p10[c] + p11[c] + 2) >> 2);
+    } else {
+      const int sx = __ldg(t.xofs + dx), sx1 = min(sx + 1, roi_w - 1);
+      const int a0 = __ldg(t.xw + 2 * dx), a1 = __ldg(t.xw + 2 * dx + 1);
+      const int b0 = __ldg(t.yw + 2 * dy), b1 = __ldg(t.yw + 2 * dy + 1);
+      const int y0 = roi_y + __ldg(t.yofs0 + dy), y1 = roi_y + __ldg(t.yofs1 + dy);
+      nv12_px_to_bgr(img, pitch, uv_off, roi_x + sx, y0, p00); nv12_px_to_bgr(img, pitch, uv_off, roi_x + sx1, y0, p01);
+      nv12_px_to_bgr(img, pitch, uv_off, roi_x + sx, y1, p10); nv12_px_to_bgr(img, pitch, uv_off, roi_x + sx1, y1, p11);
+#pragma unroll
+      for (int c = 0; c < 3; ++c) px[c] = lin_v(p00[c] * a0 + p01[c] * a1, p10[c] * a0 + p11[c] * a1, b0, b1);
+    }
+  } else if (FMT == IN_YUYV) {
     const uint8_t* img = frames + (size_t)b * frame_stride;
     if (area2x2) {
       int p00[3], p01[3], p10[3], p11[3];
@@ -93,12 +113,16 @@ __global__ void __launch_bounds__(256) k_resize_roi_swap(int B, const uint8_t* f
 
 void launch_resize_roi_swap(cudaStream_t s, int B, const uint8_t* frames, size_t frame_stride, size_t frame_pitch,
                             int roi_x, int roi_y, int roi_w, int roi_h, ResizeTab tab,
-                            uint8_t* in_u8, int mw, int mh, int in_x, int in_y, int in_w, int in_h, bool area2x2, bool in_yuyv) {
+                            uint8_t* in_u8, int mw, int mh, int in_x, int in_y, int in_w, int in_h, bool area2x2, int in_fmt,
+                            size_t uv_off) {
   const long total = (long)B * in_w * in_h;
-  if (in_yuyv) BSB_LAUNCH(k_resize_roi_swap<true>, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, s, B, frames, frame_stride, frame_pitch,
-                          roi_x, roi_y, roi_w, roi_h, tab, in_u8, mw, mh, in_x, in_y, in_w, in_h, area2x2);
-  else BSB_LAUNCH(k_resize_roi_swap<false>, dim3((unsigned)((total + 255) / 256)), dim3(256), 0, s, B, frames, frame_stride, frame_pitch,
-                  roi_x, roi_y, roi_w, roi_h, tab, in_u8, mw, mh, in_x, in_y, in_w, in_h, area2x2);
+  const dim3 grid((unsigned)((total + 255) / 256));
+  if (in_fmt == IN_NV12) BSB_LAUNCH(k_resize_roi_swap<IN_NV12>, grid, dim3(256), 0, s, B, frames, frame_stride, frame_pitch,
+                                    roi_x, roi_y, roi_w, roi_h, tab, in_u8, mw, mh, in_x, in_y, in_w, in_h, area2x2, uv_off);
+  else if (in_fmt == IN_YUYV) BSB_LAUNCH(k_resize_roi_swap<IN_YUYV>, grid, dim3(256), 0, s, B, frames, frame_stride, frame_pitch,
+                                         roi_x, roi_y, roi_w, roi_h, tab, in_u8, mw, mh, in_x, in_y, in_w, in_h, area2x2, uv_off);
+  else BSB_LAUNCH(k_resize_roi_swap<IN_BGR>, grid, dim3(256), 0, s, B, frames, frame_stride, frame_pitch,
+                  roi_x, roi_y, roi_w, roi_h, tab, in_u8, mw, mh, in_x, in_y, in_w, in_h, area2x2, uv_off);
   count_launch();
 }
 
@@ -868,6 +892,58 @@ __global__ void __launch_bounds__(256) k_rgb_to_yuyv(const uint8_t* rgb, uint8_t
 void launch_rgb_to_yuyv(cudaStream_t s, const uint8_t* rgb, uint8_t* yuyv, size_t npix, int n, size_t rgb_stride, size_t yuyv_stride) {
   const size_t npairs = npix / 2;
   BSB_LAUNCH(k_rgb_to_yuyv, dim3((unsigned)((npairs + 255) / 256), (unsigned)n), dim3(256), 0, s, rgb, yuyv, npairs, rgb_stride, yuyv_stride);
+  count_launch();
+}
+
+// ---------------------------------------------------------------------------
+// NV12 <-> the project's YUYV / BGR (definitions in include/backscrub_b200.h).  Used where the post stage cannot read or
+// write NV12 itself; one thread = a 2x2 pixel block (one UV pair), n frames along blockIdx.y.
+// ---------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_nv12_to_bgr(const uint8_t* nv12, size_t pitch, size_t uv_off, size_t in_stride, uint8_t* bgr,
+                                                     int W, int H) {
+  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int hw = W / 2;
+  if (idx >= (long)hw * (H / 2)) return;
+  const int x = (int)(idx % hw) * 2, y = (int)(idx / hw) * 2;
+  const uint8_t* img = nv12 + (size_t)blockIdx.y * in_stride;
+  const uint8_t* uv = img + uv_off + (size_t)(y >> 1) * pitch + x;
+  const int u = uv[0], v = uv[1];
+  uint8_t* d = bgr + (size_t)blockIdx.y * ((size_t)W * H * 3) + ((size_t)y * W + x) * 3;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const uint8_t* yr = img + (size_t)(y + r) * pitch + x;
+    int p0[3], p1[3];
+    yuv_px_to_bgr(yr[0], u, v, p0); yuv_px_to_bgr(yr[1], u, v, p1);
+    uint8_t* o = d + (size_t)r * W * 3;
+    o[0] = (uint8_t)p0[0]; o[1] = (uint8_t)p0[1]; o[2] = (uint8_t)p0[2]; o[3] = (uint8_t)p1[0]; o[4] = (uint8_t)p1[1]; o[5] = (uint8_t)p1[2];
+  }
+}
+
+void launch_nv12_to_bgr(cudaStream_t s, int n, const uint8_t* nv12, size_t pitch, size_t uv_off, size_t in_stride, uint8_t* bgr, int W, int H) {
+  const long blocks = ((long)(W / 2) * (H / 2) + 255) / 256;
+  BSB_LAUNCH(k_nv12_to_bgr, dim3((unsigned)blocks, (unsigned)n), dim3(256), 0, s, nv12, pitch, uv_off, in_stride, bgr, W, H);
+  count_launch();
+}
+
+// Y bytes copied; the UV pair of a 2x2 block is the truncating average of the two rows' (byte 1, byte 3) of the YUYV pair
+__global__ void __launch_bounds__(256) k_yuyv_to_nv12(const uint8_t* yuyv, size_t yuyv_stride, uint8_t* nv12, size_t nv12_stride, int W, int H) {
+  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int hw = W / 2;
+  if (idx >= (long)hw * (H / 2)) return;
+  const int j = (int)(idx % hw), r = (int)(idx / hw);
+  const uint8_t* s0 = yuyv + (size_t)blockIdx.y * yuyv_stride + ((size_t)(2 * r) * W + 2 * j) * 2;
+  const uint8_t* s1 = s0 + (size_t)W * 2;
+  uint8_t* y0 = nv12 + (size_t)blockIdx.y * nv12_stride + (size_t)(2 * r) * W + 2 * j;
+  uint8_t* y1 = y0 + W;
+  y0[0] = s0[0]; y0[1] = s0[2]; y1[0] = s1[0]; y1[1] = s1[2];
+  uint8_t* uv = nv12 + (size_t)blockIdx.y * nv12_stride + (size_t)W * H + (size_t)r * W + 2 * j;
+  uv[0] = (uint8_t)((s0[1] + s1[1]) >> 1);
+  uv[1] = (uint8_t)((s0[3] + s1[3]) >> 1);
+}
+
+void launch_yuyv_to_nv12(cudaStream_t s, int n, const uint8_t* yuyv, size_t yuyv_stride, uint8_t* nv12, size_t nv12_stride, int W, int H) {
+  const long blocks = ((long)(W / 2) * (H / 2) + 255) / 256;
+  BSB_LAUNCH(k_yuyv_to_nv12, dim3((unsigned)blocks, (unsigned)n), dim3(256), 0, s, yuyv, yuyv_stride, nv12, nv12_stride, W, H);
   count_launch();
 }
 

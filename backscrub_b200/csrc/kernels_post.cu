@@ -17,6 +17,8 @@
 #include "kernels.h"
 #include "post_math.h"
 
+#include <type_traits>
+
 #ifndef BSB_EMU
 #include <cuda.h>   // CUtensorMap types only; cuTensorMapEncodeTiled is resolved at run time (no libcuda link)
 #endif
@@ -56,6 +58,11 @@ BSB_D void prefetch_map(const CUtensorMap* map) { asm volatile("prefetch.tensorm
 }  // namespace tma
 
 struct PostMaps { CUtensorMap frame, bg, bgy, out, yuyv, mask, ofinal; };
+// NV12 calls: frame / bgy / yuyv are the Y planes of the camera frames, the background NV12 and the NV12 output; these are
+// their UV planes
+struct PostMapsNv12 : PostMaps { CUtensorMap frame_uv, bgy_uv, yuyv_uv; };
+template <int FMT> using PostMapsOf = typename std::conditional<FMT == IN_NV12, PostMapsNv12, PostMaps>::type;
+// has_yuyv / has_bgy: a video output / a cached background in the call's video format (YUYV, NV12 for NV12 calls)
 struct PostTmaCfg { int has_out, has_yuyv, has_mask, has_bgy; };
 
 // Tile geometry.  A CTA owns one TW x 32 tile (TW = 64 or 128), one thread per 16 pixels of a row.
@@ -82,14 +89,20 @@ template <int TW> struct PtL {
   static constexpr int OFF_GEO = OFF_BAR + 32;                   // 12 ints of tile geometry / classification
   static constexpr int SMEM = OFF_GEO + 48;
   static constexpr int CTAS = TW == 128 ? 4 : 8;
+  // NV12 calls: the camera tile (Y TW x 32 | UV TW x 16) in the frame tile's place, the background NV12 tile in the YUYV
+  // tile's place, and the NV12 result tile staged over Hs / Vs (dead once the mask is computed)
+  static constexpr int N_BYTES = TW * PF_H * 3 / 2, OFF_N = OFF_HS;
+  static_assert(N_BYTES <= F_BYTES && N_BYTES <= Y_BYTES && N_BYTES <= HV_BYTES && OFF_N % 128 == 0, "NV12 staging");
   static_assert(PW % 16 == 0 && OFF_P % 128 == 0 && OFF_HS % 16 == 0 && OFF_US % 128 == 0 && OFF_ROWS % 16 == 0 && OFF_BAR % 8 == 0 &&
                 (PF_H - PT_RMAX) * US * 2 >= PF_UH * 16 && PF_UH * US * 2 >= M_BYTES && US % 8 == 0 && NT % 64 == 0 && NT >= PF_UH &&
                 (SMEM + 1024) * CTAS <= 228 * 1024, "smem layout");
 };
 
-template <bool IN_YUYV, int TW>
-__global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const __grid_constant__ PostMaps tm, const PostArgs a, const PostTmaCfg cfg) {
+// FMT: IN_BGR / IN_YUYV frames with YUYV video output, or IN_NV12 frames with NV12 video output
+template <int FMT, int TW>
+__global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const __grid_constant__ PostMapsOf<FMT> tm, const PostArgs a, const PostTmaCfg cfg) {
   using L = PtL<TW>;
+  constexpr bool IN_YUYV = FMT == InFmt::IN_YUYV, NV12 = FMT == InFmt::IN_NV12;
   constexpr int NT = L::NT, UW = L::UW, US = L::US, PW = L::PW;
   extern __shared__ __align__(128) unsigned char smem[];
   unsigned short* Hs = reinterpret_cast<unsigned short*>(smem + L::OFF_HS);
@@ -102,6 +115,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
   uint8_t* sY = smem + L::OFF_Y;          // YUYV tile [32][2 TW]: cached background YUYV in, result out
   uint8_t* sM = smem + L::OFF_US;         // mask tile [32][TW] (reuses Us, dead by then)
   uint8_t* sP = smem + L::OFF_P;          // source patch of the small mask [PT_RMAX][PW]
+  uint8_t* sN = smem + L::OFF_N;          // NV12 result tile: Y [32][TW] | UV [16][TW] (NV12 calls)
   uint64_t* barP = bars; uint64_t* barB = bars + 1; uint64_t* barF = bars + 2;
 
   const int b = blockIdx.z;
@@ -134,14 +148,27 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
     if (a.bg_index) bgi = __ldg(a.bg_index + b);
     else if (a.bg_cursor) bgi = (int)(((unsigned)__ldg(a.bg_cursor) + (unsigned)b * (unsigned)a.bg_advance) % (unsigned)a.bg_count);
     else if (a.bg_stride) bgi = b;
-    tma::mbar_expect_tx(barB, (unsigned)L::F_BYTES + (cfg.has_bgy ? (unsigned)L::Y_BYTES : 0u));
+    tma::mbar_expect_tx(barB, (unsigned)L::F_BYTES + (cfg.has_bgy ? (NV12 ? (unsigned)L::N_BYTES : (unsigned)L::Y_BYTES) : 0u));
     tma::load_3d(sB, &tm.bg, blockIdx.x * (TW * 3 / 4), ty0, bgi, barB);
-    if (cfg.has_bgy) tma::load_3d(sY, &tm.bgy, blockIdx.x * (TW / 2), ty0, bgi, barB);
+    if constexpr (NV12) {
+      if (cfg.has_bgy) {
+        tma::load_3d(sY, &tm.bgy, blockIdx.x * (TW / 4), ty0, bgi, barB);
+        tma::load_3d(sY + TW * PF_H, &tm.bgy_uv, blockIdx.x * (TW / 4), ty0 / 2, bgi, barB);
+      }
+    } else {
+      if (cfg.has_bgy) tma::load_3d(sY, &tm.bgy, blockIdx.x * (TW / 2), ty0, bgi, barB);
+    }
     // ... and the camera tile when the tile can contain a person at all: waiting for the classification first would put a
     // second memory round trip on the critical path of every person / mixed tile
     if (hit) {
-      tma::mbar_expect_tx(barF, IN_YUYV ? (unsigned)L::Y_BYTES : (unsigned)L::F_BYTES);
-      tma::load_3d(sF, &tm.frame, blockIdx.x * (IN_YUYV ? TW / 2 : TW * 3 / 4), ty0, b, barF);
+      if constexpr (NV12) {
+        tma::mbar_expect_tx(barF, (unsigned)L::N_BYTES);
+        tma::load_3d(sF, &tm.frame, blockIdx.x * (TW / 4), ty0, b, barF);
+        tma::load_3d(sF + TW * PF_H, &tm.frame_uv, blockIdx.x * (TW / 4), ty0 / 2, b, barF);   // ty0 is even (PF_H = 32)
+      } else {
+        tma::mbar_expect_tx(barF, IN_YUYV ? (unsigned)L::Y_BYTES : (unsigned)L::F_BYTES);
+        tma::load_3d(sF, &tm.frame, blockIdx.x * (IN_YUYV ? TW / 2 : TW * 3 / 4), ty0, b, barF);
+      }
     }
     const bool inside = tx0 >= a.roi_x && min(tx0 + TW, a.W) <= a.roi_x + a.roi_w && ty0 >= a.roi_y && min(ty0 + PF_H, a.H) <= a.roi_y + a.roi_h;
     *reinterpret_cast<int4*>(geo) = make_int4(hit ? 1 : 0, gy_lo, gx_lo, rmin);
@@ -277,7 +304,16 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
       post_mask16(a, row_in, tile_const, x0, Vs + ly * US + lx, m);
     }
     unsigned f[12], gg[12];
-    if (IN_YUYV) {
+    if (NV12) {
+      // the thread's 16 Y bytes and the 8 UV pairs of its row pair -> 8 (Y0 U Y1 V) words, then the YUYV arithmetic
+      const uint4 yq = *reinterpret_cast<const uint4*>(sF + ly * TW + lx);
+      const uint4 cq = *reinterpret_cast<const uint4*>(sF + TW * PF_H + (ly >> 1) * TW + lx);
+      const unsigned wa[4] = {__byte_perm(yq.x, cq.x, 0x5140), __byte_perm(yq.x, cq.x, 0x7362), __byte_perm(yq.y, cq.y, 0x5140),
+                              __byte_perm(yq.y, cq.y, 0x7362)};
+      const unsigned wb[4] = {__byte_perm(yq.z, cq.z, 0x5140), __byte_perm(yq.z, cq.z, 0x7362), __byte_perm(yq.w, cq.w, 0x5140),
+                              __byte_perm(yq.w, cq.w, 0x7362)};
+      yuyv8_to_bgr24(wa, f); yuyv8_to_bgr24(wb, f + 6);
+    } else if (IN_YUYV) {
       const uint4* fq = reinterpret_cast<const uint4*>(sF + ly * (TW * 2) + lx * 2);
       const uint4 w0 = fq[0], w1 = fq[1];
       const unsigned wa[4] = {w0.x, w0.y, w0.z, w0.w}, wb[4] = {w1.x, w1.y, w1.z, w1.w};
@@ -301,7 +337,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
     post_blend16<true, true>(f, gg, m, o, yy);
     // the YUYV camera tile is fully consumed before the (wider) BGR tile overwrites it; the mask staging tile reuses Us,
     // whose last readers (phase B) are behind a barrier already
-    if (IN_YUYV) __syncthreads();
+    if (IN_YUYV || NV12) __syncthreads();
     uint4* odst = reinterpret_cast<uint4*>(sF + ly * (TW * 3) + lx * 3);
     odst[0] = make_uint4(o[0], o[1], o[2], o[3]); odst[1] = make_uint4(o[4], o[5], o[6], o[7]); odst[2] = make_uint4(o[8], o[9], o[10], o[11]);
     ydst[0] = make_uint4(yy[0], yy[1], yy[2], yy[3]); ydst[1] = make_uint4(yy[4], yy[5], yy[6], yy[7]);
@@ -309,12 +345,35 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
                        m[8] | (m[9] << 8) | (m[10] << 16) | (m[11] << 24), m[12] | (m[13] << 8) | (m[14] << 16) | (m[15] << 24));
     out_src = sF;
   }
+  const uint8_t* nv_src = sY;          // NV12 calls: the tile the NV12 stores read (the cached background, else sN)
+  if constexpr (NV12) {
+    if (cfg.has_yuyv && !engine_only) {
+      // YUYV tile -> NV12: each thread takes 4 pairs of a row pair, copies the 8 + 8 Y bytes and averages the two rows'
+      // U / V bytes with a per-byte truncating halving add (the NV12 output definition)
+      __syncthreads();
+      const int r = tid / (TW / 8), q = tid % (TW / 8);
+      const uint4 a0 = *reinterpret_cast<const uint4*>(sY + (2 * r) * (TW * 2) + 16 * q);
+      const uint4 a1 = *reinterpret_cast<const uint4*>(sY + (2 * r + 1) * (TW * 2) + 16 * q);
+      *reinterpret_cast<uint2*>(sN + (2 * r) * TW + 8 * q) = make_uint2(__byte_perm(a0.x, a0.y, 0x6420), __byte_perm(a0.z, a0.w, 0x6420));
+      *reinterpret_cast<uint2*>(sN + (2 * r + 1) * TW + 8 * q) = make_uint2(__byte_perm(a1.x, a1.y, 0x6420), __byte_perm(a1.z, a1.w, 0x6420));
+      const unsigned h0 = __vhaddu4(a0.x, a1.x), h1 = __vhaddu4(a0.y, a1.y), h2 = __vhaddu4(a0.z, a1.z), h3 = __vhaddu4(a0.w, a1.w);
+      *reinterpret_cast<uint2*>(sN + TW * PF_H + r * TW + 8 * q) = make_uint2(__byte_perm(h0, h1, 0x7531), __byte_perm(h2, h3, 0x7531));
+      nv_src = sN;
+    }
+  }
   tma::fence_proxy_async();            // generic-proxy writes of the staging tiles -> visible to the TMA engine
   __syncthreads();
   if (tid == 0) {
     if (engine_only) tma::mbar_wait(barB, 0);
     if (cfg.has_out) tma::store_3d(&tm.out, out_src, blockIdx.x * (TW * 3 / 4), ty0, b);
-    if (cfg.has_yuyv) tma::store_3d(&tm.yuyv, sY, blockIdx.x * (TW / 2), ty0, b);
+    if constexpr (NV12) {
+      if (cfg.has_yuyv) {
+        tma::store_3d(&tm.yuyv, nv_src, blockIdx.x * (TW / 4), ty0, b);
+        tma::store_3d(&tm.yuyv_uv, nv_src + TW * PF_H, blockIdx.x * (TW / 4), ty0 / 2, b);
+      }
+    } else {
+      if (cfg.has_yuyv) tma::store_3d(&tm.yuyv, sY, blockIdx.x * (TW / 2), ty0, b);
+    }
     if (cfg.has_mask) tma::store_3d(&tm.mask, sM, tx0, ty0, b);
     tma::store_commit();
     if (hits_roi && kind == 0) tma::mbar_wait(barF, 0);
@@ -350,7 +409,7 @@ static bool make_map(CUtensorMap* m, const void* base, bool words, size_t row_by
              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-static bool build_post_maps(const PostArgs& a, PostMaps* tm, int TW) {
+static bool build_post_maps(const PostArgs& a, PostMaps* tm, int TW, PostMapsNv12* nv = nullptr) {
   const unsigned bw3 = (unsigned)TW * 3, bw2 = (unsigned)TW * 2, pw = TW == 128 ? (unsigned)PtL<128>::PW : (unsigned)PtL<64>::PW;
   const size_t W = (size_t)a.W, H = (size_t)a.H, B = (size_t)a.B;
   const size_t nbg = (a.bg_index || a.bg_cursor) ? (size_t)a.bg_count : (a.bg_stride ? B : 1);
@@ -364,6 +423,26 @@ static bool build_post_maps(const PostArgs& a, PostMaps* tm, int TW) {
   if (a.yuyv) ok = ok && make_map(&tm->yuyv, a.yuyv, true, W * 2, H, B, W * 2, a.yuyv_stride, bw2, PF_H); else tm->yuyv = tm->bg;
   if (a.mask) ok = ok && make_map(&tm->mask, a.mask, false, W, H, B, W, a.mask_stride, (unsigned)TW, PF_H); else tm->mask = tm->bg;
   ok = ok && make_map(&tm->ofinal, a.ofinal, false, (size_t)a.ow, (size_t)a.oh, B, (size_t)a.opitch, (size_t)a.opitch * a.oh, pw, PT_RMAX);
+  if (a.nv12_in) {
+    // NV12 calls: Y planes (TW x 32 boxes) in the frame / bgy / yuyv maps, UV planes (TW x 16 boxes, H / 2 rows) beside them
+    if (!nv) return false;
+    const unsigned bw = (unsigned)TW;
+    const size_t npix = W * H, nvb = npix * 3 / 2;
+    ok = ok && make_map(&tm->frame, a.nv12_in, true, W, H, B, a.nv12_in_pitch, a.nv12_in_stride, bw, PF_H);
+    ok = ok && make_map(&nv->frame_uv, a.nv12_in + a.nv12_in_uv, true, W, H / 2, B, a.nv12_in_pitch, a.nv12_in_stride, bw, PF_H / 2);
+    if (a.bg_nv12) {
+      ok = ok && make_map(&tm->bgy, a.bg_nv12, true, W, H, nbg, W, nvb, bw, PF_H);
+      ok = ok && make_map(&nv->bgy_uv, a.bg_nv12 + npix, true, W, H / 2, nbg, W, nvb, bw, PF_H / 2);
+    } else {
+      nv->bgy_uv = tm->bg;
+    }
+    if (a.nv12) {
+      ok = ok && make_map(&tm->yuyv, a.nv12, true, W, H, B, W, a.nv12_stride, bw, PF_H);
+      ok = ok && make_map(&nv->yuyv_uv, a.nv12 + npix, true, W, H / 2, B, W, a.nv12_stride, bw, PF_H / 2);
+    } else {
+      nv->yuyv_uv = tm->bg;
+    }
+  }
   return ok;
 }
 
@@ -379,13 +458,20 @@ static bool post_tma_shape_ok(const PostArgs& a) {
   if (!tuning().post_tma || !encode_fn()) return false;
   auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
   if (a.B < 1 || a.W % 16 != 0 || a.area2x2 || a.tab.xcol == nullptr || a.geo_rows == nullptr) return false;
+  if (a.nv12_in) {
+    if (!al16(a.nv12_in) || a.nv12_in_pitch % 16 || a.nv12_in_uv % 16 || a.nv12_in_stride % 16 || (a.H & 1) || a.yuyv || a.bg_yuyv) return false;
+    if (a.nv12 && (!al16(a.nv12) || a.nv12_stride % 16)) return false;
+    if (a.bg_nv12 && !al16(a.bg_nv12)) return false;
+  } else if (a.nv12 || a.bg_nv12) {
+    return false;
+  }
   if (a.yuyv_in) { if (!al16(a.yuyv_in) || a.yuyv_in_stride % 16) return false; }
-  else if (!al16(a.frames) || a.frame_pitch % 16 || a.frame_stride % 16) return false;
+  else if (!a.nv12_in && (!al16(a.frames) || a.frame_pitch % 16 || a.frame_stride % 16)) return false;
   if (!al16(a.bg) || a.bg_pitch % 16 || a.bg_stride % 16 || (a.bg_yuyv && !al16(a.bg_yuyv))) return false;
   if (a.out && (!al16(a.out) || a.out_pitch % 16 || a.out_stride % 16)) return false;
   if (a.yuyv && (!al16(a.yuyv) || a.yuyv_stride % 16)) return false;
   if (a.mask && (!al16(a.mask) || a.mask_stride % 16)) return false;
-  if (!(a.out || a.yuyv || a.mask) || !al16(a.ofinal) || a.opitch % 16) return false;
+  if (!(a.out || a.yuyv || a.nv12 || a.mask) || !al16(a.ofinal) || a.opitch % 16) return false;
   if (a.ow > 32000 || a.oh > 32000 || a.roi_w < 8 || a.roi_h < 8) return false;
   const double scale_y = (double)a.out_h / (double)a.roi_h, scale_x = (double)a.out_w / (double)a.roi_w;
   const int tw = post_tile_width(a);
@@ -394,27 +480,29 @@ static bool post_tma_shape_ok(const PostArgs& a) {
 }
 
 bool post_tma_eligible(const PostArgs& a) {
-  PostMaps tm;
-  return post_tma_shape_ok(a) && build_post_maps(a, &tm, post_tile_width(a));
+  PostMapsNv12 tm;
+  return post_tma_shape_ok(a) && build_post_maps(a, &tm, post_tile_width(a), &tm);
 }
 
-template <bool IN_YUYV, int TW>
-static bool launch_post_tma_t(cudaStream_t s, const PostMaps& tm, const PostArgs& a, const PostTmaCfg& cfg) {
+template <int FMT, int TW>
+static bool launch_post_tma_t(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
   using L = PtL<TW>;
-  if (!ensure_dyn_smem(reinterpret_cast<const void*>(k_post_tma<IN_YUYV, TW>), L::SMEM)) return false;
+  if (!ensure_dyn_smem(reinterpret_cast<const void*>(k_post_tma<FMT, TW>), L::SMEM)) return false;
   const dim3 grid((unsigned)ceil_div(a.W, TW), (unsigned)ceil_div(a.H, PF_H), (unsigned)a.B);
-  k_post_tma<IN_YUYV, TW><<<grid, L::NT, L::SMEM, s>>>(tm, a, cfg);
+  k_post_tma<FMT, TW><<<grid, L::NT, L::SMEM, s>>>(tm, a, cfg);
   return true;
 }
 
 bool launch_post_tma(cudaStream_t s, const PostArgs& a) {
-  PostMaps tm;
+  PostMapsNv12 tm;
   const int tw = post_tile_width(a);
-  if (!post_tma_shape_ok(a) || !build_post_maps(a, &tm, tw)) return false;
-  const PostTmaCfg cfg{a.out ? 1 : 0, a.yuyv ? 1 : 0, a.mask ? 1 : 0, a.bg_yuyv ? 1 : 0};
+  if (!post_tma_shape_ok(a) || !build_post_maps(a, &tm, tw, &tm)) return false;
+  const PostTmaCfg cfg{a.out ? 1 : 0, (a.yuyv || a.nv12) ? 1 : 0, a.mask ? 1 : 0, (a.bg_yuyv || a.bg_nv12) ? 1 : 0};
+  const PostMaps& pm = tm;
   bool ok;
-  if (a.yuyv_in) ok = tw == 128 ? launch_post_tma_t<true, 128>(s, tm, a, cfg) : launch_post_tma_t<true, 64>(s, tm, a, cfg);
-  else ok = tw == 128 ? launch_post_tma_t<false, 128>(s, tm, a, cfg) : launch_post_tma_t<false, 64>(s, tm, a, cfg);
+  if (a.nv12_in) ok = tw == 128 ? launch_post_tma_t<IN_NV12, 128>(s, tm, a, cfg) : launch_post_tma_t<IN_NV12, 64>(s, tm, a, cfg);
+  else if (a.yuyv_in) ok = tw == 128 ? launch_post_tma_t<IN_YUYV, 128>(s, pm, a, cfg) : launch_post_tma_t<IN_YUYV, 64>(s, pm, a, cfg);
+  else ok = tw == 128 ? launch_post_tma_t<IN_BGR, 128>(s, pm, a, cfg) : launch_post_tma_t<IN_BGR, 64>(s, pm, a, cfg);
   if (ok) count_launch();
   return ok;
 }

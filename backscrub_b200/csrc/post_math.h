@@ -79,14 +79,24 @@ BSB_D void yuyv8_to_bgr24(const unsigned* w, unsigned* o) {
     o[3 * q + 2] = __byte_perm(p2, p3, 0x6542);      // r2 b3 g3 r3
   }
 }
-// one pixel of a YUYV row: BGR of pixel x (the pair's U / V are shared)
-BSB_D void yuyv_px_to_bgr(const uint8_t* row, int x, int* bgr) {
-  const uint8_t* q = row + (size_t)(x & ~1) * 2;
-  const int u = (int)q[1] - 128, v = (int)q[3] - 128;
-  const int yy = max((int)q[(x & 1) * 2] - 16, 0) * 1220542;
+// one pixel from its Y byte and the U / V bytes it shares (the arithmetic of yuyv8_to_bgr24)
+BSB_D void yuv_px_to_bgr(int y, int u8, int v8, int* bgr) {
+  const int u = u8 - 128, v = v8 - 128;
+  const int yy = max(y - 16, 0) * 1220542;
   bgr[0] = bsb_sat_u8((yy + (1 << 19) + 2116026 * u) >> 20);
   bgr[1] = bsb_sat_u8((yy + (1 << 19) - 852492 * v - 409993 * u) >> 20);
   bgr[2] = bsb_sat_u8((yy + (1 << 19) + 1673527 * v) >> 20);
+}
+// one pixel of a YUYV row: BGR of pixel x (the pair's U / V are shared)
+BSB_D void yuyv_px_to_bgr(const uint8_t* row, int x, int* bgr) {
+  const uint8_t* q = row + (size_t)(x & ~1) * 2;
+  yuv_px_to_bgr((int)q[(x & 1) * 2], (int)q[1], (int)q[3], bgr);
+}
+// one pixel of an NV12 frame (Y plane rows `pitch` bytes apart, UV plane at byte `uv_off`): pixel (x, y) takes the UV pair
+// of its 2x2 block.  cv::cvtColor(COLOR_YUV2BGR_NV12) equals COLOR_YUV2BGR_YUYV on the YUYV frame built that way.
+BSB_D void nv12_px_to_bgr(const uint8_t* img, size_t pitch, size_t uv_off, int x, int y, int* bgr) {
+  const uint8_t* q = img + uv_off + (size_t)(y >> 1) * pitch + (size_t)(x & ~1);
+  yuv_px_to_bgr((int)img[(size_t)y * pitch + x], (int)q[0], (int)q[1], bgr);
 }
 
 // 16 mask values of one thread from the vertical 5-sums `vrow` (packed u16, the thread's first column), or from the

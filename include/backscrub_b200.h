@@ -148,6 +148,32 @@ BSB_API int bsb_composite_yuyv_device(bsb_ctx* ctx, int n_frames, const uint8_t*
                                       uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv, size_t yuyv_stride,
                                       uint8_t* d_mask, size_t mask_stride, int sync);
 
+/* ---- NV12 camera frames in, NV12 composites out ------------------------------------------
+ * NV12 (8-bit 4:2:0, what hardware video decoders produce and encoders take): a Y plane of H rows, then an interleaved UV
+ * plane of H/2 rows of W/2 (U, V) byte pairs.  Frames have an even width and height.
+ * Ingest is cv::cvtColor(COLOR_YUV2BGR_NV12), which equals COLOR_YUV2BGR_YUYV on the YUYV frame built from the same Y
+ * plane and, for each pixel, the UV pair of its 2x2 block: the arithmetic of the YUYV ingest.
+ * Output is derived from the YUYV output (convert_rgb_to_yuyv, app/deepseg.cc:87-106) of the out_w x out_h composite
+ * (both even), by byte position:
+ *   Y[y][x]          = the Y byte of pixel x in row y of the YUYV output,
+ *   UV[r][2j]        = (yuyv[2r][4j+1] + yuyv[2r+1][4j+1]) >> 1,
+ *   UV[r][2j+1]      = (yuyv[2r][4j+3] + yuyv[2r+1][4j+3]) >> 1   (yuyv[row][byte]),
+ * the reference's truncating pair average applied vertically.  The reference's "RGB2YUV" runs on BGR data, so its
+ * channel names are swapped; keeping byte positions gives a consumer the colours of the YUYV output.
+ * DEVICE pointers.  Input: row pitch `in_pitch` >= W, the UV plane at byte `uv_offset` >= in_pitch*H of each frame (the
+ * pitched surfaces of a hardware decoder need no copy), `in_stride` bytes per frame.  The NV12 output is tightly packed
+ * (W-byte rows, UV plane at byte out_w*out_h), `nv12_stride` bytes per frame.  Any of d_out / d_nv12_out / d_mask may be
+ * NULL.  Asynchronous on the context's stream unless `sync`.  A violated rule (odd W or H, odd out_w / out_h with an NV12
+ * output, in_pitch < W, uv_offset < in_pitch*H, a frame larger than in_stride, NULL frames, n_frames out of range)
+ * returns 0 with a bsb_last_error() message and leaves the context usable. */
+BSB_API int bsb_composite_nv12_device(bsb_ctx* ctx, int n_frames, const uint8_t* d_nv12, size_t in_pitch, size_t uv_offset, size_t in_stride,
+                                      uint8_t* d_out, size_t out_stride, uint8_t* d_nv12_out, size_t nv12_stride,
+                                      uint8_t* d_mask, size_t mask_stride, int sync);
+/* HOST buffers, tightly packed NV12 frames (W-byte rows, UV plane at W*H), `in_stride` bytes per frame; one serial
+ * copy in -> graph -> copy out. */
+BSB_API int bsb_composite_nv12(bsb_ctx* ctx, int n_frames, const uint8_t* nv12, size_t in_stride, uint8_t* out, size_t out_stride,
+                               uint8_t* nv12_out, size_t nv12_stride, uint8_t* out_mask, size_t mask_stride);
+
 /* ---- independent sources: one frame from each of several cameras in one launch ----------
  * A "source" is one camera stream with its own temporal smoother state (what one
  * bs_maskgen_new context holds in the reference, lib/libbackscrub.cc:161-259).  A sources call
@@ -179,6 +205,10 @@ BSB_API int bsb_composite_sources(bsb_ctx* ctx, int n_frames, const int* source_
 BSB_API int bsb_composite_sources_yuyv_device(bsb_ctx* ctx, int n_frames, const int* source_ids, const uint8_t* d_yuyv_frames,
                                               uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv, size_t yuyv_stride,
                                               uint8_t* d_mask, size_t mask_stride, int sync);
+/* DEVICE pointers, camera NV12 frames and NV12 output, laid out as in bsb_composite_nv12_device. */
+BSB_API int bsb_composite_sources_nv12_device(bsb_ctx* ctx, int n_frames, const int* source_ids, const uint8_t* d_nv12, size_t in_pitch,
+                                              size_t uv_offset, size_t in_stride, uint8_t* d_out, size_t out_stride,
+                                              uint8_t* d_nv12_out, size_t nv12_stride, uint8_t* d_mask, size_t mask_stride, int sync);
 /* ---- asynchronous mask front-end: the reference's CalcMask (app/deepseg.cc:159-286) ----
  * A worker thread owns the mask-generation context.  set_input_frame clones the frame and wakes the worker (a
  * frame that arrives while the worker is busy replaces the pending one: latest frame wins); get_output_mask copies
@@ -232,6 +262,8 @@ BSB_API int bsb_alpha_blend(int device, const uint8_t* srca, const uint8_t* srcb
 BSB_API int bsb_convert_rgb_to_yuyv(int device, const uint8_t* rgb, uint8_t* yuyv, int width, int height);
 /* cv::cvtColor(COLOR_YUV2BGR_YUYV) (camera ingest, app/deepseg.cc:553,725) */
 BSB_API int bsb_convert_yuyv_to_bgr(int device, const uint8_t* yuyv, uint8_t* bgr, int width, int height);
+/* cv::cvtColor(COLOR_YUV2BGR_NV12), tightly packed NV12 (width, height even) */
+BSB_API int bsb_convert_nv12_to_bgr(int device, const uint8_t* nv12, uint8_t* bgr, int width, int height);
 /* cv::GaussianBlur(src, dst, Size(k,k), 0) 8UC3 (app/deepseg.cc:657-658) and its 8.8 fixed-point taps (host only) */
 BSB_API int bsb_gaussian_blur(int device, const uint8_t* src, uint8_t* dst, int width, int height, int ksize);
 BSB_API int bsb_gaussian_taps(int ksize, int* taps);
@@ -275,8 +307,9 @@ BSB_API long bsb_total_launches(void);
  * 3 = post (mask upsample + blur + blend + YUYV), 4 = whole call.  Returns < 0 on error.
  * Measurement aid for bench.py's roofline block; it advances the IIR state. */
 BSB_API double bsb_time_stage(bsb_ctx* ctx, int stage, int n_frames, int iters);
-/* 1 if the last fused call read camera YUYV frames in place (pre-processing and post kernels convert per tap / per tile),
- * 0 if a BGR frame was materialised first (k_yuyv_to_bgr) or the input was BGR */
+/* 1 if the last fused call read the camera frames in their wire format (YUYV or NV12) in place (pre-processing and post
+ * kernels convert per tap / per tile), 0 if a BGR frame was materialised first (k_yuyv_to_bgr / k_nv12_to_bgr) or the
+ * input was BGR */
 BSB_API int bsb_yuyv_native(bsb_ctx* ctx);
 /* 1 if at least one 1x1 conv of this context runs on the tensor cores */
 BSB_API int bsb_uses_tensor_cores(bsb_ctx* ctx);
