@@ -262,6 +262,16 @@ class MaskGen:
         if not ok:
             self._fail("bsb_set_source_background")
 
+    def set_source_effect(self, source: int, background: str = "default", bgblur: int = -1):
+        """background effect of one source: background "default" (its own image, else the context's) or "none" (no
+        image: the blurred camera frame when the strength is > 0, else green); bgblur -1 = follow set_bgblur, 0 = off,
+        odd 1..255."""
+        kinds = {"default": 0, "none": 1}
+        if background not in kinds:
+            raise BackscrubError(f"bsb_set_source_effect: unknown background {background!r} (\"default\" or \"none\")")
+        if not self._lib.bsb_set_source_effect(self._h, int(source), kinds[background], int(bgblur)):
+            self._fail("bsb_set_source_effect")
+
     def composite_sources(self, frames: np.ndarray, ids, want_out=True, want_yuyv=True, want_mask=True):
         """HOST buffers: frames [n, H, W, 3], frame b the next frame of source ids[b] (distinct ids) -> (out, yuyv, mask)."""
         frames = np.ascontiguousarray(frames, np.uint8)

@@ -502,6 +502,13 @@ int bsb_set_source_background(bsb_ctx* ctx, int source, const uint8_t* bg_raw, i
   return 1;
 }
 
+int bsb_set_source_effect(bsb_ctx* ctx, int source, int background, int bgblur) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_source_effect(source, background, bgblur, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
 int bsb_composite_sources(bsb_ctx* ctx, int n, const int* source_ids, const uint8_t* frames, size_t frame_pitch, size_t frame_stride,
                           uint8_t* out, size_t out_stride, uint8_t* out_yuyv, size_t yuyv_stride, uint8_t* out_mask, size_t mask_stride) {
   if (!check_ctx(ctx)) return 0;
@@ -669,7 +676,11 @@ int bsb_gaussian_blur(int device, const uint8_t* src, uint8_t* dst, int width, i
   DevBuf a, o, tmp;
   if (!a.alloc(nb) || !o.alloc(nb) || !tmp.alloc(nb * 2)) { g_last_error = "cudaMalloc failed"; return 0; }
   cudaMemcpy(a.p, src, nb, cudaMemcpyHostToDevice);
-  bsb::launch_gauss_blur(nullptr, 1, a.u8(), (size_t)width * 3, nb, static_cast<uint16_t*>(tmp.p), o.u8(), (size_t)width * 3, nb, width, height, t);
+  if (!bsb::launch_gauss_blur(nullptr, 1, a.u8(), (size_t)width * 3, nb, static_cast<uint16_t*>(tmp.p), o.u8(), (size_t)width * 3, nb, width,
+                              height, t)) {
+    g_last_error = "could not allocate the Gaussian tap tables";
+    return 0;
+  }
   if (!stage_end()) return 0;
   cudaMemcpy(dst, o.p, nb, cudaMemcpyDeviceToHost);
   return 1;

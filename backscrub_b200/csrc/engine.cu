@@ -919,6 +919,8 @@ bool Engine::upload(std::string* err) {
     CUDA_OK(cudaMemcpy(d_tile_geo_, geo.data(), geo.size() * sizeof(int2), cudaMemcpyHostToDevice));
   }
   if (!refresh_bg_yuyv(err)) return false;
+  // the Gaussian's tap tables must exist before a launch is captured into a graph
+  if (!gauss_tables_ready()) { *err = "could not allocate the Gaussian tap tables"; return false; }
   CUDA_OK(cudaDeviceSynchronize());
   return true;
 }
@@ -1196,12 +1198,14 @@ PostArgs Engine::post_args(int n, const uint8_t* d_frames, size_t pitch, size_t 
   }
   if (bg_yuyv_valid_ && !(bgblur_k_ && !has_bg_)) { a.bg_yuyv = d_bg_yuyv_; a.bg_nv12 = bg_nv12_valid_ ? d_bg_nv12_ : nullptr; }
   if (call_mode_ != CALL_PLAIN) {
-    // sources: frame b blends bank slot bg_index[b]; the bank's YUYV holds no camera-blur slots, so a call with such a
-    // frame converts every tile (what a plain context in camera-blur mode does)
+    // sources: frame b blends bank slot bg_index[b]; the camera-blur slots' YUYV / NV12 are written by the call's
+    // Gaussian, so every slot's cached copy is valid.  A call whose every frame is camera blur runs without them, as a
+    // plain context in camera-blur mode does: each slot is read by one tile only, and converting the blurred BGR tile
+    // the kernel loads anyway is cheaper than writing and re-reading a YUYV copy.
     a.bg = d_bank_; a.bg_stride = fbytes; a.bg_cursor = nullptr; a.bg_advance = 0;
     a.bg_index = d_src_tab_ + max_batch_; a.bg_count = bank_slots();
-    a.bg_yuyv = (call_mode_ == CALL_SOURCES && !(W_ & 1)) ? d_bank_yuyv_ : nullptr;
-    a.bg_nv12 = call_mode_ == CALL_SOURCES ? d_bank_nv12_ : nullptr;
+    a.bg_yuyv = (!call_all_blur_ && !(W_ & 1)) ? d_bank_yuyv_ : nullptr;
+    a.bg_nv12 = call_all_blur_ ? nullptr : d_bank_nv12_;
   }
   // the cached background in the call's video format (NV12 where the kernel writes NV12, else YUYV)
   if (nv12_in) a.bg_yuyv = nullptr; else a.bg_nv12 = nullptr;
@@ -1229,11 +1233,21 @@ void Engine::enqueue_post(int n, const uint8_t* d_frames, size_t pitch, size_t s
   const bool flip = flip_h_ || flip_v_, resized = out_w_ != W_ || out_h_ != H_, tail = flip || resized;
   const bool want_rgb = d_out || d_yuyv;
   const bool ring = call_mode_ == CALL_PLAIN && has_bg_ && bg_count_ > 1;
-  // app/deepseg.cc:652-658: no background source => the background is the blurred camera frame itself (sources: into the
-  // bank's camera-blur slots, slot b = frame b)
-  if (call_mode_ == CALL_SOURCES_CAMBLUR && want_rgb)
-    launch_gauss_blur(stream_, n, d_frames, pitch, stride, d_gauss_tmp_, d_bank_, (size_t)W_ * 3, fbytes, W_, H_, taps_);
-  else if (call_mode_ == CALL_PLAIN && !has_bg_ && bgblur_k_ && want_rgb)
+  // app/deepseg.cc:652-658: no background source => the background is the blurred camera frame itself (sources: frame b
+  // at its own strength into the bank's camera-blur slot b, with the slot's YUYV / NV12; the camera frame is read in
+  // its wire format when the post kernel reads it so)
+  if (call_mode_ == CALL_SOURCES_CAMBLUR && want_rgb) {
+    // the slots' cached video format is the one the post kernel copies: NV12 when it reads the NV12 frames in place, else
+    // YUYV (also for an NV12 call that falls back to BGR frames)
+    const bool nv12_in = nv12_.on && d_yuyv_in;
+    GaussSrc cam{};
+    if (nv12_in) cam = GaussSrc{d_yuyv_in, nv12_.pitch, nv12_.stride, nv12_.uv, IN_NV12};
+    else if (d_yuyv_in) cam = GaussSrc{d_yuyv_in, (size_t)W_ * 2, (size_t)W_ * H_ * 2, 0, IN_YUYV};
+    uint8_t* yv = (!call_all_blur_ && !nv12_in && !(W_ & 1)) ? d_bank_yuyv_ : nullptr;
+    uint8_t* nv = (!call_all_blur_ && nv12_in) ? d_bank_nv12_ : nullptr;
+    launch_gauss_frames(stream_, n, cam, d_src_tab_ + 2 * (size_t)max_batch_, call_gclass_, const_cast<uint8_t*>(d_frames), d_gauss_tmp_,
+                        d_bank_, yv, nv, W_, H_);
+  } else if (call_mode_ == CALL_PLAIN && !has_bg_ && bgblur_k_ && want_rgb)
     launch_gauss_blur(stream_, n, d_frames, pitch, stride, d_gauss_tmp_, d_bg_frames_, (size_t)W_ * 3, fbytes, W_, H_, taps_);
   const PostArgs a = post_args(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in);
   launch_post(stream_, a);
@@ -1259,10 +1273,13 @@ void Engine::enqueue_post(int n, const uint8_t* d_frames, size_t pitch, size_t s
 
 // Camera YUYV / NV12 input: the pre-processing kernel always reads the frames in place; the BGR frame is materialised
 // (k_yuyv_to_bgr / k_nv12_to_bgr into `d_frames`) only when the post stage cannot read the wire format itself — no TMA
-// path for this geometry or layout, or the blur-my-background mode, whose Gaussian runs on the BGR frame.
+// path for this geometry or layout, or the blur-my-background mode of plain calls, whose Gaussian runs on the BGR frame
+// (a sources call's Gaussian reads the wire format itself).
 bool Engine::yuyv_native(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
                          uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in) const {
-  const bool camblur = call_mode_ == CALL_PLAIN ? (bgblur_k_ && !has_bg_) : call_mode_ == CALL_SOURCES_CAMBLUR;
+  // a sources call whose every frame blurs its camera frame converts every frame to BGR for the Gaussian anyway, and the
+  // post kernel reads BGR frames faster than it converts the wire format
+  const bool camblur = call_mode_ == CALL_PLAIN ? (bgblur_k_ && !has_bg_) : call_all_blur_;
   if (!d_yuyv_in || camblur) return false;
   return post_tma_eligible(post_args(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in));
 }
@@ -1312,7 +1329,7 @@ bool Engine::run(int n, const uint8_t* d_frames, size_t pitch, size_t stride, ui
   }
 #ifndef BSB_EMU
   const GraphKey key{n, d_frames, pitch, stride, d_out, d_yuyv, d_mask, d_yuyv_in, d_out ? out_stride : 0, d_yuyv ? yuyv_stride : 0,
-                     d_mask ? mask_stride : 0, call_mode_, nv12_.on, nv12_.pitch, nv12_.uv, nv12_.stride};
+                     d_mask ? mask_stride : 0, call_mode_, call_gclass_, call_all_blur_, nv12_.on, nv12_.pitch, nv12_.uv, nv12_.stride};
   auto it = graphs_.find(key);
   if (it == graphs_.end()) {
     if (graphs_.size() >= 64) drop_graphs();
@@ -1423,6 +1440,7 @@ bool Engine::set_background_ring(const uint8_t* frames, int count, int bw, int b
   if (!refresh_bg_blur(err)) return false;
   if (!refresh_bg_yuyv(err)) return false;
   if (!refresh_bank_ctx(err)) return false;
+  if (!refresh_bank_sources_after_ctx(err)) return false;
   CUDA_OK(cudaStreamSynchronize(stream_));
   CUDA_OK(cudaGetLastError());
   return true;
@@ -1483,8 +1501,7 @@ bool Engine::set_bgblur(int k, std::string* err) {
   if (!refresh_bg_blur(err)) return false;
   if (!refresh_bg_yuyv(err)) return false;
   if (!refresh_bank_ctx(err)) return false;
-  for (int s = 0; s < n_sources_; ++s)
-    if (!refresh_bank_source(s, err)) return false;
+  if (!refresh_bank_sources_after_ctx(err)) return false;
   CUDA_OK(cudaStreamSynchronize(stream_));
   return true;
 }
@@ -1529,10 +1546,11 @@ bool Engine::reset_state(std::string* err) {
 // independent sources
 // ---------------------------------------------------------------------------
 void Engine::free_sources() {
-  for (void* p : {(void*)src_state_, (void*)d_bank_, (void*)d_bank_yuyv_, (void*)d_bank_nv12_, (void*)d_src_bg_}) if (p) cudaFree(p);
-  src_state_ = nullptr; d_bank_ = nullptr; d_bank_yuyv_ = nullptr; d_bank_nv12_ = nullptr; d_src_bg_ = nullptr;
+  for (void* p : {(void*)src_state_, (void*)d_bank_, (void*)d_bank_yuyv_, (void*)d_bank_nv12_, (void*)d_src_bg_, (void*)d_green_}) if (p) cudaFree(p);
+  src_state_ = nullptr; d_bank_ = nullptr; d_bank_yuyv_ = nullptr; d_bank_nv12_ = nullptr; d_src_bg_ = nullptr; d_green_ = nullptr;
   n_sources_ = 0;
   src_has_bg_.clear();
+  src_fx_.clear();
 }
 
 bool Engine::set_sources(int n_sources, std::string* err) {
@@ -1544,8 +1562,8 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   const size_t fbytes = (size_t)W_ * H_ * 3, npix = (size_t)W_ * H_, opx = (size_t)oh_ * ow_;
   const size_t slots = (size_t)max_batch_ + 1 + (size_t)n_sources;
   if (!d_src_tab_) {
-    CUDA_OK(cudaMalloc((void**)&d_src_tab_, 2 * (size_t)max_batch_ * sizeof(int)));
-    CUDA_OK(cudaMemset(d_src_tab_, 0, 2 * (size_t)max_batch_ * sizeof(int)));
+    CUDA_OK(cudaMalloc((void**)&d_src_tab_, 3 * (size_t)max_batch_ * sizeof(int)));
+    CUDA_OK(cudaMemset(d_src_tab_, 0, 3 * (size_t)max_batch_ * sizeof(int)));
   }
   CUDA_OK(cudaMalloc((void**)&src_state_, (size_t)n_sources * opx));
   CUDA_OK(cudaMemset(src_state_, 0, (size_t)n_sources * opx));
@@ -1560,8 +1578,15 @@ bool Engine::set_sources(int n_sources, std::string* err) {
     }
   }
   CUDA_OK(cudaMalloc((void**)&d_src_bg_, (size_t)n_sources * fbytes));
+  {
+    std::vector<uint8_t> green(fbytes);
+    for (size_t i = 0; i < npix; ++i) { green[3 * i] = 0; green[3 * i + 1] = 255; green[3 * i + 2] = 0; }
+    CUDA_OK(cudaMalloc((void**)&d_green_, fbytes));
+    CUDA_OK(cudaMemcpy(d_green_, green.data(), fbytes, cudaMemcpyHostToDevice));
+  }
   n_sources_ = n_sources;
   src_has_bg_.assign((size_t)n_sources, 0);
+  src_fx_.assign((size_t)n_sources, SrcEffect{});
   if (!refresh_bank_ctx(err)) return false;
   CUDA_OK(cudaStreamSynchronize(stream_));
   return true;
@@ -1590,16 +1615,67 @@ bool Engine::refresh_bank_ctx(std::string* err) {
   return true;
 }
 
-// bank slot of source s from its resized background: blurred once when bgblur is on, then its YUYV
+int Engine::source_bg(int s, int* k) const {
+  const SrcEffect& f = src_fx_[s];
+  *k = f.k < 0 ? bgblur_k_ : f.k;
+  if (f.bg == SRC_BG_DEFAULT && src_has_bg_[s]) return SRC_FROM_SLOT;                          // its own image, blurred with k
+  if (f.bg == SRC_BG_DEFAULT && has_bg_) return *k == bgblur_k_ ? SRC_FROM_CTX : SRC_FROM_SLOT;  // the context image at k
+  if (*k) return SRC_FROM_CAMBLUR;                                                            // no image: its blurred camera frame
+  return has_bg_ ? SRC_FROM_SLOT : SRC_FROM_CTX;         // green (the context slot is green while there is no context image)
+}
+
+// d_gauss_tmp_ (16-bit row sums of the row / column Gaussian) for max_batch frames
+bool Engine::ensure_gauss_tmp(std::string* err) {
+  return ensure((void**)&d_gauss_tmp_, &gauss_tmp_cap_, (size_t)max_batch_ * W_ * H_ * 3 * sizeof(uint16_t), err);
+}
+
+// bank slot of source s when its still background differs from the context slot: its own image, the context image or
+// green, blurred with the source's strength; then its YUYV / NV12
 bool Engine::refresh_bank_source(int s, std::string* err) {
-  if (!src_has_bg_[s]) return true;
-  const size_t fbytes = (size_t)W_ * H_ * 3, npix = (size_t)W_ * H_, k = (size_t)max_batch_ + 1 + (size_t)s;
-  const uint8_t* src = d_src_bg_ + (size_t)s * fbytes;
-  uint8_t* slot = d_bank_ + k * fbytes;
-  if (bgblur_k_) launch_gauss_blur(stream_, 1, src, (size_t)W_ * 3, fbytes, d_gauss_tmp_, slot, (size_t)W_ * 3, fbytes, W_, H_, taps_);
-  else CUDA_OK(cudaMemcpyAsync(slot, src, fbytes, cudaMemcpyDeviceToDevice, stream_));
-  if (d_bank_yuyv_) launch_rgb_to_yuyv(stream_, slot, d_bank_yuyv_ + k * npix * 2, npix);
-  if (d_bank_nv12_) launch_yuyv_to_nv12(stream_, 1, d_bank_yuyv_ + k * npix * 2, 0, d_bank_nv12_ + k * npix * 3 / 2, 0, W_, H_);
+  int k = 0;
+  if (source_bg(s, &k) != SRC_FROM_SLOT) return true;
+  const SrcEffect& f = src_fx_[s];
+  const size_t fbytes = (size_t)W_ * H_ * 3, npix = (size_t)W_ * H_, slot_i = (size_t)max_batch_ + 1 + (size_t)s;
+  const uint8_t* src = f.bg != SRC_BG_DEFAULT ? d_green_ : src_has_bg_[s] ? d_src_bg_ + (size_t)s * fbytes : has_bg_ ? d_bg_ : d_green_;
+  uint8_t* slot = d_bank_ + slot_i * fbytes;
+  if (k) {
+    GaussTaps t{};
+    gauss_taps(k, &t);
+    if (gauss_class(k) == GAUSS_SEPARABLE && !ensure_gauss_tmp(err)) return false;
+    launch_gauss_blur(stream_, 1, src, (size_t)W_ * 3, fbytes, d_gauss_tmp_, slot, (size_t)W_ * 3, fbytes, W_, H_, t);
+  } else {
+    CUDA_OK(cudaMemcpyAsync(slot, src, fbytes, cudaMemcpyDeviceToDevice, stream_));
+  }
+  if (d_bank_yuyv_) launch_rgb_to_yuyv(stream_, slot, d_bank_yuyv_ + slot_i * npix * 2, npix);
+  if (d_bank_nv12_) launch_yuyv_to_nv12(stream_, 1, d_bank_yuyv_ + slot_i * npix * 2, 0, d_bank_nv12_ + slot_i * npix * 3 / 2, 0, W_, H_);
+  CUDA_OK(cudaGetLastError());
+  return true;
+}
+
+// after a new context background or strength: every source slot except an own image at a fixed strength depends on them
+// (one Gaussian per such source with a strength > 0)
+bool Engine::refresh_bank_sources_after_ctx(std::string* err) {
+  for (int s = 0; s < n_sources_; ++s) {
+    const SrcEffect& f = src_fx_[s];
+    if (f.bg == SRC_BG_DEFAULT && src_has_bg_[s] && f.k >= 0) continue;
+    if (!refresh_bank_source(s, err)) return false;
+  }
+  return true;
+}
+
+bool Engine::set_source_effect(int source, int background, int bgblur, std::string* err) {
+  if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
+  if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
+  if (background != SRC_BG_DEFAULT && background != SRC_BG_NONE) {
+    *err = "unknown source background (BSB_SOURCE_BG_DEFAULT or BSB_SOURCE_BG_NONE)"; return false;
+  }
+  if (bgblur < -1 || bgblur > 255 || (bgblur > 0 && !(bgblur & 1))) {
+    *err = "source strength must be -1 (follow the context), 0 (off) or odd 1..255"; return false;
+  }
+  CUDA_OK(cudaSetDevice(device_));
+  src_fx_[source] = SrcEffect{background, bgblur};
+  if (!refresh_bank_source(source, err)) return false;
+  CUDA_OK(cudaStreamSynchronize(stream_));
   CUDA_OK(cudaGetLastError());
   return true;
 }
@@ -1607,7 +1683,13 @@ bool Engine::refresh_bank_source(int s, std::string* err) {
 bool Engine::set_source_background(int source, const uint8_t* bg_raw, int bw, int bh, size_t pitch, std::string* err) {
   if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
   if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
-  if (!bg_raw) { src_has_bg_[source] = 0; return true; }     // later calls blend the context background again
+  if (!bg_raw) {                                               // later calls blend the context background again
+    CUDA_OK(cudaSetDevice(device_));
+    src_has_bg_[source] = 0;
+    if (!refresh_bank_source(source, err)) return false;
+    CUDA_OK(cudaStreamSynchronize(stream_));
+    return true;
+  }
   if (bw <= 0 || bh <= 0 || pitch < (size_t)bw * 3) { *err = "invalid background"; return false; }
   CUDA_OK(cudaSetDevice(device_));
   const size_t raw = (size_t)bw * bh * 3, fbytes = (size_t)W_ * H_ * 3;
@@ -1641,28 +1723,35 @@ bool Engine::run_sources(int n, const int* ids, const uint8_t* d_frames, size_t 
   if (n < 1 || n > max_batch_) { *err = "n_frames out of range (1..max_batch)"; return false; }
   if (!ids) { *err = "null source id table"; return false; }
   if (has_bg_ && bg_count_ > 1) { *err = "sources calls need a still context background (animate a source with bsb_set_source_background)"; return false; }
-  // frame b: state of source ids[b]; background = the source's own, else the context's, else (bgblur, no background
-  // at all) the blurred camera frame in camera-blur slot b
-  const bool ctx_camblur = bgblur_k_ && !has_bg_;
-  std::vector<int> tab(2 * (size_t)max_batch_, 0);
-  bool camblur = false;
+  // frame b: state of source ids[b]; background (source_bg) = the context slot, the source's slot, or its camera frame
+  // blurred at the source's strength into camera-blur slot b
+  std::vector<int> tab(3 * (size_t)max_batch_, 0);
+  unsigned classes = 0;
+  int n_blur = 0;
   for (int b = 0; b < n; ++b) {
     const int id = ids[b];
     if (id < 0 || id >= n_sources_) { *err = "source id out of range"; return false; }
     for (int c = 0; c < b; ++c)
       if (ids[c] == id) { *err = "source ids must be distinct within one call"; return false; }
     tab[b] = id;
+    int k = 0;
+    const int from = source_bg(id, &k);
     int slot = max_batch_;
-    if (src_has_bg_[id]) slot = max_batch_ + 1 + id;
-    else if (ctx_camblur) { slot = b; camblur = true; }
+    if (from == SRC_FROM_SLOT) slot = max_batch_ + 1 + id;
+    else if (from == SRC_FROM_CAMBLUR) { slot = b; tab[2 * (size_t)max_batch_ + b] = k; classes |= (unsigned)gauss_class(k); ++n_blur; }
     tab[(size_t)max_batch_ + b] = slot;
   }
   CUDA_OK(cudaSetDevice(device_));
+  if ((classes & GAUSS_SEPARABLE) && !ensure_gauss_tmp(err)) return false;
   // outside the graph, before its launch: stream order keeps the previous launch's reads ahead of this write
   CUDA_OK(cudaMemcpyAsync(d_src_tab_, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, stream_));
-  call_mode_ = camblur ? CALL_SOURCES_CAMBLUR : CALL_SOURCES;
+  call_mode_ = classes ? CALL_SOURCES_CAMBLUR : CALL_SOURCES;
+  call_gclass_ = classes;
+  call_all_blur_ = n_blur == n;
   const bool ok = run(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, false, err, d_yuyv_in);
   call_mode_ = CALL_PLAIN;
+  call_gclass_ = 0;
+  call_all_blur_ = false;
   return ok;
 }
 

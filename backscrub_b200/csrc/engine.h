@@ -110,6 +110,10 @@ class Engine {
   bool reset_source(int source, std::string* err);
   // cv::resize(raw -> W x H) into the source's bank slot (+ bgblur, + its YUYV); bg_raw == nullptr clears the slot
   bool set_source_background(int source, const uint8_t* bg_raw, int bw, int bh, size_t pitch, std::string* err);
+  // background effect of one source (include/backscrub_b200.h): background SRC_BG_DEFAULT / SRC_BG_NONE, bgblur -1 (follow
+  // the context), 0 or odd 1..255
+  enum { SRC_BG_DEFAULT = 0, SRC_BG_NONE = 1 };
+  bool set_source_effect(int source, int background, int bgblur, std::string* err);
   // frame b belongs to source ids[b] (HOST array of n distinct ids); same buffers / layout as run()
   bool run_sources(int n, const int* ids, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
                    uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, std::string* err,
@@ -296,25 +300,39 @@ class Engine {
 
   // ---- independent sources (run_sources) ----
   // Kind of the call being enqueued: plain (one stream, state_), sources, or sources with at least one frame that blends
-  // its own blurred camera frame (bgblur on, no background of either kind).
+  // its own blurred camera frame (a source with no image and a strength > 0), in the Gaussian launch classes
+  // call_gclass_ (GAUSS_FUSED | GAUSS_SEPARABLE).
   enum CallMode { CALL_PLAIN = 0, CALL_SOURCES = 1, CALL_SOURCES_CAMBLUR = 2 };
   int call_mode_ = CALL_PLAIN;
+  unsigned call_gclass_ = 0;
+  bool call_all_blur_ = false;       // ... and every frame of the call blurs its camera frame (the BGR frames are materialised)
   int n_sources_ = 0;
   uint8_t* src_state_ = nullptr;     // [n_sources][oh*ow] smoother state per source
-  int* d_src_tab_ = nullptr;         // [2][max_batch]: source id of frame b | background-bank slot of frame b (written before each launch)
+  // [3][max_batch]: source id of frame b | background-bank slot of frame b | camera-blur strength of frame b (0 = none),
+  // written before each launch
+  int* d_src_tab_ = nullptr;
   // background bank, one base + one stride for the post kernel: [max_batch] camera-blur slots | [1] the context's effective
-  // background | [n_sources] source slots; d_bank_yuyv_ is its YUYV and d_bank_nv12_ its NV12 (valid for the context and
-  // source slots)
+  // background | [n_sources] source slots; d_bank_yuyv_ is its YUYV and d_bank_nv12_ its NV12 (the camera-blur slots'
+  // are written by the Gaussian of the call, in the call's video format)
   uint8_t* d_bank_ = nullptr, *d_bank_yuyv_ = nullptr, *d_bank_nv12_ = nullptr;
-  uint8_t* d_src_bg_ = nullptr;      // [n_sources] resized, unblurred source backgrounds (re-blurred when bgblur changes)
+  uint8_t* d_src_bg_ = nullptr;      // [n_sources] resized, unblurred source backgrounds (re-blurred when their strength changes)
+  uint8_t* d_green_ = nullptr;       // one plain green frame (the still background of a source without an image)
   uint8_t* d_src_raw_ = nullptr;     // staging of one decoded source background
   size_t src_raw_cap_ = 0;
   DevResizeTab tab_src_;
   int src_bg_w_ = 0, src_bg_h_ = 0;
   std::vector<char> src_has_bg_;
+  struct SrcEffect { int bg = SRC_BG_DEFAULT, k = -1; };
+  std::vector<SrcEffect> src_fx_;
+  // Where source s's background comes from: the context slot, its own bank slot (its effective still background differs
+  // from the context's), or its camera frame blurred at strength *k
+  enum SrcBg { SRC_FROM_CTX = 0, SRC_FROM_SLOT = 1, SRC_FROM_CAMBLUR = 2 };
+  int source_bg(int s, int* k) const;
   int bank_slots() const { return max_batch_ + 1 + n_sources_; }
   bool refresh_bank_ctx(std::string* err);
   bool refresh_bank_source(int s, std::string* err);
+  bool refresh_bank_sources_after_ctx(std::string* err);   // every source slot that depends on the context background / strength
+  bool ensure_gauss_tmp(std::string* err);
   void free_sources();
 
   // everything a captured launch sequence bakes into its kernel arguments
@@ -322,10 +340,13 @@ class Engine {
     int n; const void* f; size_t pitch, stride; const void* o; const void* y; const void* m; const void* yin;
     size_t ostride, ystride, mstride;
     int mode;                        // CallMode: a plain and a sources graph over the same buffers are different graphs
+    unsigned gclass;                 // call_gclass_: the Gaussian launches captured (strengths within them replay)
+    bool all_blur;                   // call_all_blur_: the camera frames were converted to BGR before the graph's kernels
     bool nv12; size_t npitch, nuv, nstride;   // NV12 call and its input layout: never confused with a YUYV call
     bool operator<(const GraphKey& r) const {
-      return std::tie(n, f, pitch, stride, o, y, m, yin, ostride, ystride, mstride, mode, nv12, npitch, nuv, nstride) <
-             std::tie(r.n, r.f, r.pitch, r.stride, r.o, r.y, r.m, r.yin, r.ostride, r.ystride, r.mstride, r.mode, r.nv12, r.npitch, r.nuv, r.nstride);
+      return std::tie(n, f, pitch, stride, o, y, m, yin, ostride, ystride, mstride, mode, gclass, all_blur, nv12, npitch, nuv, nstride) <
+             std::tie(r.n, r.f, r.pitch, r.stride, r.o, r.y, r.m, r.yin, r.ostride, r.ystride, r.mstride, r.mode, r.gclass, r.all_blur, r.nv12, r.npitch, r.nuv,
+                      r.nstride);
     }
   };
 #ifndef BSB_EMU

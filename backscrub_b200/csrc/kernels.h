@@ -262,9 +262,24 @@ void launch_resize_u8c3(cudaStream_t s, const uint8_t* src, int sw, int sh, size
 // app/deepseg.cc:657-658: cv::GaussianBlur(bg, bg, Size(k,k), 0), 8UC3 — OpenCV's 8.8 fixed-point taps (sum 256)
 struct GaussTaps { int k; uint16_t q[255]; };
 bool gauss_taps(int k, GaussTaps* out);           // false unless k is odd, 1..255
-// n frames; tmp holds n*H*W*3 16-bit row sums
-void launch_gauss_blur(cudaStream_t s, int n, const uint8_t* src, size_t spitch, size_t sstride, uint16_t* tmp,
+// n frames; tmp holds n*H*W*3 16-bit row sums.  False if the per-device tap tables could not be allocated.
+bool launch_gauss_blur(cudaStream_t s, int n, const uint8_t* src, size_t spitch, size_t sstride, uint16_t* tmp,
                        uint8_t* dst, size_t dpitch, size_t dstride, int W, int H, const GaussTaps& g);
+// Launch classes of the Gaussian: the fused tile kernel (strengths 3..31) or the row / column pair (1, 33..255); 0 = off
+enum : unsigned { GAUSS_FUSED = 1, GAUSS_SEPARABLE = 2 };
+BSB_HD int gauss_class(int k) { return k == 0 ? 0 : (k >= 3 && k <= 31) ? (int)GAUSS_FUSED : (int)GAUSS_SEPARABLE; }
+// camera frames in their wire format: YUYV or NV12 (InFmt), `pitch` bytes per row, `stride` per frame, NV12's UV plane
+// at byte `uv`
+struct GaussSrc { const uint8_t* p; size_t pitch, stride, uv; int fmt; };
+// the per-device tap tables every launch reads (built on first use); false if they could not be allocated
+bool gauss_tables_ready();
+// Sources calls: frame b blurred with strength ks[b] (DEVICE table [n]; 0 = not blurred) from the tightly packed BGR
+// frame b of `frames` into frame b of dst (same layout); `classes` (GAUSS_FUSED | GAUSS_SEPARABLE) are the launch classes
+// the call may need, so a captured launch replays for any strengths within them.  cam.p non-null: `frames` is first
+// filled, for the blurred frames only, from the camera frames.  dst_yuyv / dst_nv12 (may be null): the blurred frames'
+// YUYV / NV12 (W*H*2 / W*H*3/2 bytes per frame; W even, NV12 also H even).
+bool launch_gauss_frames(cudaStream_t s, int n, const GaussSrc& cam, const int* ks, unsigned classes, uint8_t* frames, uint16_t* tmp,
+                         uint8_t* dst, uint8_t* dst_yuyv, uint8_t* dst_nv12, int W, int H);
 // app/deepseg.cc:667-673: cv::flip on n packed frames
 void launch_flip_u8c3(cudaStream_t s, int n, const uint8_t* src, size_t sstride, uint8_t* dst, size_t dstride, int W, int H, bool flip_h, bool flip_v);
 

@@ -4,7 +4,12 @@
 //   * `-H` / `-V`    cv::flip(raw, raw, 1 / 0 / -1)                     (:667-673)
 //   * virtual-camera geometry  cv::resize(raw, raw, vidGeo)             (:677-679) — k_resize_u8c3 (kernels_img.cu)
 // Integer arithmetic is OpenCV's bit-exact 8-bit path restated (oracle/oracle_img.c pins it on cv2).
-#include "kernels.h"
+#include <cstring>
+#include <map>
+#include <mutex>
+#include <vector>
+
+#include "post_math.h"
 
 namespace bsb {
 
@@ -15,18 +20,59 @@ void count_launch();
 //   rows: h = sum_j q[j]*src[x+j-r]   (<= 255*256, 16 bit)     cols: (sum_j q[j]*h[y+j-r] + 32768) >> 16
 // Both sums are exact integers, so tap order is free.
 //
+// Every kernel blurs frame b with strength ks[b] when given a per-frame strength table (sources calls; 0 = the frame is
+// not blurred), else every frame with k_all.  Strengths 3..31 run the fused tile kernel, 1 and 33..255 the row /
+// column pair (the two launch classes); a CTA whose frame belongs to the other class, or has strength 0, exits at
+// once.  The taps of every odd strength are pre-computed once per device (GaussTables), so a captured launch stays
+// valid whatever strengths its frames get.  The kernels read BGR frames; a sources call whose post kernel reads the
+// camera YUYV / NV12 in place first converts only its camera-blur frames (k_gauss_stage_bgr): converting each pixel
+// once there is cheaper than converting every pixel of every overlapping halo patch inside the Gaussian.
+// ---------------------------------------------------------------------------
+constexpr int GF_TW = 64, GF_TH = 32, GF_MAXR = 15, GF_RM = GF_TH + 2 * GF_MAXR, GF_PW = 100, GF_HR = 66;
+constexpr int GF_NW = 9, GF_NV = 16, GF_NK = GF_MAXR;    // fused strengths 3, 5, .., 31
+
+struct GaussFast { int k, nw, nv; unsigned hq[4][GF_NW]; unsigned cw[GF_NV]; };
+struct GaussTables { GaussFast fast[GF_NK]; GaussTaps taps[128]; };   // fast[(k - 3) / 2], taps[(k - 1) / 2]
+
+// The camera frames of a sources call's camera-blur frames (ks[b] != 0) as tightly packed BGR, for the Gaussian:
+// cv::cvtColor(COLOR_YUV2BGR_YUYV / _NV12), the arithmetic of yuyv_px_to_bgr / nv12_px_to_bgr.  One thread = one pixel
+// pair (W even).
+__global__ void __launch_bounds__(256) k_gauss_stage_bgr(GaussSrc src, uint8_t* bgr, int W, int H, const int* ks) {
+  const int b = blockIdx.y;
+  if (!ks[b]) return;
+  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int hw = W / 2;
+  if (idx >= (long)hw * H) return;
+  const int x = (int)(idx % hw) * 2, y = (int)(idx / hw);
+  const uint8_t* img = src.p + (size_t)b * src.stride;
+  int p0[3], p1[3];
+  if (src.fmt == IN_YUYV) {
+    const uint8_t* q = img + (size_t)y * src.pitch + (size_t)x * 2;
+    yuv_px_to_bgr(q[0], q[1], q[3], p0); yuv_px_to_bgr(q[2], q[1], q[3], p1);
+  } else {
+    const uint8_t* yr = img + (size_t)y * src.pitch + x;
+    const uint8_t* uv = img + src.uv + (size_t)(y >> 1) * src.pitch + x;
+    yuv_px_to_bgr(yr[0], uv[0], uv[1], p0); yuv_px_to_bgr(yr[1], uv[0], uv[1], p1);
+  }
+  uint8_t* o = bgr + (size_t)b * ((size_t)W * H * 3) + ((size_t)y * W + x) * 3;
+  o[0] = (uint8_t)p0[0]; o[1] = (uint8_t)p0[1]; o[2] = (uint8_t)p0[2]; o[3] = (uint8_t)p1[0]; o[4] = (uint8_t)p1[1]; o[5] = (uint8_t)p1[2];
+}
+
 // Row pass: one block = 256 pixels of one row; the reflected source span is staged in shared
 // memory once, every thread then produces three byte lanes.
-// ---------------------------------------------------------------------------
 constexpr int GAUSS_TW = 256;
 
-__global__ void __launch_bounds__(256) k_gauss_rows(const uint8_t* src, size_t pitch, size_t frame_stride, uint16_t* tmp,
-                                                    int W, int H, GaussTaps g) {
+__global__ void __launch_bounds__(256) k_gauss_rows(const uint8_t* src, size_t pitch, size_t frame_stride, uint16_t* tmp, int W, int H,
+                                                    const GaussTables* T, int k_all, const int* ks) {
   __shared__ uint8_t s[(GAUSS_TW + 2 * 127) * 3 + 2];
-  const int r = g.k >> 1;
+  __shared__ uint16_t q[256];
   const int x0 = blockIdx.x * GAUSS_TW, y = blockIdx.y, b = blockIdx.z;
+  const int k = ks ? ks[b] : k_all;
+  if (gauss_class(k) != GAUSS_SEPARABLE) return;
+  const int r = k >> 1;
   const int tw = min(GAUSS_TW, W - x0);
   const uint8_t* row = src + (size_t)b * frame_stride + (size_t)y * pitch;
+  for (int j = threadIdx.x; j < k; j += blockDim.x) q[j] = T->taps[(k - 1) >> 1].q[j];
   const int span = tw + 2 * r;
   for (int i = threadIdx.x; i < span; i += blockDim.x) {
     const int sx = bsb_reflect101(x0 + i - r, W);
@@ -36,23 +82,28 @@ __global__ void __launch_bounds__(256) k_gauss_rows(const uint8_t* src, size_t p
   uint16_t* d = tmp + ((size_t)b * H + y) * (size_t)W * 3 + (size_t)x0 * 3;
   for (int l = threadIdx.x; l < tw * 3; l += blockDim.x) {
     unsigned acc = 0;
-    for (int j = 0; j < g.k; ++j) acc += (unsigned)g.q[j] * s[l + 3 * j];
+    for (int j = 0; j < k; ++j) acc += (unsigned)q[j] * s[l + 3 * j];
     d[l] = (uint16_t)acc;
   }
 }
 
 // Column pass: one block = 128 byte lanes x 32 rows; the (32 + 2r) reflected rows of 16-bit row sums
-// are staged in dynamic shared memory.
+// are staged in dynamic shared memory (sized by the launcher for the largest strength of the call's class).
 constexpr int GAUSS_CL = 128, GAUSS_CH = 32;
 
 __global__ void __launch_bounds__(256) k_gauss_cols(const uint16_t* tmp, uint8_t* dst, size_t pitch, size_t frame_stride,
-                                                    int W, int H, GaussTaps g) {
+                                                    int W, int H, const GaussTables* T, int k_all, const int* ks) {
   BSB_DYN_SMEM(smem_raw);
+  __shared__ uint16_t q[256];
   uint16_t* sm = reinterpret_cast<uint16_t*>(smem_raw);
-  const int r = g.k >> 1, lanes = W * 3;
-  const int l0 = blockIdx.x * GAUSS_CL, y0 = blockIdx.y * GAUSS_CH, b = blockIdx.z;
+  const int b = blockIdx.z;
+  const int k = ks ? ks[b] : k_all;
+  if (gauss_class(k) != GAUSS_SEPARABLE) return;
+  const int r = k >> 1, lanes = W * 3;
+  const int l0 = blockIdx.x * GAUSS_CL, y0 = blockIdx.y * GAUSS_CH;
   const int nl = min(GAUSS_CL, lanes - l0), nr = min(GAUSS_CH, H - y0);
   const uint16_t* t = tmp + (size_t)b * H * lanes;
+  for (int j = threadIdx.x; j < k; j += blockDim.x) q[j] = T->taps[(k - 1) >> 1].q[j];
   const int rows = nr + 2 * r;
   for (int i = threadIdx.x; i < rows * GAUSS_CL; i += blockDim.x) {
     const int rr = i / GAUSS_CL, l = i % GAUSS_CL;
@@ -63,7 +114,7 @@ __global__ void __launch_bounds__(256) k_gauss_cols(const uint16_t* tmp, uint8_t
   if (l >= nl) return;
   for (int yy = threadIdx.x / GAUSS_CL; yy < nr; yy += 256 / GAUSS_CL) {
     unsigned acc = 32768u;
-    for (int j = 0; j < g.k; ++j) acc += (unsigned)g.q[j] * sm[(yy + j) * GAUSS_CL + l];
+    for (int j = 0; j < k; ++j) acc += (unsigned)q[j] * sm[(yy + j) * GAUSS_CL + l];
     dst[(size_t)b * frame_stride + (size_t)(y0 + yy) * pitch + l0 + l] = (uint8_t)(acc >> 16);
   }
 }
@@ -79,57 +130,12 @@ __global__ void __launch_bounds__(256) k_gauss_cols(const uint16_t* tmp, uint8_t
 //   D  the re-interleaved tile goes out in 16-byte stores.
 // All sums are exact integers (<= 255*256*256 < 2^24), so the regrouping is bit-neutral.
 // ---------------------------------------------------------------------------
-constexpr int GF_TW = 64, GF_TH = 32, GF_MAXR = 15, GF_RM = GF_TH + 2 * GF_MAXR, GF_PW = 100, GF_HR = 66;
-constexpr int GF_NW = 9, GF_NV = 16;
 
-struct GaussFast { int k, nw, nv; unsigned hq[4][GF_NW]; unsigned cw[GF_NV]; };
-
-// NWC / NVC > 0: tap-word counts fixed at compile time (the default strength 25 -> 7 / 13), so the dot-product
-// chains are straight-line code; 0: run-time loops for the other strengths.
+// B and C.  NWC / NVC > 0: tap-word counts fixed at compile time (the default strength 25 -> 7 / 13), so the
+// dot-product chains are straight-line code; 0: run-time loops for the other strengths.
 template <int NWC, int NVC>
-__global__ void __launch_bounds__(256) k_gauss_fused(const uint8_t* src, size_t spitch, size_t sstride, uint8_t* dst, size_t dpitch,
-                                                     size_t dstride, int W, int H, GaussFast g, int vec_ok) {
-  __shared__ __align__(16) uint8_t P[3 * GF_RM * GF_PW];      // planes; reused as the interleaved output tile in C/D
-  __shared__ __align__(16) uint16_t Ht[3 * GF_TW * GF_HR];
-  const int r = g.k >> 1, tid = threadIdx.x;
-  const int x0 = blockIdx.x * GF_TW, y0 = blockIdx.y * GF_TH, b = blockIdx.z;
-  const int tw = min(GF_TW, W - x0), th = min(GF_TH, H - y0);
-  const int rows = GF_TH + 2 * r, cols = GF_TW + 2 * r;
-  const uint8_t* frame = src + (size_t)b * sstride;
+BSB_D void gauss_fused_bc(uint8_t* P, uint16_t* Ht, const GaussFast& g, int rows, int tid) {
   const int warp = tid >> 5, lane = tid & 31;
-
-  // ---- A: stage + de-interleave (loads of three column groups and two rows are issued before any store: the
-  //      patch comes from L2/HBM and the loop is latency bound unless several requests per thread are in flight)
-  const bool interior = x0 - r >= 0 && x0 + GF_TW + r <= W && y0 - r >= 0 && y0 + GF_TH + r <= H;
-  if (interior) {
-    const uint8_t* base = frame + (size_t)(y0 - r) * spitch + (size_t)(x0 - r) * 3;
-#pragma unroll 2
-    for (int row = warp; row < rows; row += 8) {
-      const uint8_t* srow = base + (size_t)row * spitch;
-      uint8_t v[3][3];
-#pragma unroll
-      for (int j = 0; j < 3; ++j) {
-        const int col = lane + 32 * j;
-        if (col < cols) { const uint8_t* sp = srow + col * 3; v[j][0] = sp[0]; v[j][1] = sp[1]; v[j][2] = sp[2]; }
-      }
-#pragma unroll
-      for (int j = 0; j < 3; ++j) {
-        const int col = lane + 32 * j;
-        if (col < cols) { uint8_t* pp = P + row * GF_PW + col; pp[0] = v[j][0]; pp[GF_RM * GF_PW] = v[j][1]; pp[2 * GF_RM * GF_PW] = v[j][2]; }
-      }
-    }
-  } else {
-    for (int row = warp; row < rows; row += 8) {
-      const uint8_t* srow = frame + (size_t)bsb_reflect101(y0 + row - r, H) * spitch;
-      for (int col = lane; col < cols; col += 32) {
-        const uint8_t* sp = srow + (size_t)bsb_reflect101(x0 + col - r, W) * 3;
-        uint8_t* pp = P + row * GF_PW + col;
-        pp[0] = sp[0]; pp[GF_RM * GF_PW] = sp[1]; pp[2 * GF_RM * GF_PW] = sp[2];
-      }
-    }
-  }
-  __syncthreads();
-
   // ---- B: row sums (DP4A), stored transposed ----
   const int nw = NWC > 0 ? NWC : g.nw, nv = NVC > 0 ? NVC : g.nv;
   for (int cm = warp; cm < 3 * (GF_TW / 4); cm += 8) {          // one (plane, 4-pixel group) per warp, lanes walk the rows
@@ -180,9 +186,83 @@ __global__ void __launch_bounds__(256) k_gauss_fused(const uint8_t* src, size_t 
     O[(2 * yp) * (GF_TW * 3) + x * 3 + c] = (uint8_t)(a0 >> 16);
     O[(2 * yp + 1) * (GF_TW * 3) + x * 3 + c] = (uint8_t)(a1 >> 16);
   }
+}
+
+// convert_rgb_to_yuyv of one pixel pair (6 BGR bytes) as the word (Y0, V, Y1, U): what the post kernel produces for
+// mask 255, i.e. the cached YUYV of a background slot
+BSB_D unsigned yuyv_pair_word(const uint8_t* s) {
+  int Y0, U0, V0, Y1, U1, V1;
+  rgb2yuv(s[0], s[1], s[2], Y0, U0, V0);
+  rgb2yuv(s[3], s[4], s[5], Y1, U1, V1);
+  return (unsigned)Y0 | ((unsigned)((V0 + V1) / 2) << 8) | ((unsigned)Y1 << 16) | ((unsigned)((U0 + U1) / 2) << 24);
+}
+// the NV12 of one 2x2 block from the YUYV words of its two rows: Y copied, UV the truncating row-pair average
+BSB_D void nv12_block(unsigned w0, unsigned w1, uint8_t* y0, int W, uint8_t* uv) {
+  y0[0] = (uint8_t)w0; y0[1] = (uint8_t)(w0 >> 16); y0[W] = (uint8_t)w1; y0[W + 1] = (uint8_t)(w1 >> 16);
+  uv[0] = (uint8_t)((((w0 >> 8) & 255u) + ((w1 >> 8) & 255u)) >> 1);
+  uv[1] = (uint8_t)(((w0 >> 24) + (w1 >> 24)) >> 1);
+}
+
+// yuyv / nv12 (may be null; W even, NV12 also H even): [n] W*H*2 / W*H*3/2-byte frames that receive the blurred frame's
+// YUYV / NV12, written from the output tile in stage D
+__global__ void __launch_bounds__(256) k_gauss_fused(const uint8_t* src, size_t spitch, size_t sstride, uint8_t* dst, size_t dpitch,
+                                                     size_t dstride, int W, int H, const GaussTables* T, GaussFast g25, int k_all,
+                                                     const int* ks, int vec_ok, uint8_t* yuyv, uint8_t* nv12) {
+  __shared__ __align__(16) uint8_t P[3 * GF_RM * GF_PW];      // planes; reused as the interleaved output tile in C/D
+  __shared__ __align__(16) uint16_t Ht[3 * GF_TW * GF_HR];
+  __shared__ GaussFast g;
+  const int tid = threadIdx.x;
+  const int x0 = blockIdx.x * GF_TW, y0 = blockIdx.y * GF_TH, b = blockIdx.z;
+  const int k = ks ? ks[b] : k_all;
+  if (gauss_class(k) != GAUSS_FUSED) return;
+  if (k != 25 && tid < (int)(sizeof(GaussFast) / 4))            // the 25-tap body takes g25
+    reinterpret_cast<unsigned*>(&g)[tid] = reinterpret_cast<const unsigned*>(&T->fast[(k - 3) >> 1])[tid];
+  const int r = k >> 1;
+  const int tw = min(GF_TW, W - x0), th = min(GF_TH, H - y0);
+  const int rows = GF_TH + 2 * r, cols = GF_TW + 2 * r;
+  const uint8_t* frame = src + (size_t)b * sstride;
+  const int warp = tid >> 5, lane = tid & 31;
+
+  // ---- A: stage + de-interleave (loads of three column groups and two rows are issued before any store: the
+  //      patch comes from L2/HBM and the loop is latency bound unless several requests per thread are in flight)
+  const bool interior = x0 - r >= 0 && x0 + GF_TW + r <= W && y0 - r >= 0 && y0 + GF_TH + r <= H;
+  if (interior) {
+    const uint8_t* base = frame + (size_t)(y0 - r) * spitch + (size_t)(x0 - r) * 3;
+#pragma unroll 2
+    for (int row = warp; row < rows; row += 8) {
+      const uint8_t* srow = base + (size_t)row * spitch;
+      uint8_t v[3][3];
+#pragma unroll
+      for (int j = 0; j < 3; ++j) {
+        const int col = lane + 32 * j;
+        if (col < cols) { const uint8_t* sp = srow + col * 3; v[j][0] = sp[0]; v[j][1] = sp[1]; v[j][2] = sp[2]; }
+      }
+#pragma unroll
+      for (int j = 0; j < 3; ++j) {
+        const int col = lane + 32 * j;
+        if (col < cols) { uint8_t* pp = P + row * GF_PW + col; pp[0] = v[j][0]; pp[GF_RM * GF_PW] = v[j][1]; pp[2 * GF_RM * GF_PW] = v[j][2]; }
+      }
+    }
+  } else {
+    for (int row = warp; row < rows; row += 8) {
+      const uint8_t* srow = frame + (size_t)bsb_reflect101(y0 + row - r, H) * spitch;
+      for (int col = lane; col < cols; col += 32) {
+        const uint8_t* sp = srow + (size_t)bsb_reflect101(x0 + col - r, W) * 3;
+        uint8_t* pp = P + row * GF_PW + col;
+        pp[0] = sp[0]; pp[GF_RM * GF_PW] = sp[1]; pp[2 * GF_RM * GF_PW] = sp[2];
+      }
+    }
+  }
   __syncthreads();
 
-  // ---- D: write out ----
+  // ---- B, C: the unrolled 25-tap specialisation (its tap words are kernel parameters: operands of the dot products,
+  //      no loads), or the run-time loops ----
+  if (k == 25) gauss_fused_bc<7, 13>(P, Ht, g25, rows, tid);
+  else gauss_fused_bc<0, 0>(P, Ht, g, rows, tid);
+  __syncthreads();
+
+  // ---- D: write out, and the tile's YUYV / NV12 from the same shared tile ----
+  const uint8_t* O = P;
   uint8_t* out = dst + (size_t)b * dstride + (size_t)y0 * dpitch + (size_t)x0 * 3;
   if (vec_ok && tw == GF_TW) {
     for (int i = tid; i < th * (GF_TW * 3 / 16); i += 256) {
@@ -194,6 +274,47 @@ __global__ void __launch_bounds__(256) k_gauss_fused(const uint8_t* src, size_t 
       const int row = i / (tw * 3), l = i - row * (tw * 3);
       out[(size_t)row * dpitch + l] = O[row * (GF_TW * 3) + l];
     }
+  }
+  const int np = tw / 2;                                        // pixel pairs per tile row (x0 and W are even)
+  const size_t npix = (size_t)W * H;
+  if (nv12) {                                                   // tile rows start even, th is even (H even)
+    uint8_t* f = nv12 + (size_t)b * (npix * 3 / 2);
+    for (int i = tid; i < (th / 2) * np; i += 256) {
+      const int rp = i / np, j = i - rp * np;
+      const unsigned w0 = yuyv_pair_word(O + (2 * rp) * (GF_TW * 3) + 6 * j), w1 = yuyv_pair_word(O + (2 * rp + 1) * (GF_TW * 3) + 6 * j);
+      const int y = y0 + 2 * rp, x = x0 + 2 * j;
+      nv12_block(w0, w1, f + (size_t)y * W + x, W, f + npix + (size_t)(y >> 1) * W + x);
+    }
+  } else if (yuyv) {
+    unsigned* f = reinterpret_cast<unsigned*>(yuyv + (size_t)b * npix * 2);
+    for (int i = tid; i < th * np; i += 256) {
+      const int row = i / np, j = i - row * np;
+      f[((size_t)(y0 + row) * W + x0) / 2 + j] = yuyv_pair_word(O + row * (GF_TW * 3) + 6 * j);
+    }
+  }
+}
+
+// The same YUYV / NV12 for the frames of the row / column class (ks[b] in it), from the blurred BGR frames.  One
+// thread = one pixel pair of two rows.
+__global__ void __launch_bounds__(256) k_gauss_slot_yuv(const uint8_t* bgr, size_t bstride, uint8_t* yuyv, uint8_t* nv12, int W, int H,
+                                                        const int* ks) {
+  const int b = blockIdx.y;
+  if (gauss_class(ks[b]) != GAUSS_SEPARABLE) return;
+  const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const int hw = W / 2;
+  if (idx >= (long)hw * ((H + 1) / 2)) return;
+  const int j = (int)(idx % hw), rp = (int)(idx / hw);
+  const size_t npix = (size_t)W * H;
+  const uint8_t* s0 = bgr + (size_t)b * bstride + ((size_t)(2 * rp) * W + 2 * j) * 3;
+  const unsigned w0 = yuyv_pair_word(s0);
+  if (nv12) {                                                   // H even (NV12 calls)
+    const unsigned w1 = yuyv_pair_word(s0 + (size_t)W * 3);
+    uint8_t* f = nv12 + (size_t)b * (npix * 3 / 2);
+    nv12_block(w0, w1, f + (size_t)(2 * rp) * W + 2 * j, W, f + npix + (size_t)rp * W + 2 * j);
+  } else if (yuyv) {
+    unsigned* f = reinterpret_cast<unsigned*>(yuyv + (size_t)b * npix * 2);
+    f[((size_t)(2 * rp) * W) / 2 + j] = w0;
+    if (2 * rp + 1 < H) f[((size_t)(2 * rp + 1) * W) / 2 + j] = yuyv_pair_word(s0 + (size_t)W * 3);
   }
 }
 
@@ -211,27 +332,83 @@ static bool gauss_fast_params(const GaussTaps& t, GaussFast* f) {
   return true;
 }
 
+// the taps of every odd strength on the CURRENT device, built from gauss_taps on first use (one per device, under a
+// mutex like ensure_dyn_smem; contexts call it before they capture a graph)
+static const GaussTables* gauss_tables() {
+  static std::mutex mu;
+  static std::map<int, GaussTables*> tabs;
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
+  std::lock_guard<std::mutex> lock(mu);
+  auto it = tabs.find(dev);
+  if (it != tabs.end()) return it->second;
+  std::vector<GaussTables> h(1);
+  GaussTables& t = h[0];
+  std::memset(&t, 0, sizeof(t));
+  for (int k = 1; k <= 255; k += 2) {
+    gauss_taps(k, &t.taps[(k - 1) >> 1]);
+    if (gauss_class(k) == GAUSS_FUSED) gauss_fast_params(t.taps[(k - 1) >> 1], &t.fast[(k - 3) >> 1]);
+  }
+  GaussTables* d = nullptr;
+  if (cudaMalloc((void**)&d, sizeof(GaussTables)) != cudaSuccess) return nullptr;
+  if (cudaMemcpy(d, &t, sizeof(GaussTables), cudaMemcpyHostToDevice) != cudaSuccess) { cudaFree(d); return nullptr; }
+  tabs[dev] = d;
+  return d;
+}
+
+bool gauss_tables_ready() { return gauss_tables() != nullptr; }
+
 size_t gauss_cols_smem(int k) { return (size_t)(GAUSS_CH + 2 * (k >> 1)) * GAUSS_CL * sizeof(uint16_t); }
 
-void launch_gauss_blur(cudaStream_t s, int n, const uint8_t* src, size_t spitch, size_t sstride, uint16_t* tmp,
-                       uint8_t* dst, size_t dpitch, size_t dstride, int W, int H, const GaussTaps& g) {
-  GaussFast f;
-  if (gauss_fast_params(g, &f)) {
+// classes: GAUSS_FUSED and / or GAUSS_SEPARABLE launches; ks null: every frame at k_all
+static bool launch_gauss_classes(cudaStream_t s, int n, const uint8_t* src, size_t spitch, size_t sstride, const int* ks, int k_all,
+                                 unsigned classes, uint16_t* tmp, uint8_t* dst, size_t dpitch, size_t dstride, int W, int H,
+                                 uint8_t* yuyv = nullptr, uint8_t* nv12 = nullptr) {
+  const GaussTables* T = gauss_tables();
+  if (!T) return false;
+  static const GaussFast g25 = [] { GaussTaps t{}; GaussFast f{}; gauss_taps(25, &t); gauss_fast_params(t, &f); return f; }();
+  if (classes & GAUSS_FUSED) {
     const int vec_ok = (reinterpret_cast<uintptr_t>(dst) % 16 == 0 && dpitch % 16 == 0 && dstride % 16 == 0) ? 1 : 0;
     const dim3 grid((unsigned)ceil_div(W, GF_TW), (unsigned)ceil_div(H, GF_TH), (unsigned)n);
-    if (f.nw == 7 && f.nv == 13) { auto kern = k_gauss_fused<7, 13>; BSB_LAUNCH(kern, grid, dim3(256), 0, s, src, spitch, sstride, dst, dpitch, dstride, W, H, f, vec_ok); }
-    else { auto kern = k_gauss_fused<0, 0>; BSB_LAUNCH(kern, grid, dim3(256), 0, s, src, spitch, sstride, dst, dpitch, dstride, W, H, f, vec_ok); }
+    BSB_LAUNCH(k_gauss_fused, grid, dim3(256), 0, s, src, spitch, sstride, dst, dpitch, dstride, W, H, T, g25, k_all, ks, vec_ok, yuyv,
+               nv12);
     count_launch();
-    return;
   }
-  BSB_LAUNCH(k_gauss_rows, dim3((unsigned)ceil_div(W, GAUSS_TW), (unsigned)H, (unsigned)n), dim3(256), 0, s,
-             src, spitch, sstride, tmp, W, H, g);
-  count_launch();
-  const size_t smem = gauss_cols_smem(g.k);
-  ensure_dyn_smem(reinterpret_cast<const void*>(k_gauss_cols), smem);
-  BSB_LAUNCH(k_gauss_cols, dim3((unsigned)ceil_div(W * 3, GAUSS_CL), (unsigned)ceil_div(H, GAUSS_CH), (unsigned)n), dim3(256), smem, s,
-             tmp, dst, dpitch, dstride, W, H, g);
-  count_launch();
+  if (classes & GAUSS_SEPARABLE) {
+    BSB_LAUNCH(k_gauss_rows, dim3((unsigned)ceil_div(W, GAUSS_TW), (unsigned)H, (unsigned)n), dim3(256), 0, s, src, spitch, sstride, tmp, W, H,
+               T, k_all, ks);
+    count_launch();
+    // a table call may replay with any strength of the class: room for k = 255
+    const size_t smem = gauss_cols_smem(ks ? 255 : k_all);
+    ensure_dyn_smem(reinterpret_cast<const void*>(k_gauss_cols), smem);
+    BSB_LAUNCH(k_gauss_cols, dim3((unsigned)ceil_div(W * 3, GAUSS_CL), (unsigned)ceil_div(H, GAUSS_CH), (unsigned)n), dim3(256), smem, s,
+               tmp, dst, dpitch, dstride, W, H, T, k_all, ks);
+    count_launch();
+  }
+  return true;
+}
+
+bool launch_gauss_blur(cudaStream_t s, int n, const uint8_t* src, size_t spitch, size_t sstride, uint16_t* tmp,
+                       uint8_t* dst, size_t dpitch, size_t dstride, int W, int H, const GaussTaps& g) {
+  return launch_gauss_classes(s, n, src, spitch, sstride, nullptr, g.k, (unsigned)gauss_class(g.k), tmp, dst, dpitch, dstride, W, H);
+}
+
+bool launch_gauss_frames(cudaStream_t s, int n, const GaussSrc& cam, const int* ks, unsigned classes, uint8_t* frames, uint16_t* tmp,
+                         uint8_t* dst, uint8_t* dst_yuyv, uint8_t* dst_nv12, int W, int H) {
+  const size_t fbytes = (size_t)W * H * 3;
+  if (cam.p) {
+    const long blocks = ((long)(W / 2) * H + 255) / 256;
+    BSB_LAUNCH(k_gauss_stage_bgr, dim3((unsigned)blocks, (unsigned)n), dim3(256), 0, s, cam, frames, W, H, ks);
+    count_launch();
+  }
+  if (!launch_gauss_classes(s, n, frames, (size_t)W * 3, fbytes, ks, 0, classes, tmp, dst, (size_t)W * 3, fbytes, W, H, dst_yuyv, dst_nv12))
+    return false;
+  if ((classes & GAUSS_SEPARABLE) && (dst_yuyv || dst_nv12)) {
+    const long blocks = ((long)(W / 2) * ((H + 1) / 2) + 255) / 256;
+    BSB_LAUNCH(k_gauss_slot_yuv, dim3((unsigned)blocks, (unsigned)n), dim3(256), 0, s, dst, fbytes, dst_yuyv, dst_nv12, W, H, ks);
+    count_launch();
+  }
+  return true;
 }
 
 // OpenCV getGaussianKernelBitExact + getGaussianKernelFixedPoint_ED for sigma = 0 (8 fractional bits).

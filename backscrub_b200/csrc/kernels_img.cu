@@ -449,16 +449,6 @@ BSB_D void load48(const uint8_t* p, bool fast, Px16& r) {
   }
 }
 
-BSB_D void rgb2yuv(int R, int G, int Bc, int& Y, int& U, int& V) {
-  // cv::cvtColor(COLOR_RGB2YUV) 8-bit, 14-bit fixed point (oracle_img.c:or_rgb2yuv_u8)
-  Y = (4899 * R + 9617 * G + 1868 * Bc + 8192) >> 14;
-  U = ((Bc - Y) * 8061 + (128 << 14) + 8192) >> 14;
-  V = ((R - Y) * 14369 + (128 << 14) + 8192) >> 14;
-  Y = Y > 255 ? 255 : Y;
-  U = U < 0 ? 0 : (U > 255 ? 255 : U);
-  V = V < 0 ? 0 : (V > 255 ? 255 : V);
-}
-
 __global__ void __launch_bounds__(256) k_post(PostArgs a) {
   __shared__ __align__(16) uint8_t Us[PT_UH * PT_US];
   __shared__ __align__(16) unsigned short Vs[PT_H * PT_UW];

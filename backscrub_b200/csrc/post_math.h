@@ -79,6 +79,16 @@ BSB_D void yuyv8_to_bgr24(const unsigned* w, unsigned* o) {
     o[3 * q + 2] = __byte_perm(p2, p3, 0x6542);      // r2 b3 g3 r3
   }
 }
+BSB_D void rgb2yuv(int R, int G, int Bc, int& Y, int& U, int& V) {
+  // cv::cvtColor(COLOR_RGB2YUV) 8-bit, 14-bit fixed point (oracle_img.c:or_rgb2yuv_u8)
+  Y = (4899 * R + 9617 * G + 1868 * Bc + 8192) >> 14;
+  U = ((Bc - Y) * 8061 + (128 << 14) + 8192) >> 14;
+  V = ((R - Y) * 14369 + (128 << 14) + 8192) >> 14;
+  Y = Y > 255 ? 255 : Y;
+  U = U < 0 ? 0 : (U > 255 ? 255 : U);
+  V = V < 0 ? 0 : (V > 255 ? 255 : V);
+}
+
 // one pixel from its Y byte and the U / V bytes it shares (the arithmetic of yuyv8_to_bgr24)
 BSB_D void yuv_px_to_bgr(int y, int u8, int v8, int* bgr) {
   const int u = u8 - 128, v = v8 - 128;

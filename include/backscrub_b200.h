@@ -182,7 +182,8 @@ BSB_API int bsb_composite_nv12(bsb_ctx* ctx, int n_frames, const uint8_t* nv12, 
  * in this order: the source's own background (bsb_set_source_background); else the context
  * background (bsb_set_background, or the green default), blurred when bgblur is on; else, with
  * bgblur on and no background of either kind, its own blurred camera frame (app/deepseg.cc:652-658).
- * bsb_set_bgblur and bsb_set_output apply to every frame; callbacks do not fire; the context
+ * That is the default effect of every source; bsb_set_source_effect changes it per source.
+ * bsb_set_output applies to every frame; callbacks do not fire; the context
  * background must not be a ring of more than one image.  Plain calls never touch the per-source
  * states and sources calls never touch the plain smoother state, so both can be mixed on one
  * context.  A violated rule returns 0 with a bsb_last_error() message and leaves the context usable. */
@@ -195,6 +196,21 @@ BSB_API int bsb_reset_source(bsb_ctx* ctx, int source);
  * the source's slot, blurred once if bgblur is on.  bg_raw NULL clears the slot (the source blends the
  * context background again).  Video backgrounds: call again for each decoded frame. */
 BSB_API int bsb_set_source_background(bsb_ctx* ctx, int source, const uint8_t* bg_raw, int bg_w, int bg_h, size_t bg_pitch);
+/* Background effect of one source.  Frame b of a sources call, from source s, gives exactly the bytes a plain
+ * context gives for that camera's stream when set up with the background s would blend (its own image, else the
+ * context image, else none) and bsb_set_bgblur(k), k = s's effective strength.
+ * background: BSB_SOURCE_BG_DEFAULT = the source's own image if set, else the context background (the rule above);
+ *             BSB_SOURCE_BG_NONE    = no image at all, as a reference run without -b: the blurred camera frame when
+ *                                     the strength is > 0, else plain green (the source's own image is kept,
+ *                                     unused, until DEFAULT again).
+ * bgblur:     -1 = follow the context (bsb_set_bgblur, including later changes), 0 = off, odd 1..255.
+ * bsb_set_sources resets every source to (DEFAULT, -1).  bsb_set_output and the camera-blur mode of plain calls stay
+ * per context.  An unknown background, an even / out-of-range strength, a source id out of range or no
+ * bsb_set_sources yet return 0 with a bsb_last_error() message.
+ * Cost: bsb_set_background and bsb_set_bgblur refresh the still background of every source except one with its own
+ * image at a fixed strength (a Gaussian for each such source with a strength > 0; nothing is cached by strength). */
+enum { BSB_SOURCE_BG_DEFAULT = 0, BSB_SOURCE_BG_NONE = 1 };
+BSB_API int bsb_set_source_effect(bsb_ctx* ctx, int source, int background, int bgblur);
 /* HOST buffers, BGR frames, laid out as in bsb_composite (out rows tightly packed, `out_stride` bytes
  * per frame).  Any of out / out_yuyv / out_mask may be NULL. */
 BSB_API int bsb_composite_sources(bsb_ctx* ctx, int n_frames, const int* source_ids, const uint8_t* frames, size_t frame_pitch,
