@@ -272,6 +272,14 @@ class MaskGen:
         if not self._lib.bsb_set_source_effect(self._h, int(source), kinds[background], int(bgblur)):
             self._fail("bsb_set_source_effect")
 
+    def set_source_flip(self, source: int, flip_h=None, flip_v=None):
+        """mirroring of one source's composite and video output (cv::flip, app/deepseg.cc:667-673; the mask is never
+        flipped): flip_h / flip_v both None = follow set_output's flips, including later changes; otherwise the source's
+        own setting (a None beside a bool counts as False)."""
+        flip = -1 if flip_h is None and flip_v is None else (1 if flip_h else 0) | (2 if flip_v else 0)
+        if not self._lib.bsb_set_source_flip(self._h, int(source), flip):
+            self._fail("bsb_set_source_flip")
+
     def composite_sources(self, frames: np.ndarray, ids, want_out=True, want_yuyv=True, want_mask=True):
         """HOST buffers: frames [n, H, W, 3], frame b the next frame of source ids[b] (distinct ids) -> (out, yuyv, mask)."""
         frames = np.ascontiguousarray(frames, np.uint8)

@@ -509,6 +509,13 @@ int bsb_set_source_effect(bsb_ctx* ctx, int source, int background, int bgblur) 
   return 1;
 }
 
+int bsb_set_source_flip(bsb_ctx* ctx, int source, int flip) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_source_flip(source, flip, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
 int bsb_composite_sources(bsb_ctx* ctx, int n, const int* source_ids, const uint8_t* frames, size_t frame_pitch, size_t frame_stride,
                           uint8_t* out, size_t out_stride, uint8_t* out_yuyv, size_t yuyv_stride, uint8_t* out_mask, size_t mask_stride) {
   if (!check_ctx(ctx)) return 0;

@@ -927,7 +927,7 @@ bool Engine::upload(std::string* err) {
 
 Engine::~Engine() {
 #ifndef BSB_EMU
-  for (auto& kv : graphs_) cudaGraphExecDestroy(kv.second);
+  for (auto& kv : graphs_) cudaGraphExecDestroy(kv.second.exec);
 #endif
   if (stream_) { cudaStreamSynchronize(stream_); }
   for (void* p : {(void*)wblob_, (void*)arena_, (void*)lut_, (void*)rowsum_, (void*)in_u8_, (void*)filt_u8_, (void*)state_, (void*)ofinal_,
@@ -1178,7 +1178,7 @@ void Engine::enqueue_decision(int n) {
 PostArgs Engine::post_args(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
                            uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in) const {
   const size_t fbytes = (size_t)W_ * H_ * 3;
-  const bool flip = flip_h_ || flip_v_, resized = out_w_ != W_ || out_h_ != H_, tail = flip || resized;
+  const bool tail = call_tail();
   const bool want_rgb = d_out || d_yuyv;
   const bool nv12_in = nv12_.on && d_yuyv_in;
   PostArgs a{};
@@ -1218,6 +1218,9 @@ PostArgs Engine::post_args(int n, const uint8_t* d_frames, size_t pitch, size_t 
     a.out = d_out; a.out_stride = out_stride;
     if (nv12_in) { a.nv12 = d_yuyv; a.nv12_stride = yuyv_stride; }
     else { a.yuyv = d_yuyv; a.yuyv_stride = yuyv_stride; }
+    // sources calls with flipped frames and no tail: k_post_tma writes the frames of the table's flip row mirrored.
+    // Without flipped frames no table is passed, and the post kernel runs as for a plain call.
+    if (call_mode_ != CALL_PLAIN && call_flipped_) a.flip = d_src_tab_ + 3 * (size_t)max_batch_;
   } else {
     a.out = want_rgb ? d_stage_a_ : nullptr; a.out_stride = fbytes;
     a.yuyv = nullptr; a.yuyv_stride = 0;
@@ -1227,10 +1230,12 @@ PostArgs Engine::post_args(int n, const uint8_t* d_frames, size_t pitch, size_t 
   return a;
 }
 
-void Engine::enqueue_post(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
+bool Engine::enqueue_post(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
                           uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in) {
   const size_t fbytes = (size_t)W_ * H_ * 3;
-  const bool flip = flip_h_ || flip_v_, resized = out_w_ != W_ || out_h_ != H_, tail = flip || resized;
+  const bool resized = out_w_ != W_ || out_h_ != H_, tail = call_tail();
+  // plain calls flip by the context; sources calls by frame, from the table's flip row
+  const bool flip = call_mode_ == CALL_PLAIN ? (flip_h_ || flip_v_) : call_flip_tail_;
   const bool want_rgb = d_out || d_yuyv;
   const bool ring = call_mode_ == CALL_PLAIN && has_bg_ && bg_count_ > 1;
   // app/deepseg.cc:652-658: no background source => the background is the blurred camera frame itself (sources: frame b
@@ -1250,16 +1255,17 @@ void Engine::enqueue_post(int n, const uint8_t* d_frames, size_t pitch, size_t s
   } else if (call_mode_ == CALL_PLAIN && !has_bg_ && bgblur_k_ && want_rgb)
     launch_gauss_blur(stream_, n, d_frames, pitch, stride, d_gauss_tmp_, d_bg_frames_, (size_t)W_ * 3, fbytes, W_, H_, taps_);
   const PostArgs a = post_args(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in);
-  launch_post(stream_, a);
+  if (!launch_post(stream_, a)) return false;
   if (ring && bg_advance_) launch_advance_cursor(stream_, d_bg_cursor_, (int)(((long)n * bg_advance_) % bg_count_), bg_count_);
-  if (!tail || !want_rgb) return;
+  if (!tail || !want_rgb) return true;
   // app/deepseg.cc:667-679: flip, then scale to the virtual-camera geometry, then YUYV (:681)
   const size_t obytes = (size_t)out_w_ * out_h_ * 3;
   const uint8_t* cur = d_stage_a_; size_t cur_stride = fbytes;
   if (flip) {
     uint8_t* dst = (!resized && d_out) ? d_out : d_stage_b_;
     const size_t ds = (!resized && d_out) ? out_stride : fbytes;
-    launch_flip_u8c3(stream_, n, cur, cur_stride, dst, ds, W_, H_, flip_h_, flip_v_);
+    if (call_mode_ == CALL_PLAIN) launch_flip_u8c3(stream_, n, cur, cur_stride, dst, ds, W_, H_, flip_h_, flip_v_);
+    else launch_flip_u8c3_frames(stream_, n, cur, cur_stride, dst, ds, W_, H_, d_src_tab_ + 3 * (size_t)max_batch_);
     cur = dst; cur_stride = ds;
   }
   if (resized) {
@@ -1269,6 +1275,7 @@ void Engine::enqueue_post(int n, const uint8_t* d_frames, size_t pitch, size_t s
     cur = dst; cur_stride = ds;
   }
   if (d_yuyv) launch_rgb_to_yuyv(stream_, cur, d_yuyv, (size_t)out_w_ * out_h_, n, cur_stride, yuyv_stride);
+  return true;
 }
 
 // Camera YUYV / NV12 input: the pre-processing kernel always reads the frames in place; the BGR frame is materialised
@@ -1284,7 +1291,42 @@ bool Engine::yuyv_native(int n, const uint8_t* d_frames, size_t pitch, size_t st
   return post_tma_eligible(post_args(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in));
 }
 
-void Engine::enqueue_all(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
+// NV12 output: the post kernel writes it when it reads the NV12 frames in place and no tail follows (a sources call
+// mirrored in place included); otherwise the YUYV output goes to the context staging and k_yuyv_to_nv12 derives the NV12
+// from it (the definition)
+bool Engine::nv12_staged(bool native, const uint8_t* d_yuyv) const { return nv12_.on && d_yuyv && !(native && !call_tail()); }
+
+// the PostArgs enqueue_all's post stage gets: camera frames in place when native, the video output staged per nv12_staged
+PostArgs Engine::call_post_args(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv,
+                                size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in, bool native) const {
+  const bool staged = nv12_staged(native, d_yuyv);
+  return post_args(n, d_frames, pitch, stride, d_out, out_stride, staged ? d_yuyv_ : d_yuyv, staged ? (size_t)out_w_ * out_h_ * 2 : yuyv_stride,
+                   d_mask, mask_stride, native ? d_yuyv_in : nullptr);
+}
+
+// Sources calls with flipped frames (app/deepseg.cc:667-681 flips before the resize): without a resize, and where
+// k_post_tma takes the call, it writes them mirrored in place; otherwise the tail flips them (and copies the others)
+// between the post kernel and the resize.  Decided where the call is enqueued (eagerly, or on a graph miss: the
+// GraphKey fixes everything the decision reads), so a replay costs no host work.
+bool Engine::plan_flips(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv,
+                        size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in, std::string* err) {
+  call_flip_tail_ = false;
+  if (call_mode_ == CALL_PLAIN || !call_flipped_) return true;
+  bool in_place = out_w_ == W_ && out_h_ == H_ && tuning().post_tma;
+  if (in_place) {
+    const bool native = yuyv_native(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in);
+    in_place = post_tma_eligible(call_post_args(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in, native));
+  }
+  call_flip_tail_ = !in_place;
+  if (call_flip_tail_ && (d_out || d_yuyv)) {
+    // set_output allocates the staging for a context flip / resize only; grown once (dropping the graphs) on first need
+    const size_t fbytes = (size_t)max_batch_ * W_ * H_ * 3;
+    return ensure((void**)&d_stage_a_, &stage_a_cap_, fbytes, err) && ensure((void**)&d_stage_b_, &stage_b_cap_, fbytes, err);
+  }
+  return true;
+}
+
+bool Engine::enqueue_all(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
                          uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in,
                          bool native, bool sync_cbs) {
   const long l0 = thread_launch_count();
@@ -1298,15 +1340,15 @@ void Engine::enqueue_all(int n, const uint8_t* d_frames, size_t pitch, size_t st
   if (sync_cbs && cb_.oninfer) { cudaStreamSynchronize(stream_); cb_.oninfer(cb_.caller_ctx); }
   enqueue_decision(n);
   if (sync_cbs && cb_.onmask) { cudaStreamSynchronize(stream_); cb_.onmask(cb_.caller_ctx); }
-  // NV12 output: the post kernel writes it when it reads the NV12 frames in place and no flip / resize follows; otherwise
-  // the YUYV output goes to the context staging and k_yuyv_to_nv12 derives the NV12 from it (the definition)
-  const bool tail = flip_h_ || flip_v_ || out_w_ != W_ || out_h_ != H_;
-  const bool nv12_staged = nv12_.on && d_yuyv && !(native && !tail);
+  const bool staged = nv12_staged(native, d_yuyv);
   const size_t opix = (size_t)out_w_ * out_h_;
-  enqueue_post(n, d_frames, pitch, stride, d_out, out_stride, nv12_staged ? d_yuyv_ : d_yuyv, nv12_staged ? opix * 2 : yuyv_stride, d_mask,
-               mask_stride, native ? d_yuyv_in : nullptr);
-  if (nv12_staged) launch_yuyv_to_nv12(stream_, n, d_yuyv_, opix * 2, d_yuyv, yuyv_stride, out_w_, out_h_);
+  // the arguments call_post_args gives (plan_flips decides on those)
+  if (!enqueue_post(n, d_frames, pitch, stride, d_out, out_stride, staged ? d_yuyv_ : d_yuyv, staged ? opix * 2 : yuyv_stride, d_mask,
+                    mask_stride, native ? d_yuyv_in : nullptr))
+    return false;
+  if (staged) launch_yuyv_to_nv12(stream_, n, d_yuyv_, opix * 2, d_yuyv, yuyv_stride, out_w_, out_h_);
   last_call_launches_ = (int)(thread_launch_count() - l0);
+  return true;
 }
 
 bool Engine::run(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
@@ -1320,27 +1362,39 @@ bool Engine::run(int n, const uint8_t* d_frames, size_t pitch, size_t stride, ui
 #ifdef BSB_EMU
   eager = true;
 #endif
+  static const char* kNoMirror = "the post kernel cannot write this call's mirrored frames";
   if (eager) {
+    if (!plan_flips(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in, err)) return false;
     const bool native = yuyv_native(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in);
     last_native_ = native;
-    enqueue_all(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in, native, cbs);
+    if (!enqueue_all(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in, native, cbs)) {
+      *err = kNoMirror; return false;
+    }
     CUDA_OK(cudaGetLastError());
     return true;
   }
 #ifndef BSB_EMU
   const GraphKey key{n, d_frames, pitch, stride, d_out, d_yuyv, d_mask, d_yuyv_in, d_out ? out_stride : 0, d_yuyv ? yuyv_stride : 0,
-                     d_mask ? mask_stride : 0, call_mode_, call_gclass_, call_all_blur_, nv12_.on, nv12_.pitch, nv12_.uv, nv12_.stride};
+                     d_mask ? mask_stride : 0, call_mode_, call_gclass_, call_all_blur_, nv12_.on, nv12_.pitch, nv12_.uv, nv12_.stride,
+                     call_flipped_};
   auto it = graphs_.find(key);
   if (it == graphs_.end()) {
     if (graphs_.size() >= 64) drop_graphs();
+    if (!plan_flips(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in, err)) return false;
     const bool native = yuyv_native(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in);
     last_native_ = native;
     cudaGraph_t graph = nullptr;
     CUDA_OK(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
-    enqueue_all(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in, native, false);
+    const bool enq = enqueue_all(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in, native, false);
     // the capture is always closed, also when a launch inside it failed: a stream left in capture mode would
     // poison every later call on this context
     const cudaError_t ce = cudaStreamEndCapture(stream_, &graph);
+    if (!enq) {
+      if (graph) cudaGraphDestroy(graph);
+      cudaGetLastError();
+      *err = kNoMirror;
+      return false;
+    }
     if (ce != cudaSuccess || !graph) {
       if (graph) cudaGraphDestroy(graph);
       cudaGetLastError();
@@ -1351,9 +1405,10 @@ bool Engine::run(int n, const uint8_t* d_frames, size_t pitch, size_t stride, ui
     const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
     cudaGraphDestroy(graph);
     if (ie != cudaSuccess) { cudaGetLastError(); *err = std::string("cudaGraphInstantiate failed: ") + cudaGetErrorString(ie); return false; }
-    it = graphs_.emplace(key, exec).first;
+    it = graphs_.emplace(key, CapturedCall{exec, last_call_launches_}).first;
   }
-  CUDA_OK(cudaGraphLaunch(it->second, stream_));
+  last_call_launches_ = it->second.launches;
+  CUDA_OK(cudaGraphLaunch(it->second.exec, stream_));
 #endif
   return true;
 }
@@ -1399,7 +1454,7 @@ bool Engine::infer(int n, const float* h_in, float* h_out, std::string* err) {
 
 void Engine::drop_graphs() {
 #ifndef BSB_EMU
-  for (auto& kv : graphs_) cudaGraphExecDestroy(kv.second);
+  for (auto& kv : graphs_) cudaGraphExecDestroy(kv.second.exec);
   graphs_.clear();
 #endif
 }
@@ -1551,6 +1606,7 @@ void Engine::free_sources() {
   n_sources_ = 0;
   src_has_bg_.clear();
   src_fx_.clear();
+  src_flip_.clear();
 }
 
 bool Engine::set_sources(int n_sources, std::string* err) {
@@ -1562,8 +1618,8 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   const size_t fbytes = (size_t)W_ * H_ * 3, npix = (size_t)W_ * H_, opx = (size_t)oh_ * ow_;
   const size_t slots = (size_t)max_batch_ + 1 + (size_t)n_sources;
   if (!d_src_tab_) {
-    CUDA_OK(cudaMalloc((void**)&d_src_tab_, 3 * (size_t)max_batch_ * sizeof(int)));
-    CUDA_OK(cudaMemset(d_src_tab_, 0, 3 * (size_t)max_batch_ * sizeof(int)));
+    CUDA_OK(cudaMalloc((void**)&d_src_tab_, 4 * (size_t)max_batch_ * sizeof(int)));
+    CUDA_OK(cudaMemset(d_src_tab_, 0, 4 * (size_t)max_batch_ * sizeof(int)));
   }
   CUDA_OK(cudaMalloc((void**)&src_state_, (size_t)n_sources * opx));
   CUDA_OK(cudaMemset(src_state_, 0, (size_t)n_sources * opx));
@@ -1587,6 +1643,7 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   n_sources_ = n_sources;
   src_has_bg_.assign((size_t)n_sources, 0);
   src_fx_.assign((size_t)n_sources, SrcEffect{});
+  src_flip_.assign((size_t)n_sources, -1);
   if (!refresh_bank_ctx(err)) return false;
   CUDA_OK(cudaStreamSynchronize(stream_));
   return true;
@@ -1680,6 +1737,14 @@ bool Engine::set_source_effect(int source, int background, int bgblur, std::stri
   return true;
 }
 
+bool Engine::set_source_flip(int source, int flip, std::string* err) {
+  if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
+  if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
+  if (flip < -1 || flip > 3) { *err = "source flip must be -1 (follow the context) or 0..3 (BSB_FLIP_H | BSB_FLIP_V)"; return false; }
+  src_flip_[source] = (signed char)flip;
+  return true;
+}
+
 bool Engine::set_source_background(int source, const uint8_t* bg_raw, int bw, int bh, size_t pitch, std::string* err) {
   if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
   if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
@@ -1724,10 +1789,12 @@ bool Engine::run_sources(int n, const int* ids, const uint8_t* d_frames, size_t 
   if (!ids) { *err = "null source id table"; return false; }
   if (has_bg_ && bg_count_ > 1) { *err = "sources calls need a still context background (animate a source with bsb_set_source_background)"; return false; }
   // frame b: state of source ids[b]; background (source_bg) = the context slot, the source's slot, or its camera frame
-  // blurred at the source's strength into camera-blur slot b
-  std::vector<int> tab(3 * (size_t)max_batch_, 0);
+  // blurred at the source's strength into camera-blur slot b; flip = the source's own, else the context's
+  std::vector<int> tab(4 * (size_t)max_batch_, 0);
   unsigned classes = 0;
   int n_blur = 0;
+  bool flipped = false;                          // some frame of the call is mirrored
+  const int ctx_flip = (flip_h_ ? 1 : 0) | (flip_v_ ? 2 : 0);
   for (int b = 0; b < n; ++b) {
     const int id = ids[b];
     if (id < 0 || id >= n_sources_) { *err = "source id out of range"; return false; }
@@ -1740,6 +1807,9 @@ bool Engine::run_sources(int n, const int* ids, const uint8_t* d_frames, size_t 
     if (from == SRC_FROM_SLOT) slot = max_batch_ + 1 + id;
     else if (from == SRC_FROM_CAMBLUR) { slot = b; tab[2 * (size_t)max_batch_ + b] = k; classes |= (unsigned)gauss_class(k); ++n_blur; }
     tab[(size_t)max_batch_ + b] = slot;
+    const int fl = src_flip_[id] < 0 ? ctx_flip : src_flip_[id];
+    tab[3 * (size_t)max_batch_ + b] = fl;
+    flipped = flipped || fl != 0;
   }
   CUDA_OK(cudaSetDevice(device_));
   if ((classes & GAUSS_SEPARABLE) && !ensure_gauss_tmp(err)) return false;
@@ -1748,10 +1818,13 @@ bool Engine::run_sources(int n, const int* ids, const uint8_t* d_frames, size_t 
   call_mode_ = classes ? CALL_SOURCES_CAMBLUR : CALL_SOURCES;
   call_gclass_ = classes;
   call_all_blur_ = n_blur == n;
+  call_flipped_ = flipped;
   const bool ok = run(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, false, err, d_yuyv_in);
   call_mode_ = CALL_PLAIN;
   call_gclass_ = 0;
   call_all_blur_ = false;
+  call_flipped_ = false;
+  call_flip_tail_ = false;
   return ok;
 }
 
@@ -1773,7 +1846,7 @@ double Engine::time_stage(int stage, int n, int iters, std::string* err) {
     if (stage == 0 || stage == 4) enqueue_pre(n, d_frames_, row, fbytes, yin);
     if (stage == 1 || stage == 4) enqueue_cnn(n, true);
     if (stage == 2 || stage == 4) enqueue_decision(n);
-    if (stage == 3 || stage == 4) enqueue_post(n, d_frames_, row, fbytes, d_out_, fbytes, d_yuyv_, npix * 2, d_mask_, npix, yin);
+    if (stage == 3 || stage == 4) (void)enqueue_post(n, d_frames_, row, fbytes, d_out_, fbytes, d_yuyv_, npix * 2, d_mask_, npix, yin);
   };
   once();                                   // warm-up (instruction cache, tables)
   cudaStreamSynchronize(stream_);

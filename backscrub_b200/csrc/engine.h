@@ -114,6 +114,9 @@ class Engine {
   // the context), 0 or odd 1..255
   enum { SRC_BG_DEFAULT = 0, SRC_BG_NONE = 1 };
   bool set_source_effect(int source, int background, int bgblur, std::string* err);
+  // mirroring of one source: -1 follows set_output's flips, 0..3 its own (bit 0 horizontal, bit 1 vertical).  Host
+  // bookkeeping only: the flip reaches the device through the per-frame table of each call.
+  bool set_source_flip(int source, int flip, std::string* err);
   // frame b belongs to source ids[b] (HOST array of n distinct ids); same buffers / layout as run()
   bool run_sources(int n, const int* ids, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
                    uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, std::string* err,
@@ -147,7 +150,9 @@ class Engine {
   void out_hwc(int* v) const { v[0] = oh_; v[1] = ow_; v[2] = oc_; }
   double flops() const { return flops_; }
   int launches_per_call() const {
-    if (last_call_launches_ > 0) return last_call_launches_;      // counted while the last call was enqueued / captured
+    // counted while the last call was enqueued / captured (a replay restores its graph's count, so a sources call reports
+    // whether its tail mirrors frames)
+    if (last_call_launches_ > 0) return last_call_launches_;
     int n = 4;
     for (const Step& s : steps_) n += s.launches();
     if (bgblur_k_ && !has_bg_) n += 2;
@@ -180,13 +185,26 @@ class Engine {
                      uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in) const;
   bool yuyv_native(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
                    uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in) const;
-  void enqueue_all(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
+  // the call ends with a stand-alone tail (post -> stage -> flip -> resize -> YUYV): plain calls with a context flip or
+  // resize; sources calls with a resize, or with mirrored frames the post kernel cannot mirror in place
+  bool call_tail() const {
+    const bool resized = out_w_ != W_ || out_h_ != H_;
+    return call_mode_ == CALL_PLAIN ? (flip_h_ || flip_v_ || resized) : (resized || call_flip_tail_);
+  }
+  bool nv12_staged(bool native, const uint8_t* d_yuyv) const;
+  PostArgs call_post_args(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv,
+                          size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in, bool native) const;
+  // sources calls with flipped frames: sets call_flip_tail_ (and grows the tail's staging when it is needed)
+  bool plan_flips(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv,
+                  size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in, std::string* err);
+  // false (nothing more enqueued) only when the post kernel cannot write a call's mirrored frames
+  bool enqueue_all(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
                    uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in,
                    bool native, bool sync_cbs);
   bool refresh_bg_yuyv(std::string* err);
   void enqueue_cnn(int n, bool from_u8);
   void enqueue_decision(int n);
-  void enqueue_post(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
+  bool enqueue_post(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
                     uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in = nullptr);
   // base of tensor t for the frames [frame_off_, ...) of the batch (frame_off_ != 0 only inside a sub-batched segment)
   float* tptr(int t) const {
@@ -306,10 +324,13 @@ class Engine {
   int call_mode_ = CALL_PLAIN;
   unsigned call_gclass_ = 0;
   bool call_all_blur_ = false;       // ... and every frame of the call blurs its camera frame (the BGR frames are materialised)
+  bool call_flipped_ = false;        // ... and some frame of the call is mirrored (the table's flip row is not all 0)
+  bool call_flip_tail_ = false;      // ... and its tail mirrors them (k_flip_u8c3_frames): the call resizes or its post kernel is
+                                     // not k_post_tma (plan_flips)
   int n_sources_ = 0;
   uint8_t* src_state_ = nullptr;     // [n_sources][oh*ow] smoother state per source
-  // [3][max_batch]: source id of frame b | background-bank slot of frame b | camera-blur strength of frame b (0 = none),
-  // written before each launch
+  // [4][max_batch]: source id of frame b | background-bank slot of frame b | camera-blur strength of frame b (0 = none) |
+  // flip code of frame b (bit 0 horizontal, bit 1 vertical; the source's own, or the context's), written before each launch
   int* d_src_tab_ = nullptr;
   // background bank, one base + one stride for the post kernel: [max_batch] camera-blur slots | [1] the context's effective
   // background | [n_sources] source slots; d_bank_yuyv_ is its YUYV and d_bank_nv12_ its NV12 (the camera-blur slots'
@@ -324,6 +345,7 @@ class Engine {
   std::vector<char> src_has_bg_;
   struct SrcEffect { int bg = SRC_BG_DEFAULT, k = -1; };
   std::vector<SrcEffect> src_fx_;
+  std::vector<signed char> src_flip_;   // per source: -1 = the context's flips (flip_h_ / flip_v_), else 0..3
   // Where source s's background comes from: the context slot, its own bank slot (its effective still background differs
   // from the context's), or its camera frame blurred at strength *k
   enum SrcBg { SRC_FROM_CTX = 0, SRC_FROM_SLOT = 1, SRC_FROM_CAMBLUR = 2 };
@@ -343,14 +365,17 @@ class Engine {
     unsigned gclass;                 // call_gclass_: the Gaussian launches captured (strengths within them replay)
     bool all_blur;                   // call_all_blur_: the camera frames were converted to BGR before the graph's kernels
     bool nv12; size_t npitch, nuv, nstride;   // NV12 call and its input layout: never confused with a YUYV call
+    bool flipped;                    // call_flipped_: the post kernel mirrors in place, or the tail contains the per-frame flip
+                                     // (decided from the rest of the key); which frames flip is table data
     bool operator<(const GraphKey& r) const {
-      return std::tie(n, f, pitch, stride, o, y, m, yin, ostride, ystride, mstride, mode, gclass, all_blur, nv12, npitch, nuv, nstride) <
+      return std::tie(n, f, pitch, stride, o, y, m, yin, ostride, ystride, mstride, mode, gclass, all_blur, nv12, npitch, nuv, nstride, flipped) <
              std::tie(r.n, r.f, r.pitch, r.stride, r.o, r.y, r.m, r.yin, r.ostride, r.ystride, r.mstride, r.mode, r.gclass, r.all_blur, r.nv12, r.npitch, r.nuv,
-                      r.nstride);
+                      r.nstride, r.flipped);
     }
   };
 #ifndef BSB_EMU
-  std::map<GraphKey, cudaGraphExec_t> graphs_;
+  struct CapturedCall { cudaGraphExec_t exec; int launches; };
+  std::map<GraphKey, CapturedCall> graphs_;
 #endif
 };
 

@@ -248,8 +248,12 @@ struct PostArgs {
   // per tile row / tile column: the patch of the small mask a (TW + 4) x 36 halo tile touches, {first, count}
   // (precomputed once per context from `tab`: the patch request is the head of every CTA's critical path)
   const int2* geo_rows; const int2* geo_cols64; const int2* geo_cols128;
+  // TMA path only: non-null (DEVICE [B]): frame b's out / YUYV / NV12 are written mirrored by flip[b] (bit 0 horizontally,
+  // bit 1 vertically; 0 = as is).  The mask is never mirrored.  launch_post refuses it where k_post_tma cannot run.
+  const int* flip;
 };
-void launch_post(cudaStream_t s, const PostArgs& a);
+// false (nothing launched) when a.flip is set and k_post_tma cannot take the arguments
+bool launch_post(cudaStream_t s, const PostArgs& a);
 // true if launch_post will take the TMA kernel for these arguments (the only one that can read a.yuyv_in / a.nv12_in)
 bool post_tma_eligible(const PostArgs& a);
 
@@ -282,6 +286,8 @@ bool launch_gauss_frames(cudaStream_t s, int n, const GaussSrc& cam, const int* 
                          uint8_t* dst, uint8_t* dst_yuyv, uint8_t* dst_nv12, int W, int H);
 // app/deepseg.cc:667-673: cv::flip on n packed frames
 void launch_flip_u8c3(cudaStream_t s, int n, const uint8_t* src, size_t sstride, uint8_t* dst, size_t dstride, int W, int H, bool flip_h, bool flip_v);
+// the same per frame: frame b flipped by flip[b] (DEVICE [n]; bit 0 horizontally, bit 1 vertically), copied when it is 0
+void launch_flip_u8c3_frames(cudaStream_t s, int n, const uint8_t* src, size_t sstride, uint8_t* dst, size_t dstride, int W, int H, const int* flip);
 
 // cv::cvtColor(COLOR_YUV2BGR_YUYV): camera YUYV frames -> BGR (what cv::VideoCapture does for the
 // reference, app/deepseg.cc:553).  n frames of W x H, tightly packed.

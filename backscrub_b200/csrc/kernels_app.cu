@@ -464,6 +464,24 @@ void launch_flip_u8c3(cudaStream_t s, int n, const uint8_t* src, size_t sstride,
   count_launch();
 }
 
+// per-frame variant (sources calls): frame b flipped by flip[b], copied when 0, so the resize that follows sees every frame
+__global__ void __launch_bounds__(256) k_flip_u8c3_frames(const uint8_t* src, size_t sstride, uint8_t* dst, size_t dstride, int W, int H,
+                                                          const int* flip) {
+  const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= (size_t)W * H) return;
+  const int fl = __ldg(flip + blockIdx.y);
+  const int x = (int)(p % W), y = (int)(p / W);
+  const uint8_t* sp = src + (size_t)blockIdx.y * sstride + ((size_t)((fl & 2) ? H - 1 - y : y) * W + ((fl & 1) ? W - 1 - x : x)) * 3;
+  uint8_t* dp = dst + (size_t)blockIdx.y * dstride + 3 * p;
+  dp[0] = sp[0]; dp[1] = sp[1]; dp[2] = sp[2];
+}
+
+void launch_flip_u8c3_frames(cudaStream_t s, int n, const uint8_t* src, size_t sstride, uint8_t* dst, size_t dstride, int W, int H, const int* flip) {
+  const size_t npix = (size_t)W * H;
+  BSB_LAUNCH(k_flip_u8c3_frames, dim3((unsigned)((npix + 255) / 256), (unsigned)n), dim3(256), 0, s, src, sstride, dst, dstride, W, H, flip);
+  count_launch();
+}
+
 __global__ void k_advance_cursor(int* cursor, int step, int count) { *cursor = (int)(((unsigned)*cursor + (unsigned)step) % (unsigned)count); }
 
 void launch_advance_cursor(cudaStream_t s, int* cursor, int step, int count) {

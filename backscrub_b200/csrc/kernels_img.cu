@@ -742,8 +742,10 @@ static bool post_fast_ok(const PostArgs& a) {
 
 bool launch_post_tma(cudaStream_t s, const PostArgs& a);   // kernels_post.cu
 
-void launch_post(cudaStream_t s, const PostArgs& a_in) {
-  if (launch_post_tma(s, a_in)) return;
+bool launch_post(cudaStream_t s, const PostArgs& a_in) {
+  if (launch_post_tma(s, a_in)) return true;
+  // only k_post_tma writes mirrored frames: a flip table it could not take is an error, never unmirrored output
+  if (a_in.flip) return false;
   PostArgs a = a_in;
   a.frame_l1 = tuning().post_l1;                 // measurement switch: frame loads allocate in L1
   if (post_fast_ok(a)) {
@@ -753,11 +755,12 @@ void launch_post(cudaStream_t s, const PostArgs& a_in) {
     else if (a.out) { auto k = k_post_fast<true, false>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
     else { auto k = k_post_fast<false, false>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
     count_launch();
-    return;
+    return true;
   }
   dim3 grid((unsigned)ceil_div(a.W, PT_W), (unsigned)ceil_div(a.H, PT_H), (unsigned)a.B);
   BSB_LAUNCH(k_post, grid, dim3(256), 0, s, a);
   count_launch();
+  return true;
 }
 
 // ---------------------------------------------------------------------------

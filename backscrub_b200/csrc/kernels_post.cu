@@ -12,7 +12,9 @@
 //                         (the camera frame is not even read),
 //       person tile:      out <- frame tile (camera YUYV converted per thread when the frames are in wire format),
 //       mixed tile:       the k_post_fast arithmetic on shared-memory operands;
-//   * results are staged in shared memory and leave with TMA stores.
+//   * results are staged in shared memory and leave with TMA stores;
+//   * a frame with a flip code (PostArgs::flip, sources calls) is written mirrored: each thread puts its 16 pixels,
+//     reversed, into the mirrored slot of the staging tiles, and the stores go to the mirrored box.
 // Arithmetic is shared with k_post_fast through post_math.h, so both kernels produce the oracle's bits.
 #include "kernels.h"
 #include "post_math.h"
@@ -57,6 +59,40 @@ BSB_D void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" :
 BSB_D void prefetch_map(const CUtensorMap* map) { asm volatile("prefetch.tensormap [%0];" :: "l"(map) : "memory"); }
 }  // namespace tma
 
+// 16 pixels in reversed order: BGR (12 words; four groups of 4 pixels = 3 words, each group's pixels reversed), YUYV
+// (8 words of 2 pixels: word order reversed, Y0 / Y1 swapped; a pair's U / V are a symmetric average and stay), 16 Y
+// bytes, 4 UV pairs (2-byte units)
+BSB_D void rev_bgr16(const unsigned* s, unsigned* d) {
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    const unsigned A = s[3 * (3 - q)], B = s[3 * (3 - q) + 1], C = s[3 * (3 - q) + 2];   // p0 p0 p0 p1 | p1 p1 p2 p2 | p2 p3 p3 p3
+    d[3 * q] = __byte_perm(C, B, 0x6321);
+    d[3 * q + 1] = __byte_perm(__byte_perm(B, C, 0x0043), A, 0x3710);
+    d[3 * q + 2] = __byte_perm(A, B, 0x2105);
+  }
+}
+BSB_D void rev_yuyv16(const unsigned* s, unsigned* d) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) d[j] = __byte_perm(s[7 - j], 0, 0x3012);
+}
+BSB_D uint4 rev_y16(uint4 v) {
+  return make_uint4(__byte_perm(v.w, 0, 0x0123), __byte_perm(v.z, 0, 0x0123), __byte_perm(v.y, 0, 0x0123), __byte_perm(v.x, 0, 0x0123));
+}
+BSB_D uint2 rev_uv4(uint2 v) { return make_uint2(__byte_perm(v.y, 0, 0x1032), __byte_perm(v.x, 0, 0x1032)); }
+
+// A staged tile of `rows` rows of RB bytes whose box starts at byte column gx / row gy of a frame with fb-byte rows
+// (`pitch` apart) and fh rows, stored by every thread with 16-byte stores, clipped to the frame.  Mirrored boxes of ragged
+// edge tiles start at negative coordinates, which the TMA store does not take; gx and fb are multiples of 16.
+template <int NT, int RB>
+BSB_D void store_clipped(const uint8_t* src, int rows, uint8_t* dst, size_t pitch, int gx, int gy, int fb, int fh, int tid) {
+  constexpr int CPR = RB / 16;                       // 16-byte chunks per row
+  for (int i = tid; i < rows * CPR; i += NT) {
+    const int r = i / CPR, c = (i % CPR) * 16, x = gx + c, y = gy + r;
+    if (x >= 0 && x < fb && y >= 0 && y < fh)
+      *reinterpret_cast<uint4*>(dst + (size_t)y * pitch + x) = *reinterpret_cast<const uint4*>(src + r * RB + c);
+  }
+}
+
 struct PostMaps { CUtensorMap frame, bg, bgy, out, yuyv, mask, ofinal; };
 // NV12 calls: frame / bgy / yuyv are the Y planes of the camera frames, the background NV12 and the NV12 output; these are
 // their UV planes
@@ -98,8 +134,9 @@ template <int TW> struct PtL {
                 (SMEM + 1024) * CTAS <= 228 * 1024, "smem layout");
 };
 
-// FMT: IN_BGR / IN_YUYV frames with YUYV video output, or IN_NV12 frames with NV12 video output
-template <int FMT, int TW>
+// FMT: IN_BGR / IN_YUYV frames with YUYV video output, or IN_NV12 frames with NV12 video output.  FLIP: the launch has a
+// flip table (sources calls); without one the kernel is compiled without the mirroring paths.
+template <int FMT, int TW, bool FLIP>
 __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const __grid_constant__ PostMapsOf<FMT> tm, const PostArgs a, const PostTmaCfg cfg) {
   using L = PtL<TW>;
   constexpr bool IN_YUYV = FMT == InFmt::IN_YUYV, NV12 = FMT == InFmt::IN_NV12;
@@ -148,6 +185,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
     if (a.bg_index) bgi = __ldg(a.bg_index + b);
     else if (a.bg_cursor) bgi = (int)(((unsigned)__ldg(a.bg_cursor) + (unsigned)b * (unsigned)a.bg_advance) % (unsigned)a.bg_count);
     else if (a.bg_stride) bgi = b;
+    if (FLIP) geo[9] = __ldg(a.flip + b);             // the frame's flip code, read by every thread after the first barrier
     tma::mbar_expect_tx(barB, (unsigned)L::F_BYTES + (cfg.has_bgy ? (NV12 ? (unsigned)L::N_BYTES : (unsigned)L::Y_BYTES) : 0u));
     tma::load_3d(sB, &tm.bg, blockIdx.x * (TW * 3 / 4), ty0, bgi, barB);
     if constexpr (NV12) {
@@ -277,14 +315,68 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
 
   // a background tile with a cached YUYV copy is moved by the copy engine alone: only thread 0 (which issues the stores)
   // waits for the background tiles, and for the (speculatively loaded, unused) camera tile after the stores are on their
-  // way — shared memory must be quiet when the CTA exits
-  const bool engine_only = kind == 0 && !(cfg.has_yuyv && !cfg.has_bgy);
+  // way — shared memory must be quiet when the CTA exits.  A mirrored frame's background tile is reversed by the threads.
+  const bool bg_copy = kind == 0 && !(cfg.has_yuyv && !cfg.has_bgy);
+  const bool engine_only = bg_copy && !(FLIP && geo[9]);
   if (!engine_only) tma::mbar_wait(barB, 0);
   if (hits_roi && kind != 0) tma::mbar_wait(barF, 0);
   if (kind == 0) {
     // ---- background tile: out = background tile, YUYV = cached YUYV tile, mask = 255.  No per-pixel arithmetic ----
     if (cfg.has_mask) *mdst = make_uint4(0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu);
-    if (cfg.has_yuyv && !cfg.has_bgy) {
+    const int fl = FLIP ? geo[9] : 0;
+    if (fl) {
+      // mirrored frame: every thread reads its chunk of the staged tiles (the YUYV converted from the background when
+      // there is no cached copy), and after a barrier writes it reversed to the mirrored slot — in place, since every
+      // slot is read before any is written
+      const int mx = (fl & 1) ? TW - PF_PX - lx : lx, my = (fl & 2) ? PF_H - 1 - ly : ly;
+      const int ur = tid / (TW / 8), uq = tid % (TW / 8);            // NV12 UV tile: 8 bytes (4 pairs) per thread
+      const uint4* gq = reinterpret_cast<const uint4*>(sB + ly * (TW * 3) + lx * 3);
+      const uint4 g0 = gq[0], g1 = gq[1], g2 = gq[2];
+      unsigned gg[12] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w, g2.x, g2.y, g2.z, g2.w};
+      unsigned yy[8];
+      if (cfg.has_yuyv && !cfg.has_bgy) {
+        unsigned m[PF_PX], o[12];
+#pragma unroll
+        for (int i = 0; i < PF_PX; ++i) m[i] = 255u;
+        post_blend16<false, true>(gg, gg, m, o, yy);
+      } else if (NV12) {
+        const uint4 yq = *reinterpret_cast<const uint4*>(sY + ly * TW + lx);
+        const uint2 cq = *reinterpret_cast<const uint2*>(sY + TW * PF_H + ur * TW + 8 * uq);
+        yy[0] = yq.x; yy[1] = yq.y; yy[2] = yq.z; yy[3] = yq.w; yy[4] = cq.x; yy[5] = cq.y;
+      } else {
+        const uint4 y0 = ydst[0], y1 = ydst[1];
+        yy[0] = y0.x; yy[1] = y0.y; yy[2] = y0.z; yy[3] = y0.w; yy[4] = y1.x; yy[5] = y1.y; yy[6] = y1.z; yy[7] = y1.w;
+      }
+      __syncthreads();
+      if (cfg.has_out) {
+        unsigned r[12];
+        if (fl & 1) rev_bgr16(gg, r);
+        else {
+#pragma unroll
+          for (int i = 0; i < 12; ++i) r[i] = gg[i];
+        }
+        uint4* bq = reinterpret_cast<uint4*>(sB + my * (TW * 3) + mx * 3);
+        bq[0] = make_uint4(r[0], r[1], r[2], r[3]); bq[1] = make_uint4(r[4], r[5], r[6], r[7]); bq[2] = make_uint4(r[8], r[9], r[10], r[11]);
+      }
+      if (cfg.has_yuyv) {
+        if (NV12 && cfg.has_bgy) {
+          const uint4 yq = make_uint4(yy[0], yy[1], yy[2], yy[3]);
+          const uint2 cq = make_uint2(yy[4], yy[5]);
+          *reinterpret_cast<uint4*>(sY + my * TW + mx) = (fl & 1) ? rev_y16(yq) : yq;
+          *reinterpret_cast<uint2*>(sY + TW * PF_H + ((fl & 2) ? PF_H / 2 - 1 - ur : ur) * TW + ((fl & 1) ? TW - 8 - 8 * uq : 8 * uq)) =
+              (fl & 1) ? rev_uv4(cq) : cq;
+        } else {
+          unsigned r[8];
+          if (fl & 1) rev_yuyv16(yy, r);
+          else {
+#pragma unroll
+            for (int i = 0; i < 8; ++i) r[i] = yy[i];
+          }
+          uint4* yq = reinterpret_cast<uint4*>(sY + my * (TW * 2) + mx * 2);
+          yq[0] = make_uint4(r[0], r[1], r[2], r[3]); yq[1] = make_uint4(r[4], r[5], r[6], r[7]);
+        }
+      }
+    } else if (cfg.has_yuyv && !cfg.has_bgy) {
       const uint4* gq = reinterpret_cast<const uint4*>(sB + ly * (TW * 3) + lx * 3);
       const uint4 g0 = gq[0], g1 = gq[1], g2 = gq[2];
       const unsigned gg[12] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w, g2.x, g2.y, g2.z, g2.w};
@@ -335,19 +427,38 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
     }
     unsigned o[12], yy[8];
     post_blend16<true, true>(f, gg, m, o, yy);
-    // the YUYV camera tile is fully consumed before the (wider) BGR tile overwrites it; the mask staging tile reuses Us,
-    // whose last readers (phase B) are behind a barrier already
-    if (IN_YUYV || NV12) __syncthreads();
-    uint4* odst = reinterpret_cast<uint4*>(sF + ly * (TW * 3) + lx * 3);
-    odst[0] = make_uint4(o[0], o[1], o[2], o[3]); odst[1] = make_uint4(o[4], o[5], o[6], o[7]); odst[2] = make_uint4(o[8], o[9], o[10], o[11]);
-    ydst[0] = make_uint4(yy[0], yy[1], yy[2], yy[3]); ydst[1] = make_uint4(yy[4], yy[5], yy[6], yy[7]);
+    // the YUYV camera tile is fully consumed before the (wider) BGR tile overwrites it, and a mirrored frame's camera tile
+    // before any thread writes another's slot; the mask staging tile reuses Us, whose last readers (phase B) are behind a
+    // barrier already
+    const int fl = FLIP ? geo[9] : 0;
+    if (IN_YUYV || NV12 || fl) __syncthreads();
+    if (fl) {
+      // mirrored frame: the thread's 16 pixels, reversed when horizontal, go to the mirrored slot
+      const int mx = (fl & 1) ? TW - PF_PX - lx : lx, my = (fl & 2) ? PF_H - 1 - ly : ly;
+      unsigned ro[12], ry[8];
+      if (fl & 1) { rev_bgr16(o, ro); rev_yuyv16(yy, ry); }
+      else {
+#pragma unroll
+        for (int i = 0; i < 12; ++i) ro[i] = o[i];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) ry[i] = yy[i];
+      }
+      uint4* odst = reinterpret_cast<uint4*>(sF + my * (TW * 3) + mx * 3);
+      odst[0] = make_uint4(ro[0], ro[1], ro[2], ro[3]); odst[1] = make_uint4(ro[4], ro[5], ro[6], ro[7]); odst[2] = make_uint4(ro[8], ro[9], ro[10], ro[11]);
+      uint4* yq = reinterpret_cast<uint4*>(sY + my * (TW * 2) + mx * 2);
+      yq[0] = make_uint4(ry[0], ry[1], ry[2], ry[3]); yq[1] = make_uint4(ry[4], ry[5], ry[6], ry[7]);
+    } else {
+      uint4* odst = reinterpret_cast<uint4*>(sF + ly * (TW * 3) + lx * 3);
+      odst[0] = make_uint4(o[0], o[1], o[2], o[3]); odst[1] = make_uint4(o[4], o[5], o[6], o[7]); odst[2] = make_uint4(o[8], o[9], o[10], o[11]);
+      ydst[0] = make_uint4(yy[0], yy[1], yy[2], yy[3]); ydst[1] = make_uint4(yy[4], yy[5], yy[6], yy[7]);
+    }
     *mdst = make_uint4(m[0] | (m[1] << 8) | (m[2] << 16) | (m[3] << 24), m[4] | (m[5] << 8) | (m[6] << 16) | (m[7] << 24),
                        m[8] | (m[9] << 8) | (m[10] << 16) | (m[11] << 24), m[12] | (m[13] << 8) | (m[14] << 16) | (m[15] << 24));
     out_src = sF;
   }
   const uint8_t* nv_src = sY;          // NV12 calls: the tile the NV12 stores read (the cached background, else sN)
   if constexpr (NV12) {
-    if (cfg.has_yuyv && !engine_only) {
+    if (cfg.has_yuyv && !bg_copy) {
       // YUYV tile -> NV12: each thread takes 4 pairs of a row pair, copies the 8 + 8 Y bytes and averages the two rows'
       // U / V bytes with a per-byte truncating halving add (the NV12 output definition)
       __syncthreads();
@@ -363,16 +474,37 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
   }
   tma::fence_proxy_async();            // generic-proxy writes of the staging tiles -> visible to the TMA engine
   __syncthreads();
-  if (tid == 0) {
-    if (engine_only) tma::mbar_wait(barB, 0);
-    if (cfg.has_out) tma::store_3d(&tm.out, out_src, blockIdx.x * (TW * 3 / 4), ty0, b);
+  // the tile's box, or for a mirrored frame the mirrored box (x = W - tx0 - TW, y = H - ty0 - 32, the UV plane's
+  // H/2 - ty0/2 - 16).  x stays a multiple of 16 pixels (W % 16 == 0), so every box starts 16-byte aligned.  At ragged
+  // edges the mirrored box starts at a negative coordinate: the threads store it, dropping exactly the rows / columns that
+  // came from outside the frame.
+  const int fl = FLIP ? geo[9] : 0;
+  const int sx = (fl & 1) ? a.W - tx0 - TW : tx0, sy = (fl & 2) ? a.H - ty0 - PF_H : ty0;
+  const bool clipped = FLIP && (sx < 0 || sy < 0);
+  if (clipped) {
+    if (cfg.has_out) store_clipped<NT, TW * 3>(out_src, PF_H, a.out + (size_t)b * a.out_stride, a.out_pitch, sx * 3, sy, a.W * 3, a.H, tid);
     if constexpr (NV12) {
       if (cfg.has_yuyv) {
-        tma::store_3d(&tm.yuyv, nv_src, blockIdx.x * (TW / 4), ty0, b);
-        tma::store_3d(&tm.yuyv_uv, nv_src + TW * PF_H, blockIdx.x * (TW / 4), ty0 / 2, b);
+        uint8_t* d = a.nv12 + (size_t)b * a.nv12_stride;
+        store_clipped<NT, TW>(nv_src, PF_H, d, (size_t)a.W, sx, sy, a.W, a.H, tid);
+        store_clipped<NT, TW>(nv_src + TW * PF_H, PF_H / 2, d + (size_t)a.W * a.H, (size_t)a.W, sx, sy / 2, a.W, a.H / 2, tid);
       }
     } else {
-      if (cfg.has_yuyv) tma::store_3d(&tm.yuyv, sY, blockIdx.x * (TW / 2), ty0, b);
+      if (cfg.has_yuyv) store_clipped<NT, TW * 2>(sY, PF_H, a.yuyv + (size_t)b * a.yuyv_stride, (size_t)a.W * 2, sx * 2, sy, a.W * 2, a.H, tid);
+    }
+  }
+  if (tid == 0) {
+    if (engine_only) tma::mbar_wait(barB, 0);
+    if (!clipped) {
+      if (cfg.has_out) tma::store_3d(&tm.out, out_src, sx / 4 * 3, sy, b);
+      if constexpr (NV12) {
+        if (cfg.has_yuyv) {
+          tma::store_3d(&tm.yuyv, nv_src, sx / 4, sy, b);
+          tma::store_3d(&tm.yuyv_uv, nv_src + TW * PF_H, sx / 4, sy / 2, b);
+        }
+      } else {
+        if (cfg.has_yuyv) tma::store_3d(&tm.yuyv, sY, sx / 2, sy, b);
+      }
     }
     if (cfg.has_mask) tma::store_3d(&tm.mask, sM, tx0, ty0, b);
     tma::store_commit();
@@ -484,13 +616,17 @@ bool post_tma_eligible(const PostArgs& a) {
   return post_tma_shape_ok(a) && build_post_maps(a, &tm, post_tile_width(a), &tm);
 }
 
+template <int FMT, int TW, bool FLIP>
+static bool launch_post_tma_f(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
+  using L = PtL<TW>;
+  if (!ensure_dyn_smem(reinterpret_cast<const void*>(k_post_tma<FMT, TW, FLIP>), L::SMEM)) return false;
+  const dim3 grid((unsigned)ceil_div(a.W, TW), (unsigned)ceil_div(a.H, PF_H), (unsigned)a.B);
+  k_post_tma<FMT, TW, FLIP><<<grid, L::NT, L::SMEM, s>>>(tm, a, cfg);
+  return true;
+}
 template <int FMT, int TW>
 static bool launch_post_tma_t(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
-  using L = PtL<TW>;
-  if (!ensure_dyn_smem(reinterpret_cast<const void*>(k_post_tma<FMT, TW>), L::SMEM)) return false;
-  const dim3 grid((unsigned)ceil_div(a.W, TW), (unsigned)ceil_div(a.H, PF_H), (unsigned)a.B);
-  k_post_tma<FMT, TW><<<grid, L::NT, L::SMEM, s>>>(tm, a, cfg);
-  return true;
+  return a.flip ? launch_post_tma_f<FMT, TW, true>(s, tm, a, cfg) : launch_post_tma_f<FMT, TW, false>(s, tm, a, cfg);
 }
 
 bool launch_post_tma(cudaStream_t s, const PostArgs& a) {

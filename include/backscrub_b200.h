@@ -109,7 +109,8 @@ BSB_API int bsb_set_background_cursor(bsb_ctx* ctx, int index);
 BSB_API int bsb_set_bgblur(bsb_ctx* ctx, int ksize);
 /* `-H`/`-V` cv::flip of the composited frame (:667-673) and cv::resize to the virtual-camera geometry when it
  * differs from the capture geometry (:677-679); both before the YUYV conversion.  out_w/out_h <= 0 = frame size.
- * After this call `out` buffers are out_w x out_h x 3 and `out_yuyv` out_w x out_h x 2; the mask stays W x H. */
+ * After this call `out` buffers are out_w x out_h x 3 and `out_yuyv` out_w x out_h x 2; the mask stays W x H.
+ * The flips are the default of every source of a sources call (bsb_set_source_flip); the output size is per context. */
 BSB_API int bsb_set_output(bsb_ctx* ctx, int flip_h, int flip_v, int out_w, int out_h);
 BSB_API int bsb_output_size(bsb_ctx* ctx, int* out_w, int* out_h);
 
@@ -183,7 +184,8 @@ BSB_API int bsb_composite_nv12(bsb_ctx* ctx, int n_frames, const uint8_t* nv12, 
  * background (bsb_set_background, or the green default), blurred when bgblur is on; else, with
  * bgblur on and no background of either kind, its own blurred camera frame (app/deepseg.cc:652-658).
  * That is the default effect of every source; bsb_set_source_effect changes it per source.
- * bsb_set_output applies to every frame; callbacks do not fire; the context
+ * bsb_set_output's size applies to every frame, its flips to every source without its own
+ * (bsb_set_source_flip); callbacks do not fire; the context
  * background must not be a ring of more than one image.  Plain calls never touch the per-source
  * states and sources calls never touch the plain smoother state, so both can be mixed on one
  * context.  A violated rule returns 0 with a bsb_last_error() message and leaves the context usable. */
@@ -204,13 +206,24 @@ BSB_API int bsb_set_source_background(bsb_ctx* ctx, int source, const uint8_t* b
  *                                     the strength is > 0, else plain green (the source's own image is kept,
  *                                     unused, until DEFAULT again).
  * bgblur:     -1 = follow the context (bsb_set_bgblur, including later changes), 0 = off, odd 1..255.
- * bsb_set_sources resets every source to (DEFAULT, -1).  bsb_set_output and the camera-blur mode of plain calls stay
- * per context.  An unknown background, an even / out-of-range strength, a source id out of range or no
+ * bsb_set_sources resets every source to (DEFAULT, -1).  The output size of bsb_set_output and the camera-blur mode
+ * of plain calls stay per context.  An unknown background, an even / out-of-range strength, a source id out of range or no
  * bsb_set_sources yet return 0 with a bsb_last_error() message.
  * Cost: bsb_set_background and bsb_set_bgblur refresh the still background of every source except one with its own
  * image at a fixed strength (a Gaussian for each such source with a strength > 0; nothing is cached by strength). */
 enum { BSB_SOURCE_BG_DEFAULT = 0, BSB_SOURCE_BG_NONE = 1 };
 BSB_API int bsb_set_source_effect(bsb_ctx* ctx, int source, int background, int bgblur);
+/* Mirroring of one source (cv::flip, app/deepseg.cc:667-673, toggled at run time by the `h` / `v` keys, :785-790).
+ * flip: -1 = follow bsb_set_output's flips, including later changes; 0..3 = the source's own, a mask of BSB_FLIP_H
+ * (horizontal) and BSB_FLIP_V (vertical).  Frame b of a sources call, from source s, gives exactly the composite, YUYV /
+ * NV12 output and mask of a plain context set up the same way plus bsb_set_output(flip_h_s, flip_v_s, out_w, out_h).
+ * The mask is never flipped.  bsb_set_sources resets every source to -1.  Host bookkeeping only (no device work, no
+ * synchronisation), so it may be called per frame; the flips reach the device with the call's source table.  Without a
+ * resize, where the TMA post kernel takes the geometry, it writes the mirrored frames in place; otherwise they are
+ * flipped between the post kernel and the resize.  A flip outside -1..3, a source id out of range or no
+ * bsb_set_sources yet return 0 with a bsb_last_error() message. */
+enum { BSB_FLIP_H = 1, BSB_FLIP_V = 2 };
+BSB_API int bsb_set_source_flip(bsb_ctx* ctx, int source, int flip);
 /* HOST buffers, BGR frames, laid out as in bsb_composite (out rows tightly packed, `out_stride` bytes
  * per frame).  Any of out / out_yuyv / out_mask may be NULL. */
 BSB_API int bsb_composite_sources(bsb_ctx* ctx, int n_frames, const int* source_ids, const uint8_t* frames, size_t frame_pitch,
