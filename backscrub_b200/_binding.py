@@ -25,7 +25,7 @@ SYMBOLS = [
     "bsb_set_background_ring", "bsb_set_background_cursor", "bsb_set_bgblur", "bsb_set_output", "bsb_output_size",
     "bsb_gaussian_blur", "bsb_gaussian_taps", "bsb_flip",
     "bsb_composite", "bsb_composite_device", "bsb_composite_yuyv", "bsb_composite_yuyv_device", "bsb_composite_mjpg", "bsb_decode_mjpg", "bsb_convert_yuyv_to_bgr", "bsb_synchronize", "bsb_stream", "bsb_alpha_blend",
-    "bsb_convert_rgb_to_yuyv", "bsb_resize_u8c3", "bsb_pointwise", "bsb_time_pointwise", "bsb_geometry", "bsb_infer", "bsb_get_tensor",
+    "bsb_convert_rgb_to_yuyv", "bsb_resize_u8c3", "bsb_pointwise", "bsb_pointwise_ex", "bsb_time_pointwise", "bsb_geometry", "bsb_infer", "bsb_get_tensor", "bsb_get_tensor_frame", "bsb_tc_steps",
     "bsb_get_stage_u8", "bsb_reset_state", "bsb_time_stage", "bsb_launches_per_call", "bsb_total_launches", "bsb_model_flops", "bsb_set_tuning", "bsb_frame_size", "bsb_yuyv_native", "bsb_uses_tensor_cores",
     "bsb_calcmask_new", "bsb_calcmask_delete", "bsb_calcmask_set_input_frame", "bsb_calcmask_get_output_mask", "bsb_calcmask_timings",
     "bsb_calcmask_frames_done", "bsb_calcmask_mask_serial",
@@ -80,12 +80,18 @@ def bind(path: str) -> C.CDLL:
     L.bsb_convert_rgb_to_yuyv.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
     L.bsb_resize_u8c3.argtypes = [C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_int]
     L.bsb_pointwise.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+    L.bsb_pointwise_ex.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_long, C.c_long, C.c_int,
+                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_long, C.c_long, C.c_int,
+                                   C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_long, C.c_long, C.c_int]
     L.bsb_time_pointwise.restype = C.c_double
     L.bsb_time_pointwise.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
     L.bsb_geometry.argtypes = [C.c_void_p, i32p, i32p, i32p, i32p, i32p]
     L.bsb_infer.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
     L.bsb_get_tensor.restype = C.c_long
     L.bsb_get_tensor.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_long]
+    L.bsb_get_tensor_frame.restype = C.c_long
+    L.bsb_get_tensor_frame.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_long]
+    L.bsb_tc_steps.argtypes = [C.c_void_p, i32p, C.c_int]
     L.bsb_get_stage_u8.restype = C.c_long
     L.bsb_get_stage_u8.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_long]
     L.bsb_reset_state.argtypes = [C.c_void_p]

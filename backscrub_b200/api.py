@@ -338,12 +338,21 @@ class MaskGen:
             self._fail("bsb_infer")
         return out[0] if x.ndim == 3 else out
 
-    def tensor(self, index: int, count: int):
+    def tensor(self, index: int, count: int, frame: int = 0):
         buf = np.empty(count, np.float32)
-        n = self._lib.bsb_get_tensor(self._h, index, _ptr(buf), count)
+        n = self._lib.bsb_get_tensor_frame(self._h, index, frame, _ptr(buf), count)
         if n < 0:
-            self._fail("bsb_get_tensor")
+            self._fail("bsb_get_tensor_frame")
         return buf[:n] if n else None
+
+    def tc_steps(self) -> list:
+        """the 1x1 convolutions planned for the tensor cores: dicts of op, in, out, residual (-1: none), K, N, act1..3"""
+        n = self._lib.bsb_tc_steps(self._h, None, 0)
+        rows = (C.c_int * max(1, 9 * n))()
+        if n < 0 or self._lib.bsb_tc_steps(self._h, rows, n) != n:
+            self._fail("bsb_tc_steps")
+        keys = ("op", "in", "out", "residual", "K", "N", "act1", "act2", "act3")
+        return [dict(zip(keys, rows[9 * i:9 * i + 9])) for i in range(n)]
 
     def stage_u8(self, which: int, frame: int = 0) -> np.ndarray:
         shape = self.in_hwc if which in (0, 1) else self.out_hwc[:2]
@@ -435,13 +444,51 @@ def resize_u8c3(lib, src, dw, dh, device=0):
     return out
 
 
-def pointwise(lib, A, W, bias=None, act=0, use_tc=False, device=0, variant=None):
-    """1x1 convolution stage: A [M, K] x W [N, K]^T (+ bias, activation) on the GPU."""
-    A = np.ascontiguousarray(A, np.float32); W = np.ascontiguousarray(W, np.float32)
-    M, K = A.shape; N = W.shape[0]
+def pointwise(lib, A, W, bias=None, act=0, use_tc=False, device=0, variant=None, *, rows=None, a_off=0, ld_a=None,
+              residual=None, res_off=0, ld_res=None, act2=0, act3=0, out=None, out_off=0, ld_out=None):
+    """1x1 convolution stage: act3(act2(act(A [M, K] x W [N, K]^T + bias)) + residual) on the GPU.
+
+    Plain call: A is [M, K] and a new [M, N] array is returned.  With `ld_a`, A is a flat buffer and the operand is its
+    `rows` x K sub-matrix at element offset `a_off` with row pitch `ld_a`; the residual (flat, `res_off`, `ld_res`) and
+    the output (`out`, flat, `out_off`, `ld_out`) are described the same way.  `out` is updated in place and returned:
+    every element outside the written sub-matrix keeps its value."""
+    W = np.ascontiguousarray(W, np.float32)
+    N, K = W.shape
     b = np.ascontiguousarray(bias, np.float32) if bias is not None else None
-    out = np.empty((M, N), np.float32)
-    if not lib.bsb_pointwise(device, int(use_tc) if variant is None else int(variant), M, K, N, _ptr(A), _ptr(W), _ptr(b) if b is not None else None, act, _ptr(out)):
+    v = int(use_tc) if variant is None else int(variant)
+    A = np.ascontiguousarray(A, np.float32)
+    if ld_a is None:
+        if rows is not None or a_off or A.ndim != 2 or A.shape[1] != K:
+            raise ValueError("without ld_a, A is a plain [M, K] array: rows and a_off describe a flat buffer given with ld_a")
+        rows = A.shape[0]
+    elif rows is None or A.ndim != 1:
+        raise ValueError("with ld_a, A is a flat buffer and rows (the M of the sub-matrix) is required")
+    if out is None and (ld_out is not None or out_off):
+        raise ValueError("ld_out and out_off describe a caller's out buffer")
+    if residual is None and (ld_res is not None or res_off):
+        raise ValueError("ld_res and res_off describe a residual buffer")
+    if ld_a is None and residual is None and out is None and act2 == 0 and act3 == 0:
+        M = A.shape[0]
+        res = np.empty((M, N), np.float32)
+        if not lib.bsb_pointwise(device, v, M, K, N, _ptr(A), _ptr(W), _ptr(b) if b is not None else None, act, _ptr(res)):
+            raise BackscrubError(lib.bsb_last_error().decode())
+        return res
+    ld_a = K if ld_a is None else ld_a
+    M = int(rows)
+    a = np.ascontiguousarray(A, np.float32).reshape(-1)
+    if out is None:
+        out, ld_out = np.zeros(M * N, np.float32), N
+    if out.dtype != np.float32 or not out.flags.c_contiguous:
+        raise ValueError("out must be a contiguous float32 array")
+    ld_out = N if ld_out is None else ld_out
+    r = None
+    if residual is not None:
+        r = np.ascontiguousarray(residual, np.float32).reshape(-1)
+        ld_res = N if ld_res is None else ld_res
+    flat = out.reshape(-1)
+    if not lib.bsb_pointwise_ex(device, v, M, K, N, _ptr(a), a.size, a_off, ld_a, _ptr(W), _ptr(b) if b is not None else None,
+                                _ptr(r) if r is not None else None, r.size if r is not None else 0, res_off, ld_res or 0,
+                                act, act2, act3, _ptr(flat), flat.size, out_off, ld_out):
         raise BackscrubError(lib.bsb_last_error().decode())
     return out
 

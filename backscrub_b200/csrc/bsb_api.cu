@@ -729,18 +729,42 @@ int bsb_resize_u8c3(int device, const uint8_t* src, int sw, int sh, uint8_t* dst
 }
 
 int bsb_pointwise(int device, int variant, int M, int K, int N, const float* A, const float* W, const float* bias, int act, float* out) {
+  if (M <= 0 || K <= 0 || N <= 0) { g_last_error = "invalid argument"; return 0; }
+  return bsb_pointwise_ex(device, variant, M, K, N, A, (long)M * K, 0, K, W, bias, nullptr, 0, 0, 0, act, 0, 0, out, (long)M * N, 0, N);
+}
+
+int bsb_pointwise_ex(int device, int variant, int M, int K, int N, const float* A, long a_len, long a_off, int ld_a,
+                     const float* W, const float* bias, const float* res, long res_len, long res_off, int ld_res,
+                     int act1, int act2, int act3, float* out, long out_len, long out_off, int ld_out) {
   if (!A || !W || !out || M <= 0 || K <= 0 || N <= 0) { g_last_error = "invalid argument"; return 0; }
-  if (!stage_begin(device)) return 0;
-  DevBuf dA, dW, dW2, dB, dO;
-  if (!dA.alloc((size_t)M * K * 4) || !dO.alloc((size_t)M * N * 4) || (bias && !dB.alloc((size_t)N * 4))) { g_last_error = "cudaMalloc failed"; return 0; }
-  cudaMemcpy(dA.p, A, (size_t)M * K * 4, cudaMemcpyHostToDevice);
-  if (bias) cudaMemcpy(dB.p, bias, (size_t)N * 4, cudaMemcpyHostToDevice);
-  bsb::Epilogue e; e.bias = bias ? (const float*)dB.p : nullptr; e.act1 = act;
+  // every element the kernel may touch lies inside its buffer
+  auto spans = [](long len, long off, int ld, int rows, int cols) { return off >= 0 && ld >= cols && off + (long)(rows - 1) * ld + cols <= len; };
+  if (!spans(a_len, a_off, ld_a, M, K) || !spans(out_len, out_off, ld_out, M, N) || (res && !spans(res_len, res_off, ld_res, M, N))) {
+    g_last_error = "sub-matrix outside its buffer"; return 0;
+  }
   const bool use_tc = variant == 1;
+  if (!use_tc && (a_off % 4 || out_off % 4)) { g_last_error = "the exact kernels need A and out on 16-byte boundaries"; return 0; }
+  if (!stage_begin(device)) return 0;
+  DevBuf dA, dW, dW2, dB, dO, dR;
+  if (!dA.alloc((size_t)a_len * 4) || !dO.alloc((size_t)out_len * 4) || (bias && !dB.alloc((size_t)N * 4)) || (res && !dR.alloc((size_t)res_len * 4))) {
+    g_last_error = "cudaMalloc failed"; return 0;
+  }
+  cudaMemcpy(dA.p, A, (size_t)a_len * 4, cudaMemcpyHostToDevice);
+  cudaMemcpy(dO.p, out, (size_t)out_len * 4, cudaMemcpyHostToDevice);
+  if (bias) cudaMemcpy(dB.p, bias, (size_t)N * 4, cudaMemcpyHostToDevice);
+  if (res) cudaMemcpy(dR.p, res, (size_t)res_len * 4, cudaMemcpyHostToDevice);
+  const float* dAm = (const float*)dA.p + a_off;
+  float* dOm = (float*)dO.p + out_off;
+  bsb::Epilogue e; e.bias = bias ? (const float*)dB.p : nullptr; e.act1 = act1; e.act2 = act2; e.act3 = act3;
+  if (res) { e.residual = (const float*)dR.p + res_off; e.ld_res = ld_res; }
   if (use_tc) {
+    const int kpad = (K + 31) / 32 * 32;
+    if (const char* why = bsb::pointwise_tc_refusal(K, dAm, ld_a, kpad, dOm, ld_out, e)) {
+      g_last_error = std::string("the tensor-core kernel refuses this call: ") + why; return 0;
+    }
     const int bn = bsb::pointwise_tc_tile_n(N);
-    if (bn <= 0 || K % 4) { g_last_error = "shape not supported by the tensor-core kernel"; return 0; }
-    const int kpad = (K + 31) / 32 * 32, npad = (N + bn - 1) / bn * bn;
+    if (bn <= 0) { g_last_error = "shape not supported by the tensor-core kernel"; return 0; }
+    const int npad = (N + bn - 1) / bn * bn;
     std::vector<float> hi((size_t)npad * kpad, 0.f), lo((size_t)npad * kpad, 0.f);
     for (int n = 0; n < N; ++n) for (int k = 0; k < K; ++k) {
       const float v = W[(size_t)n * K + k];
@@ -751,8 +775,8 @@ int bsb_pointwise(int device, int variant, int M, int K, int N, const float* A, 
     if (!dW.alloc(hi.size() * 4) || !dW2.alloc(lo.size() * 4)) { g_last_error = "cudaMalloc failed"; return 0; }
     cudaMemcpy(dW.p, hi.data(), hi.size() * 4, cudaMemcpyHostToDevice);
     cudaMemcpy(dW2.p, lo.data(), lo.size() * 4, cudaMemcpyHostToDevice);
-    if (!bsb::launch_pointwise_tc(nullptr, M, K, N, (const float*)dA.p, K, (const float*)dW.p, (const float*)dW2.p, kpad, npad, (float*)dO.p, N, e)) {
-      g_last_error = "tensor-core launch rejected the shape"; return 0;
+    if (!bsb::launch_pointwise_tc(nullptr, M, K, N, dAm, ld_a, (const float*)dW.p, (const float*)dW2.p, kpad, npad, dOm, ld_out, e)) {
+      g_last_error = "tensor-core launch rejected the shape or alignment"; return 0;
     }
   } else {
     const int n4 = (N + 3) / 4 * 4;
@@ -762,11 +786,11 @@ int bsb_pointwise(int device, int variant, int M, int K, int N, const float* A, 
     cudaMemcpy(dW.p, wt.data(), wt.size() * 4, cudaMemcpyHostToDevice);
     const int saved = bsb::pointwise_variant();
     bsb::set_pointwise_variant(variant);
-    bsb::launch_pointwise(nullptr, M, K, N, (const float*)dA.p, K, (const float*)dW.p, n4, (float*)dO.p, N, e, nullptr, 1, nullptr, 0);
+    bsb::launch_pointwise(nullptr, M, K, N, dAm, ld_a, (const float*)dW.p, n4, dOm, ld_out, e, nullptr, 1, nullptr, 0);
     bsb::set_pointwise_variant(saved);
   }
   if (!stage_end()) return 0;
-  cudaMemcpy(out, dO.p, (size_t)M * N * 4, cudaMemcpyDeviceToHost);
+  cudaMemcpy(out, dO.p, (size_t)out_len * 4, cudaMemcpyDeviceToHost);
   return 1;
 }
 
@@ -834,11 +858,20 @@ int bsb_infer(bsb_ctx* ctx, int n_frames, const float* input, float* output) {
 }
 
 long bsb_get_tensor(bsb_ctx* ctx, int tensor_index, float* out, long capacity) {
+  return bsb_get_tensor_frame(ctx, tensor_index, 0, out, capacity);
+}
+
+long bsb_get_tensor_frame(bsb_ctx* ctx, int tensor_index, int frame, float* out, long capacity) {
   if (!check_ctx(ctx)) return -1;
   std::string err;
-  long n = ctx->eng->get_tensor(tensor_index, out, capacity, &err);
+  long n = ctx->eng->get_tensor(tensor_index, frame, out, capacity, &err);
   if (n < 0) report(&ctx->cb, "error: " + err);
   return n;
+}
+
+int bsb_tc_steps(bsb_ctx* ctx, int* rows, int capacity) {
+  if (!check_ctx(ctx)) return -1;
+  return ctx->eng->tc_steps(rows, capacity);
 }
 
 long bsb_get_stage_u8(bsb_ctx* ctx, int which, int frame, uint8_t* out, long capacity) {

@@ -110,9 +110,11 @@ bool Engine::plan(std::string* err) {
   const int nt = (int)g_.tensors.size(), nops = (int)g_.ops.size();
   // Tensor cores for the 1x1 convs (3xTF32 split, ~1e-6 relative to the exact fp32 chain — the tolerance the reference's
   // own XNNPACK-vs-builtin conv tests use): on by default for the GEMM-dominated graphs (DeepLab 93 %, BodyPix 95 % of
-  // their FLOPs are 1x1 convs), on request for the others (BSB_FLAG_TENSOR_CORES), never with BSB_FLAG_EXACT or when
-  // every intermediate tensor is kept for bit-level comparison (BSB_FLAG_KEEP_TENSORS).
-  tc_enabled_ = !(flags_ & (1u | 16u)) && ((flags_ & 4u) || model_type_ == MODEL_DEEPLAB || model_type_ == MODEL_BODYPIX);
+  // their FLOPs are 1x1 convs), on request for the others (BSB_FLAG_TENSOR_CORES), never with BSB_FLAG_EXACT.  When
+  // every intermediate tensor is kept for bit-level comparison (BSB_FLAG_KEEP_TENSORS) they stay off unless
+  // BSB_FLAG_TENSOR_CORES is passed too (then each tensor-core layer can be checked in place against its own inputs).
+  tc_enabled_ = !(flags_ & 16u) && (!(flags_ & 1u) || (flags_ & 4u)) &&
+                ((flags_ & 4u) || model_type_ == MODEL_DEEPLAB || model_type_ == MODEL_BODYPIX);
   std::vector<std::vector<int>> consumers(nt);
   std::vector<int> produced_at(nt, -1);
   for (int i = 0; i < nops; ++i) {
@@ -1861,19 +1863,30 @@ double Engine::time_stage(int stage, int n, int iters, std::string* err) {
   return (double)ms / iters;
 }
 
-long Engine::get_tensor(int t, float* out, long cap, std::string* err) {
+long Engine::get_tensor(int t, int frame, float* out, long cap, std::string* err) {
   if (!(flags_ & 1u)) { *err = "bsb_get_tensor needs BSB_FLAG_KEEP_TENSORS"; return -1; }
   if (t < 0 || t >= (int)tinfo_.size()) { *err = "tensor index out of range"; return -1; }
+  if (frame < 0 || frame >= max_batch_) { *err = "frame index out of range"; return -1; }
   const TensorInfo& I = tinfo_[t];
   if (!I.materialized) return 0;
   const long n = (long)I.h * I.w * I.c;
   if (cap < n) { *err = "output buffer too small"; return -1; }
   if (cudaSetDevice(device_) != cudaSuccess || cudaStreamSynchronize(stream_) != cudaSuccess) { *err = "CUDA error in get_tensor"; return -1; }
-  if (I.ld == I.c) {
-    if (cudaMemcpy(out, tptr(t), (size_t)n * 4, cudaMemcpyDeviceToHost) != cudaSuccess) { *err = "CUDA memcpy failed"; return -1; }
-  } else {
-    for (long p = 0; p < (long)I.h * I.w; ++p)
-      if (cudaMemcpy(out + p * I.c, tptr(t) + p * I.ld, (size_t)I.c * 4, cudaMemcpyDeviceToHost) != cudaSuccess) { *err = "CUDA memcpy failed"; return -1; }
+  const float* src = tptr(t) + (size_t)frame * I.frame_elems;
+  const cudaError_t ce = cudaMemcpy2D(out, (size_t)I.c * 4, src, (size_t)I.ld * 4, (size_t)I.c * 4, (size_t)I.h * I.w, cudaMemcpyDeviceToHost);
+  if (ce != cudaSuccess) { *err = "CUDA memcpy failed"; return -1; }
+  return n;
+}
+
+int Engine::tc_steps(int* rows, int cap) const {
+  int n = 0;
+  for (const Step& st : steps_) {
+    if (st.kind != Step::PW || !st.use_tc || st.up_from >= 0) continue;
+    if (rows && n < cap) {
+      const int r[9] = {st.op_index, st.in, st.out, st.residual, st.K, st.N, st.act1, st.act2, st.act3};
+      std::memcpy(rows + 9 * n, r, sizeof r);
+    }
+    ++n;
   }
   return n;
 }

@@ -161,7 +161,10 @@ class Engine {
     if (flip_h_ || flip_v_ || resized) n += (flip_h_ || flip_v_ ? 1 : 0) + (resized ? 1 : 0) + 1;   // + stand-alone YUYV
     return n;
   }
-  long get_tensor(int t, float* out, long cap, std::string* err);
+  long get_tensor(int t, int frame, float* out, long cap, std::string* err);
+  // the steps that run the tensor-core 1x1 convolution: 9 ints each (op index, input, output and residual tensor, K, N,
+  // act1, act2, act3) into rows (up to cap steps); returns how many there are
+  int tc_steps(int* rows, int cap) const;
   long get_stage_u8(int which, int frame, uint8_t* out, long cap, std::string* err);
 
   // device staging owned by the context (host-buffer API)

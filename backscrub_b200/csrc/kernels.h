@@ -49,6 +49,8 @@ int pointwise_variant();
 int pointwise_tc_tile_n(int N);
 bool launch_pointwise_tc(cudaStream_t s, int M, int K, int N, const float* A, int ld_a, const float* w_hi, const float* w_lo,
                          int kpad, int npad, float* out, int ld_out, const Epilogue& e);
+// Why launch_pointwise_tc would refuse these operands (pitches, alignment), or nullptr if it takes them.
+const char* pointwise_tc_refusal(int K, const float* A, int ld_a, int kpad, const float* out, int ld_out, const Epilogue& e);
 
 // Depthwise KxK (depth multiplier 1).  w: [kh][kw][C].
 void launch_depthwise(cudaStream_t s, int B, const float* in, int ih, int iw, int c, int ld_in,

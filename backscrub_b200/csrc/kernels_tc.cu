@@ -7,7 +7,8 @@
 //     a*w ~= a_hi*w_hi + a_lo*w_hi + a_hi*w_lo,   x_hi = tf32(x) (truncation), x_lo = x - x_hi,
 // three MMAs per K step into the same accumulator (the dropped a_lo*w_lo term is ~2^-22 relative).
 // It is NOT bit-identical to the FFMA path / the oracle (different summation order); it is selected only
-// with BSB_FLAG_TENSOR_CORES and is validated on output tolerance + decision agreement.
+// with BSB_FLAG_TENSOR_CORES and is validated on output tolerance + decision agreement, and per call against float64
+// (tests/test_tc_float64.py: exact dyadic fixtures and a derived error bound).
 //
 // A 128-row output tile is computed by two consumer warpgroups, 64 rows each (wgmma's M is 64 per warpgroup).
 // Shared-memory operand layout (K-major, SWIZZLE_128B): one K chunk = 32 fp32 = one 128-byte row per
@@ -20,6 +21,18 @@
 namespace bsb {
 
 void count_launch();
+
+const char* pointwise_tc_refusal(int K, const float* A, int ld_a, int kpad, const float* out, int ld_out, const Epilogue& e) {
+  if (K % 4 != 0 || ld_a % 4 != 0) return "K and ld_a must be multiples of 4";
+  if (kpad % 32 != 0 || kpad < K) return "the padded weight depth kpad must be a multiple of 32 and at least K";
+  // both kernels read A in 16-byte pieces (cp.async / TMA)
+  if (reinterpret_cast<uintptr_t>(A) & 15) return "A must start on a 16-byte boundary";
+  // tc_store writes out and reads the residual as float2 whenever both pitches are even
+  const bool vec = (ld_out & 1) == 0 && (!e.residual || (e.ld_res & 1) == 0);
+  if (vec && ((reinterpret_cast<uintptr_t>(out) & 7) || (reinterpret_cast<uintptr_t>(e.residual) & 7)))
+    return "with even ld_out and ld_res, out and the residual must start on 8-byte boundaries";
+  return nullptr;
+}
 
 #ifndef BSB_EMU
 
@@ -429,7 +442,7 @@ int pointwise_tc_tile_n(int N) {       // tile width the launcher will use for t
 
 bool launch_pointwise_tc(cudaStream_t s, int M, int K, int N, const float* A, int ld_a, const float* w_hi, const float* w_lo,
                          int kpad, int npad, float* out, int ld_out, const Epilogue& e) {
-  if (K % 4 != 0 || ld_a % 4 != 0 || kpad % 32 != 0) return false;
+  if (pointwise_tc_refusal(K, A, ld_a, kpad, out, ld_out, e)) return false;
   const EpiDevTc ed{e.bias, e.residual, e.ld_res, e.act1, e.act2, e.act3};
   TcArgs a{A, w_hi, w_lo, out, M, K, N, ld_a, ld_out, kpad, ed};
   const int bn = pointwise_tc_tile_n(N);

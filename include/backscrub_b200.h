@@ -307,6 +307,16 @@ BSB_API int bsb_resize_u8c3(int device, const uint8_t* src, int sw, int sh, uint
  * act is a TFLite fused-activation code (0 none, 1 relu, 3 relu6). */
 BSB_API int bsb_pointwise(int device, int variant, int M, int K, int N, const float* A, const float* W,
                           const float* bias, int act, float* out);
+/* The same stage the way the engine calls it: operands that are sub-matrices of larger buffers and the full epilogue
+ *   out[m][n] = act3(act2(act1(sum_k A[m][k] W[n][k] + bias[n])) + residual[m][n])
+ * A[m][k] is a[a_off + m * ld_a + k] (ld_a >= K), residual[m][n] is res[res_off + m * ld_res + n] (optional) and
+ * out[m][n] is out[out_off + m * ld_out + n] (ld_out >= N).  Each buffer is copied whole to the device (a_len /
+ * res_len / out_len floats, `out` included, so whatever lies outside the written elements comes back unchanged).
+ * A must start on a 16-byte boundary (a_off % 4 == 0); the exact FFMA kernels also need out_off % 4 == 0.  The
+ * tensor-core kernel refuses a shape or alignment it cannot take; then the call returns 0 and says why. */
+BSB_API int bsb_pointwise_ex(int device, int variant, int M, int K, int N, const float* a, long a_len, long a_off, int ld_a,
+                             const float* W, const float* bias, const float* res, long res_len, long res_off, int ld_res,
+                             int act1, int act2, int act3, float* out, long out_len, long out_off, int ld_out);
 /* ms per launch of the pointwise kernel `variant` (0, 2, 3, ...: exact FFMA kernels; 1: the tensor-core kernel selected by the
  * "tc_variant" tuning switch) on an M x K x N problem (CUDA events, zero data) */
 BSB_API double bsb_time_pointwise(int device, int variant, int M, int K, int N, int iters);
@@ -322,6 +332,12 @@ BSB_API int bsb_infer(bsb_ctx* ctx, int n_frames, const float* input, float* out
 /* copy an intermediate activation (frame 0) to host; needs BSB_FLAG_KEEP_TENSORS.
  * Returns the element count, 0 if the tensor was folded away, -1 on error. */
 BSB_API long bsb_get_tensor(bsb_ctx* ctx, int tensor_index, float* out, long capacity);
+/* the same for frame `frame` of the last batch */
+BSB_API long bsb_get_tensor_frame(bsb_ctx* ctx, int tensor_index, int frame, float* out, long capacity);
+/* the 1x1 convolutions planned for the tensor cores, 9 ints per step into rows (at most `capacity` steps): TFLite op
+ * index, input, output and residual tensor (-1: none), K, N, act1, act2, act3 of the step's epilogue
+ * out = act3(act2(act1(in * W^T + bias)) + residual).  Returns the number of such steps, -1 on error. */
+BSB_API int bsb_tc_steps(bsb_ctx* ctx, int* rows, int capacity);
 /* stage buffers of the last call, frame `frame`: which = 0 model-sized RGB u8 (after resize +
  * BGR2RGB), 1 bilateral-filtered u8, 2 ofinal (IIR state after that frame) */
 BSB_API long bsb_get_stage_u8(bsb_ctx* ctx, int which, int frame, uint8_t* out, long capacity);
