@@ -112,6 +112,139 @@ static void bsb_jpeg_release(bsb_ctx* ctx) {
 static void bsb_jpeg_release(bsb_ctx*) {}
 #endif
 
+// ---- composite calls ---------------------------------------------------------------------------------------
+namespace {
+const char* const kProcessErr = "failed to process video frame: ";
+
+// n frames of `rows` rows of `row` bytes, `sstride` bytes apart with rows `spitch` apart, to frames `dstride` apart with
+// rows `dpitch` apart: one copy when both sides are tightly packed, else one per frame
+cudaError_t copy_frames(uint8_t* dst, size_t dpitch, size_t dstride, const uint8_t* src, size_t spitch, size_t sstride, size_t row,
+                        size_t rows, int n, cudaMemcpyKind kind, cudaStream_t s) {
+  const size_t fb = row * rows;
+  if (dpitch == row && spitch == row && dstride == fb && sstride == fb) return cudaMemcpyAsync(dst, src, fb * n, kind, s);
+  for (int b = 0; b < n; ++b) {
+    const cudaError_t e = cudaMemcpy2DAsync(dst + b * dstride, dpitch, src + b * sstride, spitch, row, rows, kind, s);
+    if (e != cudaSuccess) return e;
+  }
+  return cudaSuccess;
+}
+
+// frames [b0, b0 + n) of a call
+bsb::Call frames_of(bsb::Call c, int b0, int n) {
+  auto at = [b0](auto* p, size_t stride) { return p ? p + (size_t)b0 * stride : p; };
+  c.n = n; c.in = at(c.in, c.stride); c.out = at(c.out, c.out_stride); c.video = at(c.video, c.video_stride); c.mask = at(c.mask, c.mask_stride);
+  return c;
+}
+
+// the requested outputs of call `d` (on the context staging: packed, `orow`-byte BGR rows) back into the host buffers of
+// call `h` (BGR rows `out_pitch` bytes apart, the video and mask frames packed)
+cudaError_t copy_out(const bsb::Call& h, size_t out_pitch, const bsb::Call& d, size_t orow, cudaStream_t s) {
+  const cudaMemcpyKind k = cudaMemcpyDeviceToHost;
+  cudaError_t r = cudaSuccess;
+  if (h.out) r = copy_frames(h.out, out_pitch, h.out_stride, d.out, orow, d.out_stride, orow, d.out_stride / orow, h.n, k, s);
+  if (h.video && r == cudaSuccess) r = copy_frames(h.video, d.video_stride, h.video_stride, d.video, d.video_stride, d.video_stride, d.video_stride, 1, h.n, k, s);
+  if (h.mask && r == cudaSuccess) r = copy_frames(h.mask, d.mask_stride, h.mask_stride, d.mask, d.mask_stride, d.mask_stride, d.mask_stride, 1, h.n, k, s);
+  return r;
+}
+
+// Every host-buffer composite call.  `h` describes the caller's host buffers: every row is packed except BGR input rows
+// (h.pitch bytes apart) and, where given, output rows (*out_pitch bytes apart).  The frames are copied into the context
+// staging (MJPG: `jpegs` decoded there instead), the call runs on it, and each requested output is copied back before
+// the return.  `what` prefixes the engine's error.
+int host_call(bsb_ctx* ctx, const bsb::Call& h, const char* what, const size_t* out_pitch = nullptr,
+              const uint8_t* const* jpegs = nullptr, const size_t* jpeg_sizes = nullptr) {
+  if (!check_ctx(ctx)) return 0;
+  const bsb::Callbacks* cbp = &ctx->cb;
+  Engine* e = ctx->eng;
+  const bool bgr = h.fmt == bsb::IN_BGR, nv12 = h.fmt == bsb::IN_NV12;
+  const size_t W = e->W(), H = e->H(), opix = (size_t)e->out_w() * e->out_h(), orow = (size_t)e->out_w() * 3;
+  const size_t pitch = bgr ? W * 3 : nv12 ? W : W * 2, fbytes = nv12 ? W * H * 3 / 2 : pitch * H;   // of the staged frames
+  const size_t opitch = out_pitch ? *out_pitch : orow;
+  if (h.n < 1 || h.n > e->max_batch()) { report(cbp, "error: n_frames out of range (1..max_batch)"); return 0; }
+  if (jpegs ? !jpeg_sizes : (!h.in || (bgr ? h.pitch < pitch : h.stride < fbytes))) { report(cbp, "error: invalid frame"); return 0; }
+  if (nv12 && ((W | H) & 1)) { report(cbp, "error: NV12 needs an even frame width and height"); return 0; }
+  if (h.out && opitch < orow) { report(cbp, "error: invalid output pitch"); return 0; }
+  if (h.video && !nv12 && (e->out_w() & 1)) { report(cbp, "error: YUYV output needs an even width"); return 0; }
+  API_CUDA(cudaSetDevice(e->device()));
+  std::string err;
+  uint8_t* stage = bgr ? e->d_frames() : e->d_yuyv_in();
+  bsb::Call d = h;                                   // the same call on the context staging
+  d.in = stage; d.pitch = pitch; d.uv = nv12 ? W * H : 0; d.stride = fbytes;
+  d.out = h.out ? e->d_out() : nullptr; d.out_stride = opix * 3;
+  d.video = nullptr; d.video_stride = nv12 ? opix * 3 / 2 : opix * 2;
+  if (h.video && !(d.video = nv12 ? e->nv12_staging(&err) : e->d_yuyv())) { report(cbp, "error: " + err); return 0; }
+  d.mask = h.mask ? e->d_mask() : nullptr; d.mask_stride = W * H;
+  // YUYV calls of two chunks or more run chunked: the H2D copy of chunk c+1, the graph of chunk c and the D2H copy of
+  // chunk c-1 overlap on three streams (the temporal smoother's state simply carries from chunk to chunk on the compute
+  // stream).  A single-stream caller no longer pays copy + compute + copy back to back (app/deepseg.cc does exactly
+  // that: cap.read -> CalcMask -> write); results are identical, only the schedule changes.
+  const int chunk = bsb::tuning().e2e_chunk;
+  const bool piped = h.fmt == bsb::IN_YUYV && chunk > 0 && h.n >= 2 * chunk && (h.n + chunk - 1) / chunk <= bsb_ctx::kMaxChunks;
+  if (piped && !ctx->pipe_ready) {
+    API_CUDA(cudaStreamCreateWithFlags(&ctx->s_in, cudaStreamNonBlocking));
+    API_CUDA(cudaStreamCreateWithFlags(&ctx->s_out, cudaStreamNonBlocking));
+    for (int i = 0; i < bsb_ctx::kMaxChunks; ++i) {
+      API_CUDA(cudaEventCreateWithFlags(&ctx->ev_in[i], cudaEventDisableTiming));
+      API_CUDA(cudaEventCreateWithFlags(&ctx->ev_done[i], cudaEventDisableTiming));
+    }
+    ctx->pipe_ready = true;
+  }
+  cudaStream_t s = e->stream(), s_in = piped ? ctx->s_in : s, s_out = piped ? ctx->s_out : s;
+  const int step = piped ? chunk : h.n, nchunks = (h.n + step - 1) / step;
+  for (int c = 0; c < nchunks; ++c) {
+    const int b0 = c * step, nb = std::min(step, h.n - b0);
+#ifndef BSB_EMU
+    for (int b = b0; jpegs && b < b0 + nb; ++b) {
+      const std::string derr = jpeg_decode(ctx, jpegs[b], jpeg_sizes[b], stage + (size_t)b * fbytes);
+      if (!derr.empty()) { report(cbp, "error: " + derr); return 0; }
+    }
+#endif
+    if (!jpegs)
+      API_CUDA(copy_frames(stage + (size_t)b0 * fbytes, pitch, fbytes, h.in + (size_t)b0 * h.stride, bgr ? h.pitch : pitch, h.stride, pitch,
+                           fbytes / pitch, nb, cudaMemcpyHostToDevice, s_in));
+    if (piped) API_CUDA(cudaEventRecord(ctx->ev_in[c], s_in));
+  }
+  for (int c = 0; c < nchunks; ++c) {
+    const int b0 = c * step, nb = std::min(step, h.n - b0);
+    if (piped) API_CUDA(cudaStreamWaitEvent(s, ctx->ev_in[c], 0));
+    const bsb::Call dc = frames_of(d, b0, nb);
+    if (!e->run(dc, &err)) {
+      if (piped) { cudaStreamSynchronize(s_in); cudaStreamSynchronize(s); cudaStreamSynchronize(s_out); }
+      report(cbp, std::string("error: ") + what + err); return 0;
+    }
+    if (piped) { API_CUDA(cudaEventRecord(ctx->ev_done[c], s)); API_CUDA(cudaStreamWaitEvent(s_out, ctx->ev_done[c], 0)); }
+    API_CUDA(copy_out(frames_of(h, b0, nb), opitch, dc, orow, s_out));
+  }
+  if (piped) API_CUDA(cudaStreamSynchronize(s_out));
+  API_CUDA(cudaStreamSynchronize(s));
+  API_CUDA(cudaGetLastError());
+  return 1;
+}
+
+// Every device-pointer composite call.  The C ABI's device BGR frames have packed rows, its YUYV frames are packed.
+int device_call(bsb_ctx* ctx, bsb::Call c, int sync) {
+  if (!check_ctx(ctx)) return 0;
+  const bsb::Callbacks* cbp = &ctx->cb;
+  Engine* e = ctx->eng;
+  if (c.fmt == bsb::IN_BGR) c.pitch = (size_t)e->W() * 3;
+  if (c.fmt == bsb::IN_YUYV) { c.pitch = (size_t)e->W() * 2; c.stride = c.pitch * e->H(); }
+  // the engine checks an NV12 call's frames and output with their layout
+  if (c.fmt != bsb::IN_NV12 && !c.in) { report(cbp, "error: invalid frame"); return 0; }
+  if (c.fmt != bsb::IN_NV12 && c.video && (e->out_w() & 1)) { report(cbp, "error: YUYV output needs an even width"); return 0; }
+  std::string err;
+  if (!e->run(c, &err)) { report(cbp, "error: " + err); return 0; }
+  if (sync) { API_CUDA(cudaStreamSynchronize(e->stream())); API_CUDA(cudaGetLastError()); }
+  return 1;
+}
+
+// sources entry points refuse a null id table first (a Call without ids is a plain call)
+bool null_ids(bsb_ctx* ctx, const int* ids) {
+  if (ids || !check_ctx(ctx)) return false;
+  report(&ctx->cb, "error: null source id table");
+  return true;
+}
+}  // namespace
+
 extern "C" {
 
 const char* bsb_version(void) { return "backscrub-b200 0.1 (sm_90a CUDA; TFLite schema v3 graph runtime)"; }
@@ -158,18 +291,11 @@ void bsb_maskgen_delete(bsb_ctx* ctx) {
 
 int bsb_maskgen_process(bsb_ctx* ctx, const uint8_t* frame, size_t frame_pitch, const uint8_t** mask, size_t* mask_pitch) {
   if (!check_ctx(ctx)) return 0;
-  const bsb::Callbacks* cbp = &ctx->cb;
   Engine* e = ctx->eng;
-  if (!frame || frame_pitch < (size_t)e->W() * 3) { report(cbp, "error: invalid frame"); return 0; }
-  API_CUDA(cudaSetDevice(e->device()));
-  const size_t row = (size_t)e->W() * 3;
-  API_CUDA(cudaMemcpy2DAsync(e->d_frames(), row, frame, frame_pitch, row, (size_t)e->H(), cudaMemcpyHostToDevice, e->stream()));
-  std::string err;
-  if (!e->run(1, e->d_frames(), row, row * e->H(), nullptr, 0, nullptr, 0, e->d_mask(), (size_t)e->W() * e->H(), true, &err)) {
-    report(cbp, "error: failed to interpret video frame: " + err); return 0;
-  }
-  API_CUDA(cudaMemcpyAsync(e->h_mask(), e->d_mask(), (size_t)e->W() * e->H(), cudaMemcpyDeviceToHost, e->stream()));
-  API_CUDA(cudaStreamSynchronize(e->stream()));
+  const size_t npix = (size_t)e->W() * e->H();
+  if (!host_call(ctx, {1, bsb::IN_BGR, frame, frame_pitch, 0, npix * 3, nullptr, nullptr, 0, nullptr, 0, e->h_mask(), npix, true},
+                 "failed to interpret video frame: "))
+    return 0;
   if (mask) *mask = e->h_mask();
   if (mask_pitch) *mask_pitch = (size_t)e->W();
   return 1;
@@ -232,137 +358,20 @@ int bsb_get_background(bsb_ctx* ctx, uint8_t* out, size_t out_pitch) {
 int bsb_composite(bsb_ctx* ctx, int n_frames, const uint8_t* frames, size_t frame_pitch, size_t frame_stride,
                   uint8_t* out, size_t out_pitch, size_t out_stride, uint8_t* out_yuyv, size_t yuyv_stride,
                   uint8_t* out_mask, size_t mask_stride) {
-  if (!check_ctx(ctx)) return 0;
-  const bsb::Callbacks* cbp = &ctx->cb;
-  Engine* e = ctx->eng;
-  const size_t row = (size_t)e->W() * 3, fbytes = row * e->H(), npix = (size_t)e->W() * e->H();
-  const size_t orow = (size_t)e->out_w() * 3, obytes = orow * e->out_h(), opix = (size_t)e->out_w() * e->out_h();
-  if (n_frames < 1 || n_frames > e->max_batch()) { report(cbp, "error: n_frames out of range (1..max_batch)"); return 0; }
-  if (!frames || frame_pitch < row) { report(cbp, "error: invalid frame"); return 0; }
-  if (out && out_pitch < orow) { report(cbp, "error: invalid output pitch"); return 0; }
-  if (out_yuyv && (e->out_w() & 1)) { report(cbp, "error: YUYV output needs an even width"); return 0; }
-  API_CUDA(cudaSetDevice(e->device()));
-  if (frame_pitch == row && frame_stride == fbytes) {
-    API_CUDA(cudaMemcpyAsync(e->d_frames(), frames, fbytes * n_frames, cudaMemcpyHostToDevice, e->stream()));
-  } else {
-    for (int b = 0; b < n_frames; ++b)
-      API_CUDA(cudaMemcpy2DAsync(e->d_frames() + b * fbytes, row, frames + (size_t)b * frame_stride, frame_pitch, row, (size_t)e->H(),
-                                 cudaMemcpyHostToDevice, e->stream()));
-  }
-  std::string err;
-  if (!e->run(n_frames, e->d_frames(), row, fbytes, out ? e->d_out() : nullptr, obytes, out_yuyv ? e->d_yuyv() : nullptr, opix * 2,
-              out_mask ? e->d_mask() : nullptr, npix, false, &err)) {
-    report(cbp, "error: failed to process video frame: " + err); return 0;
-  }
-  if (out) {
-    if (out_pitch == orow && out_stride == obytes) API_CUDA(cudaMemcpyAsync(out, e->d_out(), obytes * n_frames, cudaMemcpyDeviceToHost, e->stream()));
-    else for (int b = 0; b < n_frames; ++b)
-      API_CUDA(cudaMemcpy2DAsync(out + (size_t)b * out_stride, out_pitch, e->d_out() + b * obytes, orow, orow, (size_t)e->out_h(), cudaMemcpyDeviceToHost, e->stream()));
-  }
-  if (out_yuyv) for (int b = 0; b < n_frames; ++b)
-    API_CUDA(cudaMemcpyAsync(out_yuyv + (size_t)b * yuyv_stride, e->d_yuyv() + b * opix * 2, opix * 2, cudaMemcpyDeviceToHost, e->stream()));
-  if (out_mask) for (int b = 0; b < n_frames; ++b)
-    API_CUDA(cudaMemcpyAsync(out_mask + (size_t)b * mask_stride, e->d_mask() + b * npix, npix, cudaMemcpyDeviceToHost, e->stream()));
-  API_CUDA(cudaStreamSynchronize(e->stream()));
-  API_CUDA(cudaGetLastError());
-  return 1;
+  return host_call(ctx, {n_frames, bsb::IN_BGR, frames, frame_pitch, 0, frame_stride, nullptr, out, out_stride, out_yuyv, yuyv_stride, out_mask,
+                         mask_stride}, kProcessErr, &out_pitch);
 }
 
 int bsb_composite_device(bsb_ctx* ctx, int n_frames, const uint8_t* d_frames, size_t frame_stride, uint8_t* d_out, size_t out_stride,
                          uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, int sync) {
-  if (!check_ctx(ctx)) return 0;
-  const bsb::Callbacks* cbp = &ctx->cb;
-  Engine* e = ctx->eng;
-  if (!d_frames) { report(cbp, "error: invalid frame"); return 0; }
-  if (d_yuyv && (e->out_w() & 1)) { report(cbp, "error: YUYV output needs an even width"); return 0; }
-  std::string err;
-  if (!e->run(n_frames, d_frames, (size_t)e->W() * 3, frame_stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, false, &err)) {
-    report(cbp, "error: " + err); return 0;
-  }
-  if (sync) { API_CUDA(cudaStreamSynchronize(e->stream())); API_CUDA(cudaGetLastError()); }
-  return 1;
+  return device_call(ctx, {n_frames, bsb::IN_BGR, d_frames, 0, 0, frame_stride, nullptr, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride},
+                     sync);
 }
 
 int bsb_composite_yuyv(bsb_ctx* ctx, int n_frames, const uint8_t* yuyv_frames, size_t in_stride, uint8_t* out, size_t out_stride,
                        uint8_t* out_yuyv, size_t yuyv_stride, uint8_t* out_mask, size_t mask_stride) {
-  if (!check_ctx(ctx)) return 0;
-  const bsb::Callbacks* cbp = &ctx->cb;
-  Engine* e = ctx->eng;
-  const size_t npix = (size_t)e->W() * e->H();
-  const size_t opix = (size_t)e->out_w() * e->out_h(), obytes = opix * 3;
-  if (n_frames < 1 || n_frames > e->max_batch()) { report(cbp, "error: n_frames out of range (1..max_batch)"); return 0; }
-  if (!yuyv_frames || in_stride < npix * 2) { report(cbp, "error: invalid frame"); return 0; }
-  if (out_yuyv && (e->out_w() & 1)) { report(cbp, "error: YUYV output needs an even width"); return 0; }
-  API_CUDA(cudaSetDevice(e->device()));
-  // ---- chunked, overlapped form: H2D of chunk c+1, the graph of chunk c and D2H of chunk c-1 run at the same time on
-  //      three streams (the temporal smoother's state simply carries from chunk to chunk on the compute stream).  A
-  //      single-stream caller no longer pays copy + compute + copy back to back (app/deepseg.cc does exactly that:
-  //      cap.read -> CalcMask -> write); results are identical, only the schedule changes ----
-  const int chunk = bsb::tuning().e2e_chunk;
-  if (chunk > 0 && n_frames >= 2 * chunk && (n_frames + chunk - 1) / chunk <= bsb_ctx::kMaxChunks) {
-    if (!ctx->pipe_ready) {
-      API_CUDA(cudaStreamCreateWithFlags(&ctx->s_in, cudaStreamNonBlocking));
-      API_CUDA(cudaStreamCreateWithFlags(&ctx->s_out, cudaStreamNonBlocking));
-      for (int i = 0; i < bsb_ctx::kMaxChunks; ++i) {
-        API_CUDA(cudaEventCreateWithFlags(&ctx->ev_in[i], cudaEventDisableTiming));
-        API_CUDA(cudaEventCreateWithFlags(&ctx->ev_done[i], cudaEventDisableTiming));
-      }
-      ctx->pipe_ready = true;
-    }
-    const int nchunks = (n_frames + chunk - 1) / chunk;
-    for (int c = 0; c < nchunks; ++c) {
-      const int b0 = c * chunk, nb = std::min(chunk, n_frames - b0);
-      if (in_stride == npix * 2) API_CUDA(cudaMemcpyAsync(e->d_yuyv_in() + (size_t)b0 * npix * 2, yuyv_frames + (size_t)b0 * in_stride, npix * 2 * nb, cudaMemcpyHostToDevice, ctx->s_in));
-      else for (int b = b0; b < b0 + nb; ++b)
-        API_CUDA(cudaMemcpyAsync(e->d_yuyv_in() + (size_t)b * npix * 2, yuyv_frames + (size_t)b * in_stride, npix * 2, cudaMemcpyHostToDevice, ctx->s_in));
-      API_CUDA(cudaEventRecord(ctx->ev_in[c], ctx->s_in));
-    }
-    std::string perr;
-    for (int c = 0; c < nchunks; ++c) {
-      const int b0 = c * chunk, nb = std::min(chunk, n_frames - b0);
-      API_CUDA(cudaStreamWaitEvent(e->stream(), ctx->ev_in[c], 0));
-      if (!e->run_yuyv(nb, e->d_yuyv_in() + (size_t)b0 * npix * 2, out ? e->d_out() + (size_t)b0 * obytes : nullptr, obytes, out_yuyv ? e->d_yuyv() + (size_t)b0 * opix * 2 : nullptr, opix * 2,
-                       out_mask ? e->d_mask() + (size_t)b0 * npix : nullptr, npix, &perr)) {
-        cudaStreamSynchronize(ctx->s_in); cudaStreamSynchronize(e->stream()); cudaStreamSynchronize(ctx->s_out);
-        report(cbp, "error: failed to process video frame: " + perr); return 0;
-      }
-      API_CUDA(cudaEventRecord(ctx->ev_done[c], e->stream()));
-      API_CUDA(cudaStreamWaitEvent(ctx->s_out, ctx->ev_done[c], 0));
-      if (out) for (int b = b0; b < b0 + nb; ++b)
-        API_CUDA(cudaMemcpyAsync(out + (size_t)b * out_stride, e->d_out() + (size_t)b * obytes, obytes, cudaMemcpyDeviceToHost, ctx->s_out));
-      if (out_yuyv) {
-        if (yuyv_stride == opix * 2) API_CUDA(cudaMemcpyAsync(out_yuyv + (size_t)b0 * yuyv_stride, e->d_yuyv() + (size_t)b0 * opix * 2, opix * 2 * nb, cudaMemcpyDeviceToHost, ctx->s_out));
-        else for (int b = b0; b < b0 + nb; ++b)
-          API_CUDA(cudaMemcpyAsync(out_yuyv + (size_t)b * yuyv_stride, e->d_yuyv() + (size_t)b * opix * 2, opix * 2, cudaMemcpyDeviceToHost, ctx->s_out));
-      }
-      if (out_mask) for (int b = b0; b < b0 + nb; ++b)
-        API_CUDA(cudaMemcpyAsync(out_mask + (size_t)b * mask_stride, e->d_mask() + (size_t)b * npix, npix, cudaMemcpyDeviceToHost, ctx->s_out));
-    }
-    API_CUDA(cudaStreamSynchronize(ctx->s_out));
-    API_CUDA(cudaStreamSynchronize(e->stream()));
-    API_CUDA(cudaGetLastError());
-    return 1;
-  }
-  if (in_stride == npix * 2) API_CUDA(cudaMemcpyAsync(e->d_yuyv_in(), yuyv_frames, npix * 2 * n_frames, cudaMemcpyHostToDevice, e->stream()));
-  else for (int b = 0; b < n_frames; ++b)
-    API_CUDA(cudaMemcpyAsync(e->d_yuyv_in() + b * npix * 2, yuyv_frames + (size_t)b * in_stride, npix * 2, cudaMemcpyHostToDevice, e->stream()));
-  std::string err;
-  if (!e->run_yuyv(n_frames, e->d_yuyv_in(), out ? e->d_out() : nullptr, obytes, out_yuyv ? e->d_yuyv() : nullptr, opix * 2,
-                   out_mask ? e->d_mask() : nullptr, npix, &err)) {
-    report(cbp, "error: failed to process video frame: " + err); return 0;
-  }
-  if (out) for (int b = 0; b < n_frames; ++b)
-    API_CUDA(cudaMemcpyAsync(out + (size_t)b * out_stride, e->d_out() + b * obytes, obytes, cudaMemcpyDeviceToHost, e->stream()));
-  if (out_yuyv) {
-    if (yuyv_stride == opix * 2) API_CUDA(cudaMemcpyAsync(out_yuyv, e->d_yuyv(), opix * 2 * n_frames, cudaMemcpyDeviceToHost, e->stream()));
-    else for (int b = 0; b < n_frames; ++b)
-      API_CUDA(cudaMemcpyAsync(out_yuyv + (size_t)b * yuyv_stride, e->d_yuyv() + b * opix * 2, opix * 2, cudaMemcpyDeviceToHost, e->stream()));
-  }
-  if (out_mask) for (int b = 0; b < n_frames; ++b)
-    API_CUDA(cudaMemcpyAsync(out_mask + (size_t)b * mask_stride, e->d_mask() + b * npix, npix, cudaMemcpyDeviceToHost, e->stream()));
-  API_CUDA(cudaStreamSynchronize(e->stream()));
-  API_CUDA(cudaGetLastError());
-  return 1;
+  return host_call(ctx, {n_frames, bsb::IN_YUYV, yuyv_frames, 0, 0, in_stride, nullptr, out, out_stride, out_yuyv, yuyv_stride, out_mask, mask_stride},
+                   kProcessErr);
 }
 
 int bsb_decode_mjpg(bsb_ctx* ctx, const uint8_t* jpeg, size_t jpeg_size, uint8_t* bgr_out) {
@@ -385,99 +394,34 @@ int bsb_decode_mjpg(bsb_ctx* ctx, const uint8_t* jpeg, size_t jpeg_size, uint8_t
 
 int bsb_composite_mjpg(bsb_ctx* ctx, int n_frames, const uint8_t* const* jpegs, const size_t* jpeg_sizes, uint8_t* out, size_t out_stride,
                        uint8_t* out_yuyv, size_t yuyv_stride, uint8_t* out_mask, size_t mask_stride) {
-  if (!check_ctx(ctx)) return 0;
-  const bsb::Callbacks* cbp = &ctx->cb;
 #ifdef BSB_EMU
+  if (!check_ctx(ctx)) return 0;
   (void)n_frames; (void)jpegs; (void)jpeg_sizes; (void)out; (void)out_stride; (void)out_yuyv; (void)yuyv_stride; (void)out_mask; (void)mask_stride;
-  report(cbp, "error: MJPG ingest needs a GPU (NVJPG)"); return 0;
+  report(&ctx->cb, "error: MJPG ingest needs a GPU (NVJPG)"); return 0;
 #else
-  Engine* e = ctx->eng;
-  const size_t row = (size_t)e->W() * 3, fbytes = row * e->H(), npix = (size_t)e->W() * e->H();
-  const size_t opix = (size_t)e->out_w() * e->out_h(), obytes = opix * 3;
-  if (n_frames < 1 || n_frames > e->max_batch()) { report(cbp, "error: n_frames out of range (1..max_batch)"); return 0; }
-  if (!jpegs || !jpeg_sizes) { report(cbp, "error: invalid frame"); return 0; }
-  if (out_yuyv && (e->out_w() & 1)) { report(cbp, "error: YUYV output needs an even width"); return 0; }
-  API_CUDA(cudaSetDevice(e->device()));
-  for (int b = 0; b < n_frames; ++b) {
-    const std::string derr = jpeg_decode(ctx, jpegs[b], jpeg_sizes[b], e->d_frames() + (size_t)b * fbytes);
-    if (!derr.empty()) { report(cbp, "error: " + derr); return 0; }
-  }
-  std::string err;
-  if (!e->run(n_frames, e->d_frames(), row, fbytes, out ? e->d_out() : nullptr, obytes, out_yuyv ? e->d_yuyv() : nullptr, opix * 2,
-              out_mask ? e->d_mask() : nullptr, npix, false, &err)) {
-    report(cbp, "error: failed to process video frame: " + err); return 0;
-  }
-  if (out) for (int b = 0; b < n_frames; ++b)
-    API_CUDA(cudaMemcpyAsync(out + (size_t)b * out_stride, e->d_out() + b * obytes, obytes, cudaMemcpyDeviceToHost, e->stream()));
-  if (out_yuyv) for (int b = 0; b < n_frames; ++b)
-    API_CUDA(cudaMemcpyAsync(out_yuyv + (size_t)b * yuyv_stride, e->d_yuyv() + b * opix * 2, opix * 2, cudaMemcpyDeviceToHost, e->stream()));
-  if (out_mask) for (int b = 0; b < n_frames; ++b)
-    API_CUDA(cudaMemcpyAsync(out_mask + (size_t)b * mask_stride, e->d_mask() + b * npix, npix, cudaMemcpyDeviceToHost, e->stream()));
-  API_CUDA(cudaStreamSynchronize(e->stream()));
-  API_CUDA(cudaGetLastError());
-  return 1;
+  return host_call(ctx, {n_frames, bsb::IN_BGR, nullptr, 0, 0, 0, nullptr, out, out_stride, out_yuyv, yuyv_stride, out_mask, mask_stride},
+                   kProcessErr, nullptr, jpegs, jpeg_sizes);
 #endif
 }
 
 int bsb_composite_yuyv_device(bsb_ctx* ctx, int n_frames, const uint8_t* d_yuyv_frames, uint8_t* d_out, size_t out_stride,
                               uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, int sync) {
-  if (!check_ctx(ctx)) return 0;
-  const bsb::Callbacks* cbp = &ctx->cb;
-  Engine* e = ctx->eng;
-  if (!d_yuyv_frames) { report(cbp, "error: invalid frame"); return 0; }
-  if (d_yuyv && (e->out_w() & 1)) { report(cbp, "error: YUYV output needs an even width"); return 0; }
-  std::string err;
-  if (!e->run_yuyv(n_frames, d_yuyv_frames, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, &err)) { report(cbp, "error: " + err); return 0; }
-  if (sync) { API_CUDA(cudaStreamSynchronize(e->stream())); API_CUDA(cudaGetLastError()); }
-  return 1;
+  return device_call(ctx, {n_frames, bsb::IN_YUYV, d_yuyv_frames, 0, 0, 0, nullptr, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride},
+                     sync);
 }
 
 // ---- NV12 camera frames in, NV12 composites out ------------------------------------
 int bsb_composite_nv12(bsb_ctx* ctx, int n_frames, const uint8_t* nv12, size_t in_stride, uint8_t* out, size_t out_stride,
                        uint8_t* nv12_out, size_t nv12_stride, uint8_t* out_mask, size_t mask_stride) {
-  if (!check_ctx(ctx)) return 0;
-  const bsb::Callbacks* cbp = &ctx->cb;
-  Engine* e = ctx->eng;
-  const size_t npix = (size_t)e->W() * e->H(), fnv = npix * 3 / 2;
-  const size_t opix = (size_t)e->out_w() * e->out_h(), obytes = opix * 3, onv = opix * 3 / 2;
-  if (n_frames < 1 || n_frames > e->max_batch()) { report(cbp, "error: n_frames out of range (1..max_batch)"); return 0; }
-  if (!nv12 || in_stride < fnv) { report(cbp, "error: invalid frame"); return 0; }
-  if ((e->W() & 1) || (e->H() & 1)) { report(cbp, "error: NV12 needs an even frame width and height"); return 0; }
-  API_CUDA(cudaSetDevice(e->device()));
-  std::string err;
-  uint8_t* d_nv = nullptr;
-  if (nv12_out && !(d_nv = e->nv12_staging(&err))) { report(cbp, "error: " + err); return 0; }
-  // the frames go to the context's camera staging (max_batch * W*H*2 bytes), tightly packed
-  if (in_stride == fnv) API_CUDA(cudaMemcpyAsync(e->d_yuyv_in(), nv12, fnv * n_frames, cudaMemcpyHostToDevice, e->stream()));
-  else for (int b = 0; b < n_frames; ++b)
-    API_CUDA(cudaMemcpyAsync(e->d_yuyv_in() + b * fnv, nv12 + (size_t)b * in_stride, fnv, cudaMemcpyHostToDevice, e->stream()));
-  if (!e->run_nv12(n_frames, nullptr, e->d_yuyv_in(), (size_t)e->W(), npix, fnv, out ? e->d_out() : nullptr, obytes, d_nv, onv,
-                   out_mask ? e->d_mask() : nullptr, npix, &err)) {
-    report(cbp, "error: failed to process video frame: " + err); return 0;
-  }
-  if (out) for (int b = 0; b < n_frames; ++b)
-    API_CUDA(cudaMemcpyAsync(out + (size_t)b * out_stride, e->d_out() + b * obytes, obytes, cudaMemcpyDeviceToHost, e->stream()));
-  if (nv12_out) for (int b = 0; b < n_frames; ++b)
-    API_CUDA(cudaMemcpyAsync(nv12_out + (size_t)b * nv12_stride, d_nv + b * onv, onv, cudaMemcpyDeviceToHost, e->stream()));
-  if (out_mask) for (int b = 0; b < n_frames; ++b)
-    API_CUDA(cudaMemcpyAsync(out_mask + (size_t)b * mask_stride, e->d_mask() + b * npix, npix, cudaMemcpyDeviceToHost, e->stream()));
-  API_CUDA(cudaStreamSynchronize(e->stream()));
-  API_CUDA(cudaGetLastError());
-  return 1;
+  return host_call(ctx, {n_frames, bsb::IN_NV12, nv12, 0, 0, in_stride, nullptr, out, out_stride, nv12_out, nv12_stride, out_mask, mask_stride},
+                   kProcessErr);
 }
 
 int bsb_composite_nv12_device(bsb_ctx* ctx, int n_frames, const uint8_t* d_nv12, size_t in_pitch, size_t uv_offset, size_t in_stride,
                               uint8_t* d_out, size_t out_stride, uint8_t* d_nv12_out, size_t nv12_stride, uint8_t* d_mask, size_t mask_stride,
                               int sync) {
-  if (!check_ctx(ctx)) return 0;
-  const bsb::Callbacks* cbp = &ctx->cb;
-  Engine* e = ctx->eng;
-  std::string err;
-  if (!e->run_nv12(n_frames, nullptr, d_nv12, in_pitch, uv_offset, in_stride, d_out, out_stride, d_nv12_out, nv12_stride, d_mask, mask_stride, &err)) {
-    report(cbp, "error: " + err); return 0;
-  }
-  if (sync) { API_CUDA(cudaStreamSynchronize(e->stream())); API_CUDA(cudaGetLastError()); }
-  return 1;
+  return device_call(ctx, {n_frames, bsb::IN_NV12, d_nv12, in_pitch, uv_offset, in_stride, nullptr, d_out, out_stride, d_nv12_out, nv12_stride,
+                           d_mask, mask_stride}, sync);
 }
 
 // ---- independent sources ---------------------------------------------------------
@@ -518,67 +462,23 @@ int bsb_set_source_flip(bsb_ctx* ctx, int source, int flip) {
 
 int bsb_composite_sources(bsb_ctx* ctx, int n, const int* source_ids, const uint8_t* frames, size_t frame_pitch, size_t frame_stride,
                           uint8_t* out, size_t out_stride, uint8_t* out_yuyv, size_t yuyv_stride, uint8_t* out_mask, size_t mask_stride) {
-  if (!check_ctx(ctx)) return 0;
-  const bsb::Callbacks* cbp = &ctx->cb;
-  Engine* e = ctx->eng;
-  const size_t row = (size_t)e->W() * 3, fbytes = row * e->H(), npix = (size_t)e->W() * e->H();
-  const size_t orow = (size_t)e->out_w() * 3, obytes = orow * e->out_h(), opix = (size_t)e->out_w() * e->out_h();
-  if (n < 1 || n > e->max_batch()) { report(cbp, "error: n_frames out of range (1..max_batch)"); return 0; }
-  if (!frames || frame_pitch < row) { report(cbp, "error: invalid frame"); return 0; }
-  if (out_yuyv && (e->out_w() & 1)) { report(cbp, "error: YUYV output needs an even width"); return 0; }
-  API_CUDA(cudaSetDevice(e->device()));
-  if (frame_pitch == row && frame_stride == fbytes) {
-    API_CUDA(cudaMemcpyAsync(e->d_frames(), frames, fbytes * n, cudaMemcpyHostToDevice, e->stream()));
-  } else {
-    for (int b = 0; b < n; ++b)
-      API_CUDA(cudaMemcpy2DAsync(e->d_frames() + b * fbytes, row, frames + (size_t)b * frame_stride, frame_pitch, row, (size_t)e->H(),
-                                 cudaMemcpyHostToDevice, e->stream()));
-  }
-  std::string err;
-  if (!e->run_sources(n, source_ids, e->d_frames(), row, fbytes, out ? e->d_out() : nullptr, obytes, out_yuyv ? e->d_yuyv() : nullptr, opix * 2,
-                      out_mask ? e->d_mask() : nullptr, npix, &err)) {
-    report(cbp, "error: " + err); return 0;
-  }
-  if (out) for (int b = 0; b < n; ++b)
-    API_CUDA(cudaMemcpyAsync(out + (size_t)b * out_stride, e->d_out() + b * obytes, obytes, cudaMemcpyDeviceToHost, e->stream()));
-  if (out_yuyv) for (int b = 0; b < n; ++b)
-    API_CUDA(cudaMemcpyAsync(out_yuyv + (size_t)b * yuyv_stride, e->d_yuyv() + b * opix * 2, opix * 2, cudaMemcpyDeviceToHost, e->stream()));
-  if (out_mask) for (int b = 0; b < n; ++b)
-    API_CUDA(cudaMemcpyAsync(out_mask + (size_t)b * mask_stride, e->d_mask() + b * npix, npix, cudaMemcpyDeviceToHost, e->stream()));
-  API_CUDA(cudaStreamSynchronize(e->stream()));
-  API_CUDA(cudaGetLastError());
-  return 1;
+  if (null_ids(ctx, source_ids)) return 0;
+  return host_call(ctx, {n, bsb::IN_BGR, frames, frame_pitch, 0, frame_stride, source_ids, out, out_stride, out_yuyv, yuyv_stride, out_mask, mask_stride},
+                   "");
 }
 
 int bsb_composite_sources_yuyv_device(bsb_ctx* ctx, int n, const int* source_ids, const uint8_t* d_yuyv_frames, uint8_t* d_out, size_t out_stride,
                                       uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, int sync) {
-  if (!check_ctx(ctx)) return 0;
-  const bsb::Callbacks* cbp = &ctx->cb;
-  Engine* e = ctx->eng;
-  if (!d_yuyv_frames) { report(cbp, "error: invalid frame"); return 0; }
-  if (d_yuyv && (e->out_w() & 1)) { report(cbp, "error: YUYV output needs an even width"); return 0; }
-  std::string err;
-  if (!e->run_sources_yuyv(n, source_ids, d_yuyv_frames, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, &err)) {
-    report(cbp, "error: " + err); return 0;
-  }
-  if (sync) { API_CUDA(cudaStreamSynchronize(e->stream())); API_CUDA(cudaGetLastError()); }
-  return 1;
+  if (null_ids(ctx, source_ids)) return 0;
+  return device_call(ctx, {n, bsb::IN_YUYV, d_yuyv_frames, 0, 0, 0, source_ids, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride}, sync);
 }
 
 int bsb_composite_sources_nv12_device(bsb_ctx* ctx, int n_frames, const int* source_ids, const uint8_t* d_nv12, size_t in_pitch,
                                       size_t uv_offset, size_t in_stride, uint8_t* d_out, size_t out_stride, uint8_t* d_nv12_out,
                                       size_t nv12_stride, uint8_t* d_mask, size_t mask_stride, int sync) {
-  if (!check_ctx(ctx)) return 0;
-  const bsb::Callbacks* cbp = &ctx->cb;
-  Engine* e = ctx->eng;
-  if (!source_ids) { report(cbp, "error: null source id table"); return 0; }
-  std::string err;
-  if (!e->run_nv12(n_frames, source_ids, d_nv12, in_pitch, uv_offset, in_stride, d_out, out_stride, d_nv12_out, nv12_stride, d_mask, mask_stride,
-                   &err)) {
-    report(cbp, "error: " + err); return 0;
-  }
-  if (sync) { API_CUDA(cudaStreamSynchronize(e->stream())); API_CUDA(cudaGetLastError()); }
-  return 1;
+  if (null_ids(ctx, source_ids)) return 0;
+  return device_call(ctx, {n_frames, bsb::IN_NV12, d_nv12, in_pitch, uv_offset, in_stride, source_ids, d_out, out_stride, d_nv12_out, nv12_stride,
+                           d_mask, mask_stride}, sync);
 }
 
 int bsb_synchronize(bsb_ctx* ctx) {

@@ -948,20 +948,13 @@ Engine::~Engine() {
 // ---------------------------------------------------------------------------
 // enqueue: the per-call kernel sequence (captured into a CUDA graph by run())
 // ---------------------------------------------------------------------------
-void Engine::enqueue_pre(int n, const uint8_t* d_frames, size_t pitch, size_t stride, const uint8_t* d_yuyv_in) {
+void Engine::enqueue_pre(const Call& c) {
   // camera YUYV / NV12 frames are read in place (each bilinear tap converted like cv::COLOR_YUV2BGR_YUYV / _NV12 would have)
-  if (d_yuyv_in && nv12_.on)
-    launch_resize_roi_swap(stream_, n, d_yuyv_in, nv12_.stride, nv12_.pitch, roidim_[0], roidim_[1], roidim_[2], roidim_[3], tab_in_.tab,
-                           in_u8_, mw_, mh_, in_roidim_[0], in_roidim_[1], in_roidim_[2], in_roidim_[3], tab_in_.area2x2, IN_NV12, nv12_.uv);
-  else if (d_yuyv_in)
-    launch_resize_roi_swap(stream_, n, d_yuyv_in, (size_t)W_ * H_ * 2, (size_t)W_ * 2, roidim_[0], roidim_[1], roidim_[2], roidim_[3], tab_in_.tab,
-                           in_u8_, mw_, mh_, in_roidim_[0], in_roidim_[1], in_roidim_[2], in_roidim_[3], tab_in_.area2x2, IN_YUYV);
-  else
-    launch_resize_roi_swap(stream_, n, d_frames, stride, pitch, roidim_[0], roidim_[1], roidim_[2], roidim_[3], tab_in_.tab,
-                           in_u8_, mw_, mh_, in_roidim_[0], in_roidim_[1], in_roidim_[2], in_roidim_[3], tab_in_.area2x2);
+  launch_resize_roi_swap(stream_, c.n, c.in, c.stride, c.pitch, roidim_[0], roidim_[1], roidim_[2], roidim_[3], tab_in_.tab,
+                         in_u8_, mw_, mh_, in_roidim_[0], in_roidim_[1], in_roidim_[2], in_roidim_[3], tab_in_.area2x2, c.fmt, c.uv);
   // with the fused stem the fp32 input tensor is only materialised for introspection (KEEP_TENSORS)
   float* f32 = (stem_u8_ok_ && !(flags_ & 1u)) ? nullptr : tptr(g_.input);
-  launch_bilateral_norm(stream_, n, in_u8_, mw_, mh_, lut_, lut_ + 768, scaling_, offset_, f32, filt_u8_);
+  launch_bilateral_norm(stream_, c.n, in_u8_, mw_, mh_, lut_, lut_ + 768, scaling_, offset_, f32, filt_u8_);
 }
 
 // Frames per pass of a sub-batched segment: the segment's largest tensor, in and out, should stay L2-resident
@@ -1159,8 +1152,8 @@ void Engine::run_step(size_t si, int n, bool from_u8, bool* first_p, bool* skip_
   }
 }
 
-void Engine::enqueue_decision(int n) {
-  const bool sources = call_mode_ != CALL_PLAIN;      // per-source states, looked up through the id table
+// sources: per-source states, looked up through the id table
+void Engine::enqueue_decision(int n, bool sources) {
   if (dec_up_step_ >= 0) {
     const Step& st = steps_[dec_up_step_];
     const TensorInfo& I = tinfo_[st.in];
@@ -1175,21 +1168,21 @@ void Engine::enqueue_decision(int n) {
   else launch_decision_iir(stream_, model_type_, n, tptr(g_.output), oh_, ow_, oc_, state_, ofinal_, opitch_);
 }
 
-// PostArgs of one call.  d_yuyv_in (non-null): the post kernel reads the camera frames in place — YUYV, or NV12 in an NV12
-// call, which then also writes its video output (d_yuyv) as NV12.
-PostArgs Engine::post_args(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
-                           uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in) const {
+// PostArgs of one call.  p.native: the post kernel reads the camera frames in place — YUYV, or NV12, which then also
+// writes its video output as NV12; p.nv12_staged: the video output goes to d_yuyv_ as YUYV.
+PostArgs Engine::post_args(const Call& c, const Plan& p) const {
   const size_t fbytes = (size_t)W_ * H_ * 3;
-  const bool tail = call_tail();
-  const bool want_rgb = d_out || d_yuyv;
-  const bool nv12_in = nv12_.on && d_yuyv_in;
+  const bool tail = call_tail(p);
+  const bool want_rgb = c.out || c.video;
+  const bool nv12_in = p.native && c.fmt == IN_NV12;
   PostArgs a{};
-  a.B = n; a.W = W_; a.H = H_;
-  a.frames = d_frames; a.frame_pitch = pitch; a.frame_stride = stride;
+  a.B = c.n; a.W = W_; a.H = H_;
+  if (c.fmt == IN_BGR) { a.frames = c.in; a.frame_pitch = c.pitch; a.frame_stride = c.stride; }
+  else { a.frames = d_frames_; a.frame_pitch = (size_t)W_ * 3; a.frame_stride = fbytes; }   // YUYV / NV12: the staging they are converted into
   if (nv12_in) {
-    a.nv12_in = d_yuyv_in; a.nv12_in_pitch = nv12_.pitch; a.nv12_in_uv = nv12_.uv; a.nv12_in_stride = nv12_.stride;
+    a.nv12_in = c.in; a.nv12_in_pitch = c.pitch; a.nv12_in_uv = c.uv; a.nv12_in_stride = c.stride;
   } else {
-    a.yuyv_in = d_yuyv_in; a.yuyv_in_stride = (size_t)W_ * H_ * 2;
+    a.yuyv_in = p.native ? c.in : nullptr; a.yuyv_in_stride = (size_t)W_ * H_ * 2;
   }
   a.bg = d_bg_; a.bg_pitch = (size_t)W_ * 3; a.bg_stride = 0;
   if (has_bg_) {
@@ -1199,15 +1192,15 @@ PostArgs Engine::post_args(int n, const uint8_t* d_frames, size_t pitch, size_t 
     a.bg = d_bg_frames_; a.bg_stride = fbytes;            // the blurred camera frame itself (filled by enqueue_post)
   }
   if (bg_yuyv_valid_ && !(bgblur_k_ && !has_bg_)) { a.bg_yuyv = d_bg_yuyv_; a.bg_nv12 = bg_nv12_valid_ ? d_bg_nv12_ : nullptr; }
-  if (call_mode_ != CALL_PLAIN) {
+  if (p.mode != CALL_PLAIN) {
     // sources: frame b blends bank slot bg_index[b]; the camera-blur slots' YUYV / NV12 are written by the call's
     // Gaussian, so every slot's cached copy is valid.  A call whose every frame is camera blur runs without them, as a
     // plain context in camera-blur mode does: each slot is read by one tile only, and converting the blurred BGR tile
     // the kernel loads anyway is cheaper than writing and re-reading a YUYV copy.
     a.bg = d_bank_; a.bg_stride = fbytes; a.bg_cursor = nullptr; a.bg_advance = 0;
     a.bg_index = d_src_tab_ + max_batch_; a.bg_count = bank_slots();
-    a.bg_yuyv = (!call_all_blur_ && !(W_ & 1)) ? d_bank_yuyv_ : nullptr;
-    a.bg_nv12 = call_all_blur_ ? nullptr : d_bank_nv12_;
+    a.bg_yuyv = (!p.all_blur && !(W_ & 1)) ? d_bank_yuyv_ : nullptr;
+    a.bg_nv12 = p.all_blur ? nullptr : d_bank_nv12_;
   }
   // the cached background in the call's video format (NV12 where the kernel writes NV12, else YUYV)
   if (nv12_in) a.bg_yuyv = nullptr; else a.bg_nv12 = nullptr;
@@ -1217,177 +1210,203 @@ PostArgs Engine::post_args(int n, const uint8_t* d_frames, size_t pitch, size_t 
   a.tab = tab_up_.tab; a.area2x2 = tab_up_.area2x2;
   a.out_pitch = (size_t)W_ * 3;
   if (!tail) {
-    a.out = d_out; a.out_stride = out_stride;
-    if (nv12_in) { a.nv12 = d_yuyv; a.nv12_stride = yuyv_stride; }
-    else { a.yuyv = d_yuyv; a.yuyv_stride = yuyv_stride; }
+    a.out = c.out; a.out_stride = c.out_stride;
+    uint8_t* video = p.nv12_staged ? d_yuyv_ : c.video;
+    const size_t vstride = p.nv12_staged ? (size_t)out_w_ * out_h_ * 2 : c.video_stride;
+    if (nv12_in) { a.nv12 = video; a.nv12_stride = vstride; }
+    else { a.yuyv = video; a.yuyv_stride = vstride; }
     // sources calls with flipped frames and no tail: k_post_tma writes the frames of the table's flip row mirrored.
     // Without flipped frames no table is passed, and the post kernel runs as for a plain call.
-    if (call_mode_ != CALL_PLAIN && call_flipped_) a.flip = d_src_tab_ + 3 * (size_t)max_batch_;
+    if (p.mode != CALL_PLAIN && p.flipped) a.flip = d_src_tab_ + 3 * (size_t)max_batch_;
   } else {
     a.out = want_rgb ? d_stage_a_ : nullptr; a.out_stride = fbytes;
     a.yuyv = nullptr; a.yuyv_stride = 0;
   }
-  a.mask = d_mask; a.mask_stride = mask_stride;
+  a.mask = c.mask; a.mask_stride = c.mask_stride;
   a.geo_rows = d_tile_geo_; a.geo_cols64 = d_tile_geo_ + geo_nty_; a.geo_cols128 = d_tile_geo_ + geo_nty_ + geo_ntx64_;
   return a;
 }
 
-bool Engine::enqueue_post(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
-                          uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in) {
-  const size_t fbytes = (size_t)W_ * H_ * 3;
-  const bool resized = out_w_ != W_ || out_h_ != H_, tail = call_tail();
+bool Engine::enqueue_post(const Call& c, const Plan& p) {
+  const int n = c.n;
+  const size_t fbytes = (size_t)W_ * H_ * 3, opix = (size_t)out_w_ * out_h_;
+  const bool resized = out_w_ != W_ || out_h_ != H_, tail = call_tail(p);
   // plain calls flip by the context; sources calls by frame, from the table's flip row
-  const bool flip = call_mode_ == CALL_PLAIN ? (flip_h_ || flip_v_) : call_flip_tail_;
-  const bool want_rgb = d_out || d_yuyv;
-  const bool ring = call_mode_ == CALL_PLAIN && has_bg_ && bg_count_ > 1;
+  const bool flip = p.mode == CALL_PLAIN ? (flip_h_ || flip_v_) : p.flip_tail;
+  const bool want_rgb = c.out || c.video;
+  const bool ring = p.mode == CALL_PLAIN && has_bg_ && bg_count_ > 1;
+  const PostArgs a = post_args(c, p);
   // app/deepseg.cc:652-658: no background source => the background is the blurred camera frame itself (sources: frame b
   // at its own strength into the bank's camera-blur slot b, with the slot's YUYV / NV12; the camera frame is read in
   // its wire format when the post kernel reads it so)
-  if (call_mode_ == CALL_SOURCES_CAMBLUR && want_rgb) {
+  if (p.mode == CALL_SOURCES_CAMBLUR && want_rgb) {
     // the slots' cached video format is the one the post kernel copies: NV12 when it reads the NV12 frames in place, else
     // YUYV (also for an NV12 call that falls back to BGR frames)
-    const bool nv12_in = nv12_.on && d_yuyv_in;
+    const bool nv12_in = p.native && c.fmt == IN_NV12;
     GaussSrc cam{};
-    if (nv12_in) cam = GaussSrc{d_yuyv_in, nv12_.pitch, nv12_.stride, nv12_.uv, IN_NV12};
-    else if (d_yuyv_in) cam = GaussSrc{d_yuyv_in, (size_t)W_ * 2, (size_t)W_ * H_ * 2, 0, IN_YUYV};
-    uint8_t* yv = (!call_all_blur_ && !nv12_in && !(W_ & 1)) ? d_bank_yuyv_ : nullptr;
-    uint8_t* nv = (!call_all_blur_ && nv12_in) ? d_bank_nv12_ : nullptr;
-    launch_gauss_frames(stream_, n, cam, d_src_tab_ + 2 * (size_t)max_batch_, call_gclass_, const_cast<uint8_t*>(d_frames), d_gauss_tmp_,
+    if (p.native) cam = GaussSrc{c.in, c.pitch, c.stride, c.uv, c.fmt};
+    uint8_t* yv = (!p.all_blur && !nv12_in && !(W_ & 1)) ? d_bank_yuyv_ : nullptr;
+    uint8_t* nv = (!p.all_blur && nv12_in) ? d_bank_nv12_ : nullptr;
+    launch_gauss_frames(stream_, n, cam, d_src_tab_ + 2 * (size_t)max_batch_, p.gclass, const_cast<uint8_t*>(a.frames), d_gauss_tmp_,
                         d_bank_, yv, nv, W_, H_);
-  } else if (call_mode_ == CALL_PLAIN && !has_bg_ && bgblur_k_ && want_rgb)
-    launch_gauss_blur(stream_, n, d_frames, pitch, stride, d_gauss_tmp_, d_bg_frames_, (size_t)W_ * 3, fbytes, W_, H_, taps_);
-  const PostArgs a = post_args(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in);
+  } else if (p.mode == CALL_PLAIN && !has_bg_ && bgblur_k_ && want_rgb)
+    launch_gauss_blur(stream_, n, a.frames, a.frame_pitch, a.frame_stride, d_gauss_tmp_, d_bg_frames_, (size_t)W_ * 3, fbytes, W_, H_, taps_);
   if (!launch_post(stream_, a)) return false;
   if (ring && bg_advance_) launch_advance_cursor(stream_, d_bg_cursor_, (int)(((long)n * bg_advance_) % bg_count_), bg_count_);
   if (!tail || !want_rgb) return true;
   // app/deepseg.cc:667-679: flip, then scale to the virtual-camera geometry, then YUYV (:681)
-  const size_t obytes = (size_t)out_w_ * out_h_ * 3;
+  const size_t obytes = opix * 3;
   const uint8_t* cur = d_stage_a_; size_t cur_stride = fbytes;
   if (flip) {
-    uint8_t* dst = (!resized && d_out) ? d_out : d_stage_b_;
-    const size_t ds = (!resized && d_out) ? out_stride : fbytes;
-    if (call_mode_ == CALL_PLAIN) launch_flip_u8c3(stream_, n, cur, cur_stride, dst, ds, W_, H_, flip_h_, flip_v_);
+    uint8_t* dst = (!resized && c.out) ? c.out : d_stage_b_;
+    const size_t ds = (!resized && c.out) ? c.out_stride : fbytes;
+    if (p.mode == CALL_PLAIN) launch_flip_u8c3(stream_, n, cur, cur_stride, dst, ds, W_, H_, flip_h_, flip_v_);
     else launch_flip_u8c3_frames(stream_, n, cur, cur_stride, dst, ds, W_, H_, d_src_tab_ + 3 * (size_t)max_batch_);
     cur = dst; cur_stride = ds;
   }
   if (resized) {
-    uint8_t* dst = d_out ? d_out : d_stage_c_;
-    const size_t ds = d_out ? out_stride : obytes;
+    uint8_t* dst = c.out ? c.out : d_stage_c_;
+    const size_t ds = c.out ? c.out_stride : obytes;
     launch_resize_u8c3(stream_, cur, W_, H_, (size_t)W_ * 3, dst, out_w_, out_h_, (size_t)out_w_ * 3, tab_out_.tab, tab_out_.area2x2, n, cur_stride, ds);
     cur = dst; cur_stride = ds;
   }
-  if (d_yuyv) launch_rgb_to_yuyv(stream_, cur, d_yuyv, (size_t)out_w_ * out_h_, n, cur_stride, yuyv_stride);
+  if (p.nv12_staged) launch_rgb_to_yuyv(stream_, cur, d_yuyv_, opix, n, cur_stride, opix * 2);
+  else if (c.video) launch_rgb_to_yuyv(stream_, cur, c.video, opix, n, cur_stride, c.video_stride);
   return true;
 }
 
 // Camera YUYV / NV12 input: the pre-processing kernel always reads the frames in place; the BGR frame is materialised
-// (k_yuyv_to_bgr / k_nv12_to_bgr into `d_frames`) only when the post stage cannot read the wire format itself — no TMA
+// (k_yuyv_to_bgr / k_nv12_to_bgr into d_frames_) only when the post stage cannot read the wire format itself — no TMA
 // path for this geometry or layout, or the blur-my-background mode of plain calls, whose Gaussian runs on the BGR frame
-// (a sources call's Gaussian reads the wire format itself).
-bool Engine::yuyv_native(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
-                         uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in) const {
+// (a sources call's Gaussian reads the wire format itself).  Decided on the call's own outputs.
+bool Engine::yuyv_native(const Call& c, Plan p) const {
   // a sources call whose every frame blurs its camera frame converts every frame to BGR for the Gaussian anyway, and the
   // post kernel reads BGR frames faster than it converts the wire format
-  const bool camblur = call_mode_ == CALL_PLAIN ? (bgblur_k_ && !has_bg_) : call_all_blur_;
-  if (!d_yuyv_in || camblur) return false;
-  return post_tma_eligible(post_args(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in));
+  const bool camblur = p.mode == CALL_PLAIN ? (bgblur_k_ && !has_bg_) : p.all_blur;
+  if (c.fmt == IN_BGR || camblur) return false;
+  p.native = true; p.nv12_staged = false;
+  return post_tma_eligible(post_args(c, p));
 }
 
-// NV12 output: the post kernel writes it when it reads the NV12 frames in place and no tail follows (a sources call
-// mirrored in place included); otherwise the YUYV output goes to the context staging and k_yuyv_to_nv12 derives the NV12
-// from it (the definition)
-bool Engine::nv12_staged(bool native, const uint8_t* d_yuyv) const { return nv12_.on && d_yuyv && !(native && !call_tail()); }
-
-// the PostArgs enqueue_all's post stage gets: camera frames in place when native, the video output staged per nv12_staged
-PostArgs Engine::call_post_args(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv,
-                                size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in, bool native) const {
-  const bool staged = nv12_staged(native, d_yuyv);
-  return post_args(n, d_frames, pitch, stride, d_out, out_stride, staged ? d_yuyv_ : d_yuyv, staged ? (size_t)out_w_ * out_h_ * 2 : yuyv_stride,
-                   d_mask, mask_stride, native ? d_yuyv_in : nullptr);
-}
-
-// Sources calls with flipped frames (app/deepseg.cc:667-681 flips before the resize): without a resize, and where
-// k_post_tma takes the call, it writes them mirrored in place; otherwise the tail flips them (and copies the others)
-// between the post kernel and the resize.  Decided where the call is enqueued (eagerly, or on a graph miss: the
-// GraphKey fixes everything the decision reads), so a replay costs no host work.
-bool Engine::plan_flips(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv,
-                        size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in, std::string* err) {
-  call_flip_tail_ = false;
-  if (call_mode_ == CALL_PLAIN || !call_flipped_) return true;
-  bool in_place = out_w_ == W_ && out_h_ == H_ && tuning().post_tma;
-  if (in_place) {
-    const bool native = yuyv_native(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in);
-    in_place = post_tma_eligible(call_post_args(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in, native));
-  }
-  call_flip_tail_ = !in_place;
-  if (call_flip_tail_ && (d_out || d_yuyv)) {
+// Decided where the call is enqueued (eagerly, or on a graph miss: the GraphKey fixes everything these decisions read),
+// so a replay costs no host work.
+bool Engine::plan_launch(const Call& c, Plan* p, std::string* err) {
+  // NV12 output: the post kernel writes it when it reads the NV12 frames in place and no tail follows (a sources call
+  // mirrored in place included); otherwise the YUYV output goes to the context staging and k_yuyv_to_nv12 derives the
+  // NV12 from it (the definition)
+  auto decide = [&] {
+    p->native = yuyv_native(c, *p);
+    p->nv12_staged = c.fmt == IN_NV12 && c.video && !(p->native && !call_tail(*p));
+  };
+  // Sources calls with flipped frames (app/deepseg.cc:667-681 flips before the resize): without a resize, and where
+  // k_post_tma takes the call, it writes them mirrored in place; otherwise the tail flips them (and copies the others)
+  // between the post kernel and the resize.
+  p->flip_tail = false;
+  if (p->mode != CALL_PLAIN && p->flipped) {
+    bool in_place = out_w_ == W_ && out_h_ == H_ && tuning().post_tma;
+    if (in_place) {
+      decide();
+      in_place = post_tma_eligible(post_args(c, *p));
+    }
+    p->flip_tail = !in_place;
     // set_output allocates the staging for a context flip / resize only; grown once (dropping the graphs) on first need
     const size_t fbytes = (size_t)max_batch_ * W_ * H_ * 3;
-    return ensure((void**)&d_stage_a_, &stage_a_cap_, fbytes, err) && ensure((void**)&d_stage_b_, &stage_b_cap_, fbytes, err);
+    if (p->flip_tail && (c.out || c.video) &&
+        !(ensure((void**)&d_stage_a_, &stage_a_cap_, fbytes, err) && ensure((void**)&d_stage_b_, &stage_b_cap_, fbytes, err)))
+      return false;
   }
+  decide();
   return true;
 }
 
-bool Engine::enqueue_all(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
-                         uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in,
-                         bool native, bool sync_cbs) {
+bool Engine::enqueue_all(const Call& c, const Plan& p) {
   const long l0 = thread_launch_count();
-  if (d_yuyv_in && !native) {
-    if (nv12_.on) launch_nv12_to_bgr(stream_, n, d_yuyv_in, nv12_.pitch, nv12_.uv, nv12_.stride, const_cast<uint8_t*>(d_frames), W_, H_);
-    else launch_yuyv_to_bgr(stream_, d_yuyv_in, const_cast<uint8_t*>(d_frames), (size_t)n * W_ * H_);
-  }
-  enqueue_pre(n, d_frames, pitch, stride, d_yuyv_in);
-  if (sync_cbs && cb_.onprep) { cudaStreamSynchronize(stream_); cb_.onprep(cb_.caller_ctx); }
+  const int n = c.n;
+  if (c.fmt == IN_NV12 && !p.native) launch_nv12_to_bgr(stream_, n, c.in, c.pitch, c.uv, c.stride, d_frames_, W_, H_);
+  if (c.fmt == IN_YUYV && !p.native) launch_yuyv_to_bgr(stream_, c.in, d_frames_, (size_t)n * W_ * H_);
+  enqueue_pre(c);
+  if (c.callbacks && cb_.onprep) { cudaStreamSynchronize(stream_); cb_.onprep(cb_.caller_ctx); }
   enqueue_cnn(n, true);
-  if (sync_cbs && cb_.oninfer) { cudaStreamSynchronize(stream_); cb_.oninfer(cb_.caller_ctx); }
-  enqueue_decision(n);
-  if (sync_cbs && cb_.onmask) { cudaStreamSynchronize(stream_); cb_.onmask(cb_.caller_ctx); }
-  const bool staged = nv12_staged(native, d_yuyv);
+  if (c.callbacks && cb_.oninfer) { cudaStreamSynchronize(stream_); cb_.oninfer(cb_.caller_ctx); }
+  enqueue_decision(n, p.mode != CALL_PLAIN);
+  if (c.callbacks && cb_.onmask) { cudaStreamSynchronize(stream_); cb_.onmask(cb_.caller_ctx); }
+  if (!enqueue_post(c, p)) return false;
   const size_t opix = (size_t)out_w_ * out_h_;
-  // the arguments call_post_args gives (plan_flips decides on those)
-  if (!enqueue_post(n, d_frames, pitch, stride, d_out, out_stride, staged ? d_yuyv_ : d_yuyv, staged ? opix * 2 : yuyv_stride, d_mask,
-                    mask_stride, native ? d_yuyv_in : nullptr))
-    return false;
-  if (staged) launch_yuyv_to_nv12(stream_, n, d_yuyv_, opix * 2, d_yuyv, yuyv_stride, out_w_, out_h_);
+  if (p.nv12_staged) launch_yuyv_to_nv12(stream_, n, d_yuyv_, opix * 2, c.video, c.video_stride, out_w_, out_h_);
   last_call_launches_ = (int)(thread_launch_count() - l0);
   return true;
 }
 
-bool Engine::run(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
-                 uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, bool use_callbacks, std::string* err,
-                 const uint8_t* d_yuyv_in) {
+bool Engine::run(const Call& c, std::string* err) {
+  const int n = c.n;
+  if (c.fmt == IN_NV12) {
+    if ((W_ & 1) || (H_ & 1)) { *err = "NV12 needs an even frame width and height"; return false; }
+    if (c.video && ((out_w_ & 1) || (out_h_ & 1))) { *err = "NV12 output needs an even output width and height"; return false; }
+    if (!c.in) { *err = "invalid frame"; return false; }
+    if (c.pitch < (size_t)W_) { *err = "NV12 row pitch is smaller than the frame width"; return false; }
+    if (c.uv < c.pitch * H_) { *err = "NV12 UV plane offset lies inside the Y plane"; return false; }
+    if (c.stride < c.uv + c.pitch * (size_t)(H_ / 2 - 1) + (size_t)W_) { *err = "NV12 frame does not fit in the frame stride"; return false; }
+  }
+  if (c.ids && !n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
   if (n < 1 || n > max_batch_) { *err = "n_frames out of range (1..max_batch)"; return false; }
-  if (d_yuyv_in && (W_ & 1)) { *err = "YUYV ingest needs an even width"; return false; }
+  Plan p;
+  std::vector<int> tab;
+  if (c.ids) {
+    if (has_bg_ && bg_count_ > 1) { *err = "sources calls need a still context background (animate a source with bsb_set_source_background)"; return false; }
+    // frame b: state of source ids[b]; background (source_bg) = the context slot, the source's slot, or its camera frame
+    // blurred at the source's strength into camera-blur slot b; flip = the source's own, else the context's
+    tab.assign(4 * (size_t)max_batch_, 0);
+    int n_blur = 0;
+    const int ctx_flip = (flip_h_ ? 1 : 0) | (flip_v_ ? 2 : 0);
+    for (int b = 0; b < n; ++b) {
+      const int id = c.ids[b];
+      if (id < 0 || id >= n_sources_) { *err = "source id out of range"; return false; }
+      for (int j = 0; j < b; ++j)
+        if (c.ids[j] == id) { *err = "source ids must be distinct within one call"; return false; }
+      tab[b] = id;
+      int k = 0;
+      const int from = source_bg(id, &k);
+      int slot = max_batch_;
+      if (from == SRC_FROM_SLOT) slot = max_batch_ + 1 + id;
+      else if (from == SRC_FROM_CAMBLUR) { slot = b; tab[2 * (size_t)max_batch_ + b] = k; p.gclass |= (unsigned)gauss_class(k); ++n_blur; }
+      tab[(size_t)max_batch_ + b] = slot;
+      const int fl = src_flip_[id] < 0 ? ctx_flip : src_flip_[id];
+      tab[3 * (size_t)max_batch_ + b] = fl;
+      p.flipped = p.flipped || fl != 0;
+    }
+    p.mode = p.gclass ? CALL_SOURCES_CAMBLUR : CALL_SOURCES;
+    p.all_blur = n_blur == n;
+  }
+  if (c.fmt != IN_BGR && (W_ & 1)) { *err = "YUYV ingest needs an even width"; return false; }
   CUDA_OK(cudaSetDevice(device_));
-  const bool cbs = use_callbacks && (cb_.onprep || cb_.oninfer || cb_.onmask);
+  if (c.ids) {
+    if ((p.gclass & GAUSS_SEPARABLE) && !ensure_gauss_tmp(err)) return false;
+    // outside the graph, before its launch: stream order keeps the previous launch's reads ahead of this write
+    CUDA_OK(cudaMemcpyAsync(d_src_tab_, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, stream_));
+  }
+  const bool cbs = c.callbacks && (cb_.onprep || cb_.oninfer || cb_.onmask);
   bool eager = cbs || (flags_ & 2u);
 #ifdef BSB_EMU
   eager = true;
 #endif
   static const char* kNoMirror = "the post kernel cannot write this call's mirrored frames";
   if (eager) {
-    if (!plan_flips(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in, err)) return false;
-    const bool native = yuyv_native(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in);
-    last_native_ = native;
-    if (!enqueue_all(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in, native, cbs)) {
-      *err = kNoMirror; return false;
-    }
+    if (!plan_launch(c, &p, err)) return false;
+    last_native_ = p.native;
+    if (!enqueue_all(c, p)) { *err = kNoMirror; return false; }
     CUDA_OK(cudaGetLastError());
     return true;
   }
 #ifndef BSB_EMU
-  const GraphKey key{n, d_frames, pitch, stride, d_out, d_yuyv, d_mask, d_yuyv_in, d_out ? out_stride : 0, d_yuyv ? yuyv_stride : 0,
-                     d_mask ? mask_stride : 0, call_mode_, call_gclass_, call_all_blur_, nv12_.on, nv12_.pitch, nv12_.uv, nv12_.stride,
-                     call_flipped_};
+  const GraphKey key(c, p);
   auto it = graphs_.find(key);
   if (it == graphs_.end()) {
     if (graphs_.size() >= 64) drop_graphs();
-    if (!plan_flips(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in, err)) return false;
-    const bool native = yuyv_native(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in);
-    last_native_ = native;
+    if (!plan_launch(c, &p, err)) return false;
+    last_native_ = p.native;
     cudaGraph_t graph = nullptr;
     CUDA_OK(cudaStreamBeginCapture(stream_, cudaStreamCaptureModeThreadLocal));
-    const bool enq = enqueue_all(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, d_yuyv_in, native, false);
+    const bool enq = enqueue_all(c, p);
     // the capture is always closed, also when a launch inside it failed: a stream left in capture mode would
     // poison every later call on this context
     const cudaError_t ce = cudaStreamEndCapture(stream_, &graph);
@@ -1413,28 +1432,6 @@ bool Engine::run(int n, const uint8_t* d_frames, size_t pitch, size_t stride, ui
   CUDA_OK(cudaGraphLaunch(it->second.exec, stream_));
 #endif
   return true;
-}
-
-bool Engine::run_yuyv(int n, const uint8_t* d_yuyv_in, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv, size_t yuyv_stride,
-                      uint8_t* d_mask, size_t mask_stride, std::string* err) {
-  const size_t row = (size_t)W_ * 3;
-  return run(n, d_frames_, row, row * H_, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, false, err, d_yuyv_in);
-}
-
-bool Engine::run_nv12(int n, const int* ids, const uint8_t* d_nv12, size_t pitch, size_t uv_off, size_t in_stride, uint8_t* d_out,
-                      size_t out_stride, uint8_t* d_nv12_out, size_t nv12_stride, uint8_t* d_mask, size_t mask_stride, std::string* err) {
-  if ((W_ & 1) || (H_ & 1)) { *err = "NV12 needs an even frame width and height"; return false; }
-  if (d_nv12_out && ((out_w_ & 1) || (out_h_ & 1))) { *err = "NV12 output needs an even output width and height"; return false; }
-  if (!d_nv12) { *err = "invalid frame"; return false; }
-  if (pitch < (size_t)W_) { *err = "NV12 row pitch is smaller than the frame width"; return false; }
-  if (uv_off < pitch * H_) { *err = "NV12 UV plane offset lies inside the Y plane"; return false; }
-  if (in_stride < uv_off + pitch * (size_t)(H_ / 2 - 1) + (size_t)W_) { *err = "NV12 frame does not fit in the frame stride"; return false; }
-  const size_t row = (size_t)W_ * 3;
-  nv12_ = Nv12Call{true, pitch, uv_off, in_stride};
-  const bool ok = ids ? run_sources(n, ids, d_frames_, row, row * H_, d_out, out_stride, d_nv12_out, nv12_stride, d_mask, mask_stride, err, d_nv12)
-                      : run(n, d_frames_, row, row * H_, d_out, out_stride, d_nv12_out, nv12_stride, d_mask, mask_stride, false, err, d_nv12);
-  nv12_ = Nv12Call{};
-  return ok;
 }
 
 uint8_t* Engine::nv12_staging(std::string* err) {
@@ -1783,72 +1780,24 @@ bool Engine::set_source_background(int source, const uint8_t* bg_raw, int bw, in
   return true;
 }
 
-bool Engine::run_sources(int n, const int* ids, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
-                         uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, std::string* err,
-                         const uint8_t* d_yuyv_in) {
-  if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
-  if (n < 1 || n > max_batch_) { *err = "n_frames out of range (1..max_batch)"; return false; }
-  if (!ids) { *err = "null source id table"; return false; }
-  if (has_bg_ && bg_count_ > 1) { *err = "sources calls need a still context background (animate a source with bsb_set_source_background)"; return false; }
-  // frame b: state of source ids[b]; background (source_bg) = the context slot, the source's slot, or its camera frame
-  // blurred at the source's strength into camera-blur slot b; flip = the source's own, else the context's
-  std::vector<int> tab(4 * (size_t)max_batch_, 0);
-  unsigned classes = 0;
-  int n_blur = 0;
-  bool flipped = false;                          // some frame of the call is mirrored
-  const int ctx_flip = (flip_h_ ? 1 : 0) | (flip_v_ ? 2 : 0);
-  for (int b = 0; b < n; ++b) {
-    const int id = ids[b];
-    if (id < 0 || id >= n_sources_) { *err = "source id out of range"; return false; }
-    for (int c = 0; c < b; ++c)
-      if (ids[c] == id) { *err = "source ids must be distinct within one call"; return false; }
-    tab[b] = id;
-    int k = 0;
-    const int from = source_bg(id, &k);
-    int slot = max_batch_;
-    if (from == SRC_FROM_SLOT) slot = max_batch_ + 1 + id;
-    else if (from == SRC_FROM_CAMBLUR) { slot = b; tab[2 * (size_t)max_batch_ + b] = k; classes |= (unsigned)gauss_class(k); ++n_blur; }
-    tab[(size_t)max_batch_ + b] = slot;
-    const int fl = src_flip_[id] < 0 ? ctx_flip : src_flip_[id];
-    tab[3 * (size_t)max_batch_ + b] = fl;
-    flipped = flipped || fl != 0;
-  }
-  CUDA_OK(cudaSetDevice(device_));
-  if ((classes & GAUSS_SEPARABLE) && !ensure_gauss_tmp(err)) return false;
-  // outside the graph, before its launch: stream order keeps the previous launch's reads ahead of this write
-  CUDA_OK(cudaMemcpyAsync(d_src_tab_, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, stream_));
-  call_mode_ = classes ? CALL_SOURCES_CAMBLUR : CALL_SOURCES;
-  call_gclass_ = classes;
-  call_all_blur_ = n_blur == n;
-  call_flipped_ = flipped;
-  const bool ok = run(n, d_frames, pitch, stride, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, false, err, d_yuyv_in);
-  call_mode_ = CALL_PLAIN;
-  call_gclass_ = 0;
-  call_all_blur_ = false;
-  call_flipped_ = false;
-  call_flip_tail_ = false;
-  return ok;
-}
-
-bool Engine::run_sources_yuyv(int n, const int* ids, const uint8_t* d_yuyv_in, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv,
-                              size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, std::string* err) {
-  const size_t row = (size_t)W_ * 3;
-  return run_sources(n, ids, d_frames_, row, row * H_, d_out, out_stride, d_yuyv, yuyv_stride, d_mask, mask_stride, err, d_yuyv_in);
-}
-
 double Engine::time_stage(int stage, int n, int iters, std::string* err) {
   if (n < 1 || n > max_batch_ || iters < 1 || stage < 0 || stage > 4) { *err = "bad arguments"; return -1.0; }
   if (cudaSetDevice(device_) != cudaSuccess) { *err = "cudaSetDevice failed"; return -1.0; }
   const size_t row = (size_t)W_ * 3, fbytes = row * H_, npix = (size_t)W_ * H_;
   cudaEvent_t e0, e1;
   cudaEventCreate(&e0); cudaEventCreate(&e1);
-  // the last call's input format decides which kernels are timed (camera YUYV read in place, or BGR frames)
-  const uint8_t* yin = last_native_ ? d_yuyv_in_ : nullptr;
+  // a plain call on the context buffers; the last call's input format decides which kernels are timed (camera YUYV read
+  // in place, or BGR frames)
+  const bool yuyv = last_native_;
+  const Call c{n, yuyv ? IN_YUYV : IN_BGR, yuyv ? d_yuyv_in_ : d_frames_, yuyv ? (size_t)W_ * 2 : row, 0, yuyv ? npix * 2 : fbytes,
+               nullptr, d_out_, fbytes, d_yuyv_, npix * 2, d_mask_, npix};
+  Plan p;
+  p.native = yuyv;
   auto once = [&]() {
-    if (stage == 0 || stage == 4) enqueue_pre(n, d_frames_, row, fbytes, yin);
+    if (stage == 0 || stage == 4) enqueue_pre(c);
     if (stage == 1 || stage == 4) enqueue_cnn(n, true);
-    if (stage == 2 || stage == 4) enqueue_decision(n);
-    if (stage == 3 || stage == 4) (void)enqueue_post(n, d_frames_, row, fbytes, d_out_, fbytes, d_yuyv_, npix * 2, d_mask_, npix, yin);
+    if (stage == 2 || stage == 4) enqueue_decision(n, false);
+    if (stage == 3 || stage == 4) (void)enqueue_post(c, p);
   };
   once();                                   // warm-up (instruction cache, tables)
   cudaStreamSynchronize(stream_);

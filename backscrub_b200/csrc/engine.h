@@ -73,19 +73,28 @@ struct Callbacks {
   void* caller_ctx = nullptr;
 };
 
+// One fused call: n camera frames in, up to three outputs (any may be null).  Device memory, byte pitches and strides.
+struct Call {
+  int n = 0;
+  InFmt fmt = IN_BGR;                // BGR, YUYV (tightly packed: pitch W*2, stride W*H*2) or NV12 (W and H even)
+  const uint8_t* in = nullptr;
+  size_t pitch = 0, uv = 0, stride = 0;   // row pitch, NV12's UV plane offset inside a frame (else 0), frame stride
+  const int* ids = nullptr;          // HOST array: frame b belongs to source ids[b] (n distinct ids); null: a plain call
+  uint8_t* out = nullptr; size_t out_stride = 0;       // BGR composite, out_w x out_h, rows out_w*3 bytes
+  uint8_t* video = nullptr; size_t video_stride = 0;   // tightly packed YUYV, or NV12 when the input is NV12
+  uint8_t* mask = nullptr; size_t mask_stride = 0;     // W x H
+  bool callbacks = false;            // fire the stage callbacks (the call then runs eagerly, synchronised at each stage)
+};
+
 class Engine {
  public:
   static Engine* create(const std::string& model_path, int width, int height, int device, int max_batch,
                         unsigned flags, const Callbacks& cb, std::string* err);
   ~Engine();
 
-  // frames on device: n frames, row pitch / frame stride in bytes.  Any output may be null.
-  bool run(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
-           uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, bool use_callbacks, std::string* err,
-           const uint8_t* d_yuyv_in = nullptr);
-  // same, from camera YUYV frames (tightly packed W*2 rows): converted to BGR into the context staging first
-  bool run_yuyv(int n, const uint8_t* d_yuyv_in, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv, size_t yuyv_stride,
-                uint8_t* d_mask, size_t mask_stride, std::string* err);
+  // Enqueues one call on the context's stream (a captured graph, replayed when the call matches one).  YUYV / NV12 frames
+  // that have to be read as BGR are converted into the context staging d_frames().
+  bool run(const Call& c, std::string* err);
   bool infer(int n, const float* h_in, float* h_out, std::string* err);
   bool set_background(const uint8_t* bg_raw, int bw, int bh, size_t pitch, std::string* err) {
     return set_background_ring(bg_raw, 1, bw, bh, pitch, 0, 0, err);
@@ -117,17 +126,6 @@ class Engine {
   // mirroring of one source: -1 follows set_output's flips, 0..3 its own (bit 0 horizontal, bit 1 vertical).  Host
   // bookkeeping only: the flip reaches the device through the per-frame table of each call.
   bool set_source_flip(int source, int flip, std::string* err);
-  // frame b belongs to source ids[b] (HOST array of n distinct ids); same buffers / layout as run()
-  bool run_sources(int n, const int* ids, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
-                   uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, std::string* err,
-                   const uint8_t* d_yuyv_in = nullptr);
-  bool run_sources_yuyv(int n, const int* ids, const uint8_t* d_yuyv_in, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv, size_t yuyv_stride,
-                        uint8_t* d_mask, size_t mask_stride, std::string* err);
-  // Camera NV12 frames (W, H even): Y rows `pitch` bytes apart, the UV plane at byte `uv_off` of a frame, `in_stride` bytes
-  // per frame.  The video output is tightly packed NV12 (`nv12_stride` bytes per frame).  ids == nullptr: a plain call,
-  // else a sources call as run_sources.
-  bool run_nv12(int n, const int* ids, const uint8_t* d_nv12, size_t pitch, size_t uv_off, size_t in_stride, uint8_t* d_out, size_t out_stride,
-                uint8_t* d_nv12_out, size_t nv12_stride, uint8_t* d_mask, size_t mask_stride, std::string* err);
   // device staging of max_batch NV12 output frames (host-buffer API), grown on demand; nullptr on error
   uint8_t* nv12_staging(std::string* err);
   int n_sources() const { return n_sources_; }
@@ -183,32 +181,37 @@ class Engine {
   Engine() = default;
   bool plan(std::string* err);
   bool upload(std::string* err);
-  void enqueue_pre(int n, const uint8_t* d_frames, size_t pitch, size_t stride, const uint8_t* d_yuyv_in = nullptr);
-  PostArgs post_args(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
-                     uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in) const;
-  bool yuyv_native(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
-                   uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in) const;
+  // What the engine derives from a Call and the context: the kind of call — plain (one stream, state_), sources, or
+  // sources with at least one frame that blends its own blurred camera frame (a source with no image and a strength > 0)
+  // — and how it is enqueued.
+  enum CallMode { CALL_PLAIN = 0, CALL_SOURCES = 1, CALL_SOURCES_CAMBLUR = 2 };
+  struct Plan {
+    int mode = CALL_PLAIN;
+    unsigned gclass = 0;             // sources: the Gaussian launch classes of the camera-blur frames (GAUSS_FUSED | GAUSS_SEPARABLE)
+    bool all_blur = false;           // sources: every frame blurs its camera frame (the BGR frames are materialised)
+    bool flipped = false;            // sources: some frame is mirrored (the table's flip row is not all 0)
+    bool flip_tail = false;          // ... and the tail mirrors them (k_flip_u8c3_frames): the call resizes or its post kernel
+                                     // is not k_post_tma
+    bool native = false;             // the post stage reads the camera frames (YUYV or NV12) in place, no BGR frame is materialised
+    bool nv12_staged = false;        // the NV12 output is converted from a YUYV output staged in d_yuyv_ (k_yuyv_to_nv12)
+  };
+  // flip_tail, native and nv12_staged (and the tail's staging); false with *err when a buffer cannot be grown
+  bool plan_launch(const Call& c, Plan* p, std::string* err);
+  void enqueue_pre(const Call& c);
+  PostArgs post_args(const Call& c, const Plan& p) const;
+  bool yuyv_native(const Call& c, Plan p) const;
   // the call ends with a stand-alone tail (post -> stage -> flip -> resize -> YUYV): plain calls with a context flip or
   // resize; sources calls with a resize, or with mirrored frames the post kernel cannot mirror in place
-  bool call_tail() const {
+  bool call_tail(const Plan& p) const {
     const bool resized = out_w_ != W_ || out_h_ != H_;
-    return call_mode_ == CALL_PLAIN ? (flip_h_ || flip_v_ || resized) : (resized || call_flip_tail_);
+    return p.mode == CALL_PLAIN ? (flip_h_ || flip_v_ || resized) : (resized || p.flip_tail);
   }
-  bool nv12_staged(bool native, const uint8_t* d_yuyv) const;
-  PostArgs call_post_args(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv,
-                          size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in, bool native) const;
-  // sources calls with flipped frames: sets call_flip_tail_ (and grows the tail's staging when it is needed)
-  bool plan_flips(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride, uint8_t* d_yuyv,
-                  size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in, std::string* err);
   // false (nothing more enqueued) only when the post kernel cannot write a call's mirrored frames
-  bool enqueue_all(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
-                   uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in,
-                   bool native, bool sync_cbs);
+  bool enqueue_all(const Call& c, const Plan& p);
   bool refresh_bg_yuyv(std::string* err);
   void enqueue_cnn(int n, bool from_u8);
-  void enqueue_decision(int n);
-  bool enqueue_post(int n, const uint8_t* d_frames, size_t pitch, size_t stride, uint8_t* d_out, size_t out_stride,
-                    uint8_t* d_yuyv, size_t yuyv_stride, uint8_t* d_mask, size_t mask_stride, const uint8_t* d_yuyv_in = nullptr);
+  void enqueue_decision(int n, bool sources);
+  bool enqueue_post(const Call& c, const Plan& p);
   // base of tensor t for the frames [frame_off_, ...) of the batch (frame_off_ != 0 only inside a sub-batched segment)
   float* tptr(int t) const {
     const TensorInfo& I = tinfo_[t];
@@ -310,26 +313,12 @@ class Engine {
   size_t bg_nv12_cap_ = 0;
   bool bg_nv12_valid_ = false;
   bool last_native_ = false;         // the last call read the camera frames (YUYV or NV12) in place (no BGR frame was materialised)
-  // Format of the NV12 call being enqueued (set by run_nv12 around run / run_sources, like call_mode_): the camera pointer
-  // (d_yuyv_in) holds NV12 frames with this layout, and the video output pointer (d_yuyv) receives NV12
-  struct Nv12Call { bool on = false; size_t pitch = 0, uv = 0, stride = 0; };
-  Nv12Call nv12_;
   uint8_t* d_nv12_ = nullptr;        // host-buffer API staging of the NV12 output
   size_t nv12_cap_ = 0;
   int last_call_launches_ = 0;
   size_t stage_a_cap_ = 0, stage_b_cap_ = 0, stage_c_cap_ = 0, out_cap_ = 0, yuyv_cap_ = 0;
 
-  // ---- independent sources (run_sources) ----
-  // Kind of the call being enqueued: plain (one stream, state_), sources, or sources with at least one frame that blends
-  // its own blurred camera frame (a source with no image and a strength > 0), in the Gaussian launch classes
-  // call_gclass_ (GAUSS_FUSED | GAUSS_SEPARABLE).
-  enum CallMode { CALL_PLAIN = 0, CALL_SOURCES = 1, CALL_SOURCES_CAMBLUR = 2 };
-  int call_mode_ = CALL_PLAIN;
-  unsigned call_gclass_ = 0;
-  bool call_all_blur_ = false;       // ... and every frame of the call blurs its camera frame (the BGR frames are materialised)
-  bool call_flipped_ = false;        // ... and some frame of the call is mirrored (the table's flip row is not all 0)
-  bool call_flip_tail_ = false;      // ... and its tail mirrors them (k_flip_u8c3_frames): the call resizes or its post kernel is
-                                     // not k_post_tma (plan_flips)
+  // ---- independent sources (calls with ids) ----
   int n_sources_ = 0;
   uint8_t* src_state_ = nullptr;     // [n_sources][oh*ow] smoother state per source
   // [4][max_batch]: source id of frame b | background-bank slot of frame b | camera-blur strength of frame b (0 = none) |
@@ -360,21 +349,20 @@ class Engine {
   bool ensure_gauss_tmp(std::string* err);
   void free_sources();
 
-  // everything a captured launch sequence bakes into its kernel arguments
+  // Everything a captured launch sequence bakes into its kernel arguments: the call's buffers and layouts (the stride of
+  // an absent output does not matter), and the plan's mode (a plain and a sources graph over the same buffers are
+  // different graphs), Gaussian classes (strengths within them replay), all-blur and flipped (which frames flip is table
+  // data).  The rest of the plan is decided from these.
   struct GraphKey {
-    int n; const void* f; size_t pitch, stride; const void* o; const void* y; const void* m; const void* yin;
-    size_t ostride, ystride, mstride;
-    int mode;                        // CallMode: a plain and a sources graph over the same buffers are different graphs
-    unsigned gclass;                 // call_gclass_: the Gaussian launches captured (strengths within them replay)
-    bool all_blur;                   // call_all_blur_: the camera frames were converted to BGR before the graph's kernels
-    bool nv12; size_t npitch, nuv, nstride;   // NV12 call and its input layout: never confused with a YUYV call
-    bool flipped;                    // call_flipped_: the post kernel mirrors in place, or the tail contains the per-frame flip
-                                     // (decided from the rest of the key); which frames flip is table data
-    bool operator<(const GraphKey& r) const {
-      return std::tie(n, f, pitch, stride, o, y, m, yin, ostride, ystride, mstride, mode, gclass, all_blur, nv12, npitch, nuv, nstride, flipped) <
-             std::tie(r.n, r.f, r.pitch, r.stride, r.o, r.y, r.m, r.yin, r.ostride, r.ystride, r.mstride, r.mode, r.gclass, r.all_blur, r.nv12, r.npitch, r.nuv,
-                      r.nstride, r.flipped);
-    }
+    int n, fmt; const void* in; size_t pitch, uv, stride;
+    const void* out; const void* video; const void* mask; size_t ostride, vstride, mstride;
+    int mode; unsigned gclass; bool all_blur, flipped;
+    GraphKey(const Call& c, const Plan& p)
+        : n(c.n), fmt(c.fmt), in(c.in), pitch(c.pitch), uv(c.uv), stride(c.stride), out(c.out), video(c.video), mask(c.mask),
+          ostride(c.out ? c.out_stride : 0), vstride(c.video ? c.video_stride : 0), mstride(c.mask ? c.mask_stride : 0),
+          mode(p.mode), gclass(p.gclass), all_blur(p.all_blur), flipped(p.flipped) {}
+    auto tie() const { return std::tie(n, fmt, in, pitch, uv, stride, out, video, mask, ostride, vstride, mstride, mode, gclass, all_blur, flipped); }
+    bool operator<(const GraphKey& r) const { return tie() < r.tie(); }
   };
 #ifndef BSB_EMU
   struct CapturedCall { cudaGraphExec_t exec; int launches; };
