@@ -47,6 +47,7 @@ class MaskGen:
             raise BackscrubError("".join(self._msgs).strip() or lib.bsb_last_error().decode())
         self.width, self.height, self.max_batch, self.device = width, height, max_batch, device
         self.out_width, self.out_height = width, height
+        self._n_sources, self._src_out = 0, {}       # sources with their own output size: source -> (w, h)
         r, i, o = (C.c_int * 4)(), (C.c_int * 4)(), (C.c_int * 4)()
         ih, oh = (C.c_int * 3)(), (C.c_int * 3)()
         lib.bsb_geometry(self._h, r, i, o, ih, oh)
@@ -246,6 +247,7 @@ class MaskGen:
         """n_sources zeroed smoother states + per-source background slots (again: everything reset)."""
         if not self._lib.bsb_set_sources(self._h, int(n_sources)):
             self._fail("bsb_set_sources")
+        self._n_sources, self._src_out = int(n_sources), {}
 
     def reset_source(self, source: int):
         """start `source` over as a new camera (its smoother state is zeroed)"""
@@ -280,45 +282,86 @@ class MaskGen:
         if not self._lib.bsb_set_source_flip(self._h, int(source), flip):
             self._fail("bsb_set_source_flip")
 
+    def set_source_output(self, source: int, out_size=None):
+        """virtual-camera size of one source (cv::resize after the flip, app/deepseg.cc:677-679): out_size = (w, h), or
+        None to follow set_output's size, including later changes.  The mask stays W x H."""
+        ow, oh = out_size if out_size else (0, 0)
+        if not self._lib.bsb_set_source_output(self._h, int(source), int(ow), int(oh)):
+            self._fail("bsb_set_source_output")
+        if out_size:
+            self._src_out[int(source)] = (int(ow), int(oh))
+        else:
+            self._src_out.pop(int(source), None)
+
+    def source_output_size(self, source: int):
+        """(w, h) of one source's composites: its own size, or the context's"""
+        w, h = C.c_int(), C.c_int()
+        if not self._lib.bsb_source_output_size(self._h, int(source), C.byref(w), C.byref(h)):
+            self._fail("bsb_source_output_size")
+        return w.value, h.value
+
+    def _sources_out_px(self):
+        """pixels of the largest effective output size among the sources (the context's when no source has its own)"""
+        sizes = list(self._src_out.values())
+        if len(sizes) < self._n_sources or not sizes:
+            sizes.append((self.out_width, self.out_height))
+        return max(w * h for w, h in sizes)
+
     def composite_sources(self, frames: np.ndarray, ids, want_out=True, want_yuyv=True, want_mask=True):
-        """HOST buffers: frames [n, H, W, 3], frame b the next frame of source ids[b] (distinct ids) -> (out, yuyv, mask)."""
+        """HOST buffers: frames [n, H, W, 3], frame b the next frame of source ids[b] (distinct ids) -> (out, yuyv, mask).
+        out / yuyv are stacked arrays when every frame of the call has one output size, else lists of per-frame arrays."""
         frames = np.ascontiguousarray(frames, np.uint8)
         n, tab = self._ids(ids)
         if frames.shape != (n, self.height, self.width, 3):
             raise BackscrubError(f"frames shape {frames.shape} != {(n, self.height, self.width, 3)}")
         fb, npx = self.height * self.width * 3, self.height * self.width
-        ow, oh = self.out_width, self.out_height
-        out = np.empty((n, oh, ow, 3), np.uint8) if want_out else None
-        yuyv = np.empty((n, oh, ow, 2), np.uint8) if want_yuyv else None
+        sizes = [self._src_out.get(int(s), (self.out_width, self.out_height)) for s in ids]
+        opx = max(w * h for w, h in sizes) if sizes else self.out_width * self.out_height
+        out = np.empty(n * opx * 3, np.uint8) if want_out else None
+        yuyv = np.empty(n * opx * 2, np.uint8) if want_yuyv else None
         mask = np.empty((n, self.height, self.width), np.uint8) if want_mask else None
         ok = self._lib.bsb_composite_sources(self._h, n, tab, _ptr(frames), self.width * 3, fb,
-                                             _ptr(out) if want_out else None, ow * oh * 3,
-                                             _ptr(yuyv) if want_yuyv else None, ow * oh * 2,
+                                             _ptr(out) if want_out else None, opx * 3,
+                                             _ptr(yuyv) if want_yuyv else None, opx * 2,
                                              _ptr(mask) if want_mask else None, npx)
         if not ok:
             self._fail("bsb_composite_sources")
-        return out, yuyv, mask
 
-    def composite_sources_yuyv_device(self, n, ids, d_yuyv_in, d_out=0, d_yuyv=0, d_mask=0, sync=False):
-        """DEVICE-resident camera YUYV frames (tightly packed), frame b of source ids[b]; asynchronous unless `sync`."""
+        def shape(buf, ch):
+            if buf is None:
+                return None
+            if len(set(sizes)) == 1:
+                ow, oh = sizes[0]
+                return buf.reshape(n, oh, ow, ch)
+            return [buf[b * opx * ch: b * opx * ch + w * h * ch].reshape(h, w, ch) for b, (w, h) in enumerate(sizes)]
+        return shape(out, 3), shape(yuyv, 2), mask
+
+    def composite_sources_yuyv_device(self, n, ids, d_yuyv_in, d_out=0, d_yuyv=0, d_mask=0, sync=False, out_stride=None, yuyv_stride=None):
+        """DEVICE-resident camera YUYV frames (tightly packed), frame b of source ids[b]; asynchronous unless `sync`.  Frame b's
+        outputs are packed at its own size, out_stride / yuyv_stride bytes apart (default: the largest size of the sources)."""
         m, tab = self._ids(ids)
         if m != n:
             raise BackscrubError(f"{m} source ids for {n} frames")
-        npx, opx = self.height * self.width, self.out_width * self.out_height
-        if not self._lib.bsb_composite_sources_yuyv_device(self._h, n, tab, d_yuyv_in, d_out or None, opx * 3, d_yuyv or None, opx * 2,
+        npx, opx = self.height * self.width, self._sources_out_px()
+        ost = opx * 3 if out_stride is None else int(out_stride)
+        vst = opx * 2 if yuyv_stride is None else int(yuyv_stride)
+        if not self._lib.bsb_composite_sources_yuyv_device(self._h, n, tab, d_yuyv_in, d_out or None, ost, d_yuyv or None, vst,
                                                            d_mask or None, npx, int(sync)):
             self._fail("bsb_composite_sources_yuyv_device")
 
     def composite_sources_nv12_device(self, n, ids, d_nv12, d_out=0, d_nv12_out=0, d_mask=0, sync=False, pitch=None, uv_offset=None,
-                                      in_stride=None):
-        """DEVICE-resident camera NV12 frames (layout as composite_nv12_device), frame b of source ids[b]."""
+                                      in_stride=None, out_stride=None, nv12_stride=None):
+        """DEVICE-resident camera NV12 frames (layout as composite_nv12_device), frame b of source ids[b]; output strides as
+        composite_sources_yuyv_device."""
         m, tab = self._ids(ids)
         if m != n:
             raise BackscrubError(f"{m} source ids for {n} frames")
         p, uv, st = self._nv12_layout(pitch, uv_offset, in_stride)
-        npx, opx = self.height * self.width, self.out_width * self.out_height
-        if not self._lib.bsb_composite_sources_nv12_device(self._h, n, tab, d_nv12, p, uv, st, d_out or None, opx * 3, d_nv12_out or None,
-                                                           opx * 3 // 2, d_mask or None, npx, int(sync)):
+        npx, opx = self.height * self.width, self._sources_out_px()
+        ost = opx * 3 if out_stride is None else int(out_stride)
+        vst = opx * 3 // 2 if nv12_stride is None else int(nv12_stride)
+        if not self._lib.bsb_composite_sources_nv12_device(self._h, n, tab, d_nv12, p, uv, st, d_out or None, ost, d_nv12_out or None,
+                                                           vst, d_mask or None, npx, int(sync)):
             self._fail("bsb_composite_sources_nv12_device")
 
     def synchronize(self):

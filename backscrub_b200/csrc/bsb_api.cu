@@ -136,15 +136,32 @@ bsb::Call frames_of(bsb::Call c, int b0, int n) {
   return c;
 }
 
-// the requested outputs of call `d` (on the context staging: packed, `orow`-byte BGR rows) back into the host buffers of
-// call `h` (BGR rows `out_pitch` bytes apart, the video and mask frames packed)
-cudaError_t copy_out(const bsb::Call& h, size_t out_pitch, const bsb::Call& d, size_t orow, cudaStream_t s) {
+// the requested outputs of call `d` (on the context staging: packed, `orow`-byte BGR rows, `orows` rows, `vbytes`-byte
+// video frames) back into the host buffers of call `h` (BGR rows `out_pitch` bytes apart, the video and mask frames packed)
+cudaError_t copy_out(const bsb::Call& h, size_t out_pitch, const bsb::Call& d, size_t orow, size_t orows, size_t vbytes, cudaStream_t s) {
   const cudaMemcpyKind k = cudaMemcpyDeviceToHost;
   cudaError_t r = cudaSuccess;
-  if (h.out) r = copy_frames(h.out, out_pitch, h.out_stride, d.out, orow, d.out_stride, orow, d.out_stride / orow, h.n, k, s);
-  if (h.video && r == cudaSuccess) r = copy_frames(h.video, d.video_stride, h.video_stride, d.video, d.video_stride, d.video_stride, d.video_stride, 1, h.n, k, s);
+  if (h.out) r = copy_frames(h.out, out_pitch, h.out_stride, d.out, orow, d.out_stride, orow, orows, h.n, k, s);
+  if (h.video && r == cudaSuccess) r = copy_frames(h.video, vbytes, h.video_stride, d.video, vbytes, d.video_stride, vbytes, 1, h.n, k, s);
   if (h.mask && r == cudaSuccess) r = copy_frames(h.mask, d.mask_stride, h.mask_stride, d.mask, d.mask_stride, d.mask_stride, d.mask_stride, 1, h.n, k, s);
   return r;
+}
+
+// a sources call some of whose frames have their own output size (bsb_set_source_output): each frame's composite and
+// video output back at its own size, packed
+cudaError_t copy_out_sized(const bsb::Call& h, const bsb::Call& d, const Engine* e, bool nv12, cudaStream_t s) {
+  const cudaMemcpyKind k = cudaMemcpyDeviceToHost;
+  for (int b = 0; b < h.n; ++b) {
+    int w = 0, hh = 0;
+    e->source_output_size(h.ids[b], &w, &hh);
+    const size_t px = (size_t)w * hh;
+    cudaError_t r = cudaSuccess;
+    if (h.out) r = cudaMemcpyAsync(h.out + b * h.out_stride, d.out + b * d.out_stride, px * 3, k, s);
+    if (h.video && r == cudaSuccess) r = cudaMemcpyAsync(h.video + b * h.video_stride, d.video + b * d.video_stride, nv12 ? px * 3 / 2 : px * 2, k, s);
+    if (h.mask && r == cudaSuccess) r = cudaMemcpyAsync(h.mask + b * h.mask_stride, d.mask + b * d.mask_stride, d.mask_stride, k, s);
+    if (r != cudaSuccess) return r;
+  }
+  return cudaSuccess;
 }
 
 // Every host-buffer composite call.  `h` describes the caller's host buffers: every row is packed except BGR input rows
@@ -157,7 +174,20 @@ int host_call(bsb_ctx* ctx, const bsb::Call& h, const char* what, const size_t* 
   const bsb::Callbacks* cbp = &ctx->cb;
   Engine* e = ctx->eng;
   const bool bgr = h.fmt == bsb::IN_BGR, nv12 = h.fmt == bsb::IN_NV12;
-  const size_t W = e->W(), H = e->H(), opix = (size_t)e->out_w() * e->out_h(), orow = (size_t)e->out_w() * 3;
+  const size_t W = e->W(), H = e->H(), orow = (size_t)e->out_w() * 3, cpx = (size_t)e->out_w() * e->out_h();
+  // sources calls: the staging holds frames of the largest size any source has; `sized`: some frame's size is its own
+  bool sized = false;
+  size_t opix = cpx;
+  if (h.ids && e->n_sources()) {
+    opix = std::max(opix, (size_t)e->sources_out_px_max());
+    for (int b = 0; b < h.n && b < e->max_batch(); ++b) {
+      int w = 0, hh = 0;
+      if (!e->source_output_size(h.ids[b], &w, &hh)) continue;     // the engine reports the id
+      if (w == e->out_w() && hh == e->out_h()) continue;
+      sized = true;
+      if (h.video && !nv12 && (w & 1)) { report(cbp, "error: YUYV output needs an even width"); return 0; }
+    }
+  }
   const size_t pitch = bgr ? W * 3 : nv12 ? W : W * 2, fbytes = nv12 ? W * H * 3 / 2 : pitch * H;   // of the staged frames
   const size_t opitch = out_pitch ? *out_pitch : orow;
   if (h.n < 1 || h.n > e->max_batch()) { report(cbp, "error: n_frames out of range (1..max_batch)"); return 0; }
@@ -167,6 +197,7 @@ int host_call(bsb_ctx* ctx, const bsb::Call& h, const char* what, const size_t* 
   if (h.video && !nv12 && (e->out_w() & 1)) { report(cbp, "error: YUYV output needs an even width"); return 0; }
   API_CUDA(cudaSetDevice(e->device()));
   std::string err;
+  if (sized && !e->check_source_outputs(h, &err)) { report(cbp, std::string("error: ") + what + err); return 0; }
   uint8_t* stage = bgr ? e->d_frames() : e->d_yuyv_in();
   bsb::Call d = h;                                   // the same call on the context staging
   d.in = stage; d.pitch = pitch; d.uv = nv12 ? W * H : 0; d.stride = fbytes;
@@ -213,7 +244,8 @@ int host_call(bsb_ctx* ctx, const bsb::Call& h, const char* what, const size_t* 
       report(cbp, std::string("error: ") + what + err); return 0;
     }
     if (piped) { API_CUDA(cudaEventRecord(ctx->ev_done[c], s)); API_CUDA(cudaStreamWaitEvent(s_out, ctx->ev_done[c], 0)); }
-    API_CUDA(copy_out(frames_of(h, b0, nb), opitch, dc, orow, s_out));
+    if (sized) API_CUDA(copy_out_sized(h, dc, e, nv12, s_out));
+    else API_CUDA(copy_out(frames_of(h, b0, nb), opitch, dc, orow, e->out_h(), nv12 ? cpx * 3 / 2 : cpx * 2, s_out));
   }
   if (piped) API_CUDA(cudaStreamSynchronize(s_out));
   API_CUDA(cudaStreamSynchronize(s));
@@ -457,6 +489,23 @@ int bsb_set_source_flip(bsb_ctx* ctx, int source, int flip) {
   if (!check_ctx(ctx)) return 0;
   std::string err;
   if (!ctx->eng->set_source_flip(source, flip, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
+int bsb_set_source_output(bsb_ctx* ctx, int source, int out_w, int out_h) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_source_output(source, out_w, out_h, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
+int bsb_source_output_size(bsb_ctx* ctx, int source, int* out_w, int* out_h) {
+  if (!check_ctx(ctx)) return 0;
+  int w = 0, h = 0;
+  if (!ctx->eng->n_sources()) { report(&ctx->cb, "error: no sources: call bsb_set_sources first"); return 0; }
+  if (!ctx->eng->source_output_size(source, &w, &h)) { report(&ctx->cb, "error: source id out of range"); return 0; }
+  if (out_w) *out_w = w;
+  if (out_h) *out_h = h;
   return 1;
 }
 

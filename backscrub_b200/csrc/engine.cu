@@ -935,7 +935,7 @@ Engine::~Engine() {
   for (void* p : {(void*)wblob_, (void*)arena_, (void*)lut_, (void*)rowsum_, (void*)in_u8_, (void*)filt_u8_, (void*)state_, (void*)ofinal_,
                   (void*)d_frames_, (void*)d_out_, (void*)d_yuyv_, (void*)d_mask_, (void*)d_bg_, (void*)d_bg_raw_, (void*)d_yuyv_in_,
                   tab_in_.blob, tab_up_.blob, tab_bg_.blob, tab_out_.blob, (void*)d_bg_cursor_, (void*)d_bg_eff_, (void*)d_bg_frames_,
-                  (void*)d_gauss_tmp_, (void*)d_stage_a_, (void*)d_stage_b_, (void*)d_stage_c_, (void*)d_bg_yuyv_, (void*)pool_counters_, (void*)d_tile_geo_,
+                  (void*)d_gauss_tmp_, (void*)d_stage_a_, (void*)d_bg_yuyv_, (void*)pool_counters_, (void*)d_tile_geo_,
                   (void*)d_bg_nv12_, (void*)d_nv12_})
     if (p) cudaFree(p);
   for (ChainPlan& cp : chains_) if (cp.d_ops) cudaFree(cp.d_ops);
@@ -1212,7 +1212,7 @@ PostArgs Engine::post_args(const Call& c, const Plan& p) const {
   if (!tail) {
     a.out = c.out; a.out_stride = c.out_stride;
     uint8_t* video = p.nv12_staged ? d_yuyv_ : c.video;
-    const size_t vstride = p.nv12_staged ? (size_t)out_w_ * out_h_ * 2 : c.video_stride;
+    const size_t vstride = p.nv12_staged ? (size_t)W_ * H_ * 2 : c.video_stride;
     if (nv12_in) { a.nv12 = video; a.nv12_stride = vstride; }
     else { a.yuyv = video; a.yuyv_stride = vstride; }
     // sources calls with flipped frames and no tail: k_post_tma writes the frames of the table's flip row mirrored.
@@ -1229,10 +1229,8 @@ PostArgs Engine::post_args(const Call& c, const Plan& p) const {
 
 bool Engine::enqueue_post(const Call& c, const Plan& p) {
   const int n = c.n;
-  const size_t fbytes = (size_t)W_ * H_ * 3, opix = (size_t)out_w_ * out_h_;
-  const bool resized = out_w_ != W_ || out_h_ != H_, tail = call_tail(p);
-  // plain calls flip by the context; sources calls by frame, from the table's flip row
-  const bool flip = p.mode == CALL_PLAIN ? (flip_h_ || flip_v_) : p.flip_tail;
+  const size_t fbytes = (size_t)W_ * H_ * 3;
+  const bool tail = call_tail(p);
   const bool want_rgb = c.out || c.video;
   const bool ring = p.mode == CALL_PLAIN && has_bg_ && bg_count_ > 1;
   const PostArgs a = post_args(c, p);
@@ -1254,24 +1252,20 @@ bool Engine::enqueue_post(const Call& c, const Plan& p) {
   if (!launch_post(stream_, a)) return false;
   if (ring && bg_advance_) launch_advance_cursor(stream_, d_bg_cursor_, (int)(((long)n * bg_advance_) % bg_count_), bg_count_);
   if (!tail || !want_rgb) return true;
-  // app/deepseg.cc:667-679: flip, then scale to the virtual-camera geometry, then YUYV (:681)
-  const size_t obytes = opix * 3;
-  const uint8_t* cur = d_stage_a_; size_t cur_stride = fbytes;
-  if (flip) {
-    uint8_t* dst = (!resized && c.out) ? c.out : d_stage_b_;
-    const size_t ds = (!resized && c.out) ? c.out_stride : fbytes;
-    if (p.mode == CALL_PLAIN) launch_flip_u8c3(stream_, n, cur, cur_stride, dst, ds, W_, H_, flip_h_, flip_v_);
-    else launch_flip_u8c3_frames(stream_, n, cur, cur_stride, dst, ds, W_, H_, d_src_tab_ + 3 * (size_t)max_batch_);
-    cur = dst; cur_stride = ds;
+  // app/deepseg.cc:667-681: flip, then scale to the virtual-camera geometry, then YUYV (NV12 for NV12 calls).  Plain calls
+  // by the context's flip and size; sources calls by frame, from the table's flip and geometry rows.
+  TailArgs t{};
+  t.n = n; t.W = W_; t.H = H_; t.src = d_stage_a_; t.src_stride = fbytes;
+  t.out = c.out; t.out_stride = c.out_stride; t.video = c.video; t.video_stride = c.video_stride;
+  t.nv12 = c.fmt == IN_NV12 && c.video;     // 2x2 blocks only where an NV12 output (even sizes) is written
+  long max_px = (long)out_w_ * out_h_;
+  if (p.mode == CALL_PLAIN) {
+    t.geo = ctx_geo(); t.flip = (flip_h_ ? 1 : 0) | (flip_v_ ? 2 : 0);
+  } else {
+    t.slot = d_src_tab_ + 4 * (size_t)max_batch_; t.geos = d_geo_; t.flips = d_src_tab_ + 3 * (size_t)max_batch_;
+    max_px = sources_out_px_max();
   }
-  if (resized) {
-    uint8_t* dst = c.out ? c.out : d_stage_c_;
-    const size_t ds = c.out ? c.out_stride : obytes;
-    launch_resize_u8c3(stream_, cur, W_, H_, (size_t)W_ * 3, dst, out_w_, out_h_, (size_t)out_w_ * 3, tab_out_.tab, tab_out_.area2x2, n, cur_stride, ds);
-    cur = dst; cur_stride = ds;
-  }
-  if (p.nv12_staged) launch_rgb_to_yuyv(stream_, cur, d_yuyv_, opix, n, cur_stride, opix * 2);
-  else if (c.video) launch_rgb_to_yuyv(stream_, cur, c.video, opix, n, cur_stride, c.video_stride);
+  launch_tail(stream_, t, max_px);
   return true;
 }
 
@@ -1292,29 +1286,26 @@ bool Engine::yuyv_native(const Call& c, Plan p) const {
 // so a replay costs no host work.
 bool Engine::plan_launch(const Call& c, Plan* p, std::string* err) {
   // NV12 output: the post kernel writes it when it reads the NV12 frames in place and no tail follows (a sources call
-  // mirrored in place included); otherwise the YUYV output goes to the context staging and k_yuyv_to_nv12 derives the
-  // NV12 from it (the definition)
+  // mirrored in place included), k_tail when a tail follows; otherwise the YUYV output goes to the context staging and
+  // k_yuyv_to_nv12 derives the NV12 from it (the definition)
   auto decide = [&] {
     p->native = yuyv_native(c, *p);
-    p->nv12_staged = c.fmt == IN_NV12 && c.video && !(p->native && !call_tail(*p));
+    p->nv12_staged = c.fmt == IN_NV12 && c.video && !p->native && !call_tail(*p);
   };
-  // Sources calls with flipped frames (app/deepseg.cc:667-681 flips before the resize): without a resize, and where
-  // k_post_tma takes the call, it writes them mirrored in place; otherwise the tail flips them (and copies the others)
-  // between the post kernel and the resize.
+  // Sources calls with flipped frames (app/deepseg.cc:667-681 flips before the resize): when every frame is W x H, and
+  // where k_post_tma takes the call, it writes them mirrored in place; otherwise the tail flips them.
   p->flip_tail = false;
   if (p->mode != CALL_PLAIN && p->flipped) {
-    bool in_place = out_w_ == W_ && out_h_ == H_ && tuning().post_tma;
+    bool in_place = !p->resized && tuning().post_tma;
     if (in_place) {
       decide();
       in_place = post_tma_eligible(post_args(c, *p));
     }
     p->flip_tail = !in_place;
-    // set_output allocates the staging for a context flip / resize only; grown once (dropping the graphs) on first need
-    const size_t fbytes = (size_t)max_batch_ * W_ * H_ * 3;
-    if (p->flip_tail && (c.out || c.video) &&
-        !(ensure((void**)&d_stage_a_, &stage_a_cap_, fbytes, err) && ensure((void**)&d_stage_b_, &stage_b_cap_, fbytes, err)))
-      return false;
   }
+  // set_output allocates the staging for a context flip / resize; grown once (dropping the graphs) on first other need
+  if (call_tail(*p) && (c.out || c.video) && !ensure((void**)&d_stage_a_, &stage_a_cap_, (size_t)max_batch_ * W_ * H_ * 3, err))
+    return false;
   decide();
   return true;
 }
@@ -1331,8 +1322,7 @@ bool Engine::enqueue_all(const Call& c, const Plan& p) {
   enqueue_decision(n, p.mode != CALL_PLAIN);
   if (c.callbacks && cb_.onmask) { cudaStreamSynchronize(stream_); cb_.onmask(cb_.caller_ctx); }
   if (!enqueue_post(c, p)) return false;
-  const size_t opix = (size_t)out_w_ * out_h_;
-  if (p.nv12_staged) launch_yuyv_to_nv12(stream_, n, d_yuyv_, opix * 2, c.video, c.video_stride, out_w_, out_h_);
+  if (p.nv12_staged) launch_yuyv_to_nv12(stream_, n, d_yuyv_, (size_t)W_ * H_ * 2, c.video, c.video_stride, W_, H_);
   last_call_launches_ = (int)(thread_launch_count() - l0);
   return true;
 }
@@ -1354,8 +1344,8 @@ bool Engine::run(const Call& c, std::string* err) {
   if (c.ids) {
     if (has_bg_ && bg_count_ > 1) { *err = "sources calls need a still context background (animate a source with bsb_set_source_background)"; return false; }
     // frame b: state of source ids[b]; background (source_bg) = the context slot, the source's slot, or its camera frame
-    // blurred at the source's strength into camera-blur slot b; flip = the source's own, else the context's
-    tab.assign(4 * (size_t)max_batch_, 0);
+    // blurred at the source's strength into camera-blur slot b; flip and geometry = the source's own, else the context's
+    tab.assign(5 * (size_t)max_batch_, 0);
     int n_blur = 0;
     const int ctx_flip = (flip_h_ ? 1 : 0) | (flip_v_ ? 2 : 0);
     for (int b = 0; b < n; ++b) {
@@ -1373,7 +1363,12 @@ bool Engine::run(const Call& c, std::string* err) {
       const int fl = src_flip_[id] < 0 ? ctx_flip : src_flip_[id];
       tab[3 * (size_t)max_batch_ + b] = fl;
       p.flipped = p.flipped || fl != 0;
+      const int sz = src_size_[id];
+      tab[4 * (size_t)max_batch_ + b] = sz + 1;
+      const int ow = sz < 0 ? out_w_ : own_sizes_[sz].w, oh = sz < 0 ? out_h_ : own_sizes_[sz].h;
+      p.resized = p.resized || ow != W_ || oh != H_;
     }
+    if (!check_source_outputs(c, err)) return false;
     p.mode = p.gclass ? CALL_SOURCES_CAMBLUR : CALL_SOURCES;
     p.all_blur = n_blur == n;
   }
@@ -1398,7 +1393,7 @@ bool Engine::run(const Call& c, std::string* err) {
     return true;
   }
 #ifndef BSB_EMU
-  const GraphKey key(c, p);
+  const GraphKey key(c, p, c.ids ? sources_out_px_max() : 0);
   auto it = graphs_.find(key);
   if (it == graphs_.end()) {
     if (graphs_.size() >= 64) drop_graphs();
@@ -1435,7 +1430,8 @@ bool Engine::run(const Call& c, std::string* err) {
 }
 
 uint8_t* Engine::nv12_staging(std::string* err) {
-  if (!ensure((void**)&d_nv12_, &nv12_cap_, (size_t)max_batch_ * out_w_ * out_h_ * 3 / 2, err)) return nullptr;
+  const long px = std::max((long)out_w_ * out_h_, n_sources_ ? sources_out_px_max() : 0L);
+  if (!ensure((void**)&d_nv12_, &nv12_cap_, (size_t)max_batch_ * px * 3 / 2, err)) return nullptr;
   return d_nv12_;
 }
 
@@ -1570,16 +1566,14 @@ bool Engine::set_output(bool flip_h, bool flip_v, int out_w, int out_h, std::str
   const size_t B = (size_t)max_batch_, fbytes = (size_t)W_ * H_ * 3, obytes = (size_t)out_w * out_h * 3;
   const bool flip = flip_h || flip_v, resized = out_w != W_ || out_h != H_;
   if (flip || resized) { if (!ensure((void**)&d_stage_a_, &stage_a_cap_, B * fbytes, err)) return false; }
-  if (flip) { if (!ensure((void**)&d_stage_b_, &stage_b_cap_, B * fbytes, err)) return false; }
   if (resized) {
-    if (!ensure((void**)&d_stage_c_, &stage_c_cap_, B * obytes, err)) return false;
     if (!upload_resize_tab(build_resize_tab(W_, H_, out_w, out_h), &tab_out_, err)) return false;
     // host-buffer API staging must hold the larger of the two geometries
     if (!ensure((void**)&d_out_, &out_cap_, B * std::max(fbytes, obytes), err)) return false;
     if (!ensure((void**)&d_yuyv_, &yuyv_cap_, B * std::max(fbytes, obytes) / 3 * 2, err)) return false;
   }
   flip_h_ = flip_h; flip_v_ = flip_v; out_w_ = out_w; out_h_ = out_h;
-  return true;
+  return !d_geo_ || upload_geo(0, ctx_geo(), err);
 }
 
 bool Engine::sync(std::string* err) {
@@ -1606,6 +1600,11 @@ void Engine::free_sources() {
   src_has_bg_.clear();
   src_fx_.clear();
   src_flip_.clear();
+  src_size_.clear();
+  for (OwnSize& o : own_sizes_) if (o.tab.blob) cudaFree(o.tab.blob);
+  own_sizes_.clear();
+  if (d_geo_) cudaFree(d_geo_);
+  d_geo_ = nullptr;
 }
 
 bool Engine::set_sources(int n_sources, std::string* err) {
@@ -1617,8 +1616,8 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   const size_t fbytes = (size_t)W_ * H_ * 3, npix = (size_t)W_ * H_, opx = (size_t)oh_ * ow_;
   const size_t slots = (size_t)max_batch_ + 1 + (size_t)n_sources;
   if (!d_src_tab_) {
-    CUDA_OK(cudaMalloc((void**)&d_src_tab_, 4 * (size_t)max_batch_ * sizeof(int)));
-    CUDA_OK(cudaMemset(d_src_tab_, 0, 4 * (size_t)max_batch_ * sizeof(int)));
+    CUDA_OK(cudaMalloc((void**)&d_src_tab_, 5 * (size_t)max_batch_ * sizeof(int)));
+    CUDA_OK(cudaMemset(d_src_tab_, 0, 5 * (size_t)max_batch_ * sizeof(int)));
   }
   CUDA_OK(cudaMalloc((void**)&src_state_, (size_t)n_sources * opx));
   CUDA_OK(cudaMemset(src_state_, 0, (size_t)n_sources * opx));
@@ -1643,6 +1642,9 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   src_has_bg_.assign((size_t)n_sources, 0);
   src_fx_.assign((size_t)n_sources, SrcEffect{});
   src_flip_.assign((size_t)n_sources, -1);
+  src_size_.assign((size_t)n_sources, -1);
+  CUDA_OK(cudaMalloc((void**)&d_geo_, (1 + (size_t)n_sources) * sizeof(TailGeo)));
+  if (!upload_geo(0, ctx_geo(), err)) return false;
   if (!refresh_bank_ctx(err)) return false;
   CUDA_OK(cudaStreamSynchronize(stream_));
   return true;
@@ -1741,6 +1743,92 @@ bool Engine::set_source_flip(int source, int flip, std::string* err) {
   if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
   if (flip < -1 || flip > 3) { *err = "source flip must be -1 (follow the context) or 0..3 (BSB_FLIP_H | BSB_FLIP_V)"; return false; }
   src_flip_[source] = (signed char)flip;
+  return true;
+}
+
+TailGeo Engine::ctx_geo() const {
+  return TailGeo{out_w_, out_h_, tab_out_.tab, tab_out_.area2x2 ? 1 : 0};
+}
+
+// after a synchronisation, or into a slot no queued call reads
+bool Engine::upload_geo(int slot, const TailGeo& g, std::string* err) {
+  CUDA_OK(cudaMemcpy(d_geo_ + slot, &g, sizeof(TailGeo), cudaMemcpyHostToDevice));
+  return true;
+}
+
+bool Engine::source_output_size(int s, int* out_w, int* out_h) const {
+  if (s < 0 || s >= n_sources_) return false;
+  const int i = src_size_[s];
+  *out_w = i < 0 ? out_w_ : own_sizes_[i].w;
+  *out_h = i < 0 ? out_h_ : own_sizes_[i].h;
+  return true;
+}
+
+long Engine::sources_out_px_max() const {
+  int own_refs = 0;
+  long px = 0;
+  for (const OwnSize& o : own_sizes_)
+    if (o.refs) { own_refs += o.refs; px = std::max(px, (long)o.w * o.h); }
+  if (own_refs < n_sources_) px = std::max(px, (long)out_w_ * out_h_);
+  return px;
+}
+
+bool Engine::check_source_outputs(const Call& c, std::string* err) const {
+  for (int b = 0; b < c.n; ++b) {
+    const int id = c.ids[b];
+    if (id < 0 || id >= n_sources_) continue;                   // run() reports the id
+    const int i = src_size_[id];
+    if (i < 0) continue;                                        // at the context size: checked as a plain call's frames
+    const size_t w = (size_t)own_sizes_[i].w, h = (size_t)own_sizes_[i].h;
+    if (c.out && w * h * 3 > c.out_stride) { *err = "a source's output frame does not fit in the output stride"; return false; }
+    if (!c.video) continue;
+    if (c.fmt == IN_NV12 && ((w & 1) || (h & 1))) { *err = "NV12 output needs an even output width and height"; return false; }
+    if ((c.fmt == IN_NV12 ? w * h * 3 / 2 : w * h / 2 * 4) > c.video_stride) {
+      *err = "a source's video frame does not fit in the video stride"; return false;
+    }
+  }
+  return true;
+}
+
+bool Engine::set_source_output(int source, int out_w, int out_h, std::string* err) {
+  if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
+  if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
+  const bool follow = out_w <= 0 && out_h <= 0;
+  if (!follow && (out_w < 1 || out_h < 1 || out_w > 16384 || out_h > 16384)) {
+    *err = "source output size out of range (both <= 0 to follow the context, else 1..16384)"; return false;
+  }
+  CUDA_OK(cudaSetDevice(device_));
+  // the old size is released first, so at most n_sources sizes are ever in use (d_geo_ has a slot for each)
+  const int old = src_size_[source];
+  if (old >= 0 && !follow && own_sizes_[old].w == out_w && own_sizes_[old].h == out_h) return true;
+  if (old >= 0) --own_sizes_[old].refs;
+  src_size_[source] = -1;
+  int idx = -1;
+  if (!follow) {
+    for (size_t i = 0; i < own_sizes_.size() && idx < 0; ++i)
+      if (own_sizes_[i].refs && own_sizes_[i].w == out_w && own_sizes_[i].h == out_h) idx = (int)i;
+    if (idx < 0) {
+      // a new size: a free slot (a queued call may still read its old tables, so wait for it) or a new one
+      for (size_t i = 0; i < own_sizes_.size() && idx < 0; ++i)
+        if (!own_sizes_[i].refs) idx = (int)i;
+      if (idx >= 0) CUDA_OK(cudaStreamSynchronize(stream_));
+      else { idx = (int)own_sizes_.size(); own_sizes_.emplace_back(); }
+      OwnSize& o = own_sizes_[idx];
+      o.w = out_w; o.h = out_h;
+      TailGeo g{out_w, out_h, ResizeTab{}, 0};
+      if (out_w != W_ || out_h != H_) {
+        if (!upload_resize_tab(build_resize_tab(W_, H_, out_w, out_h), &o.tab, err)) return false;
+        g.tab = o.tab.tab; g.area2x2 = o.tab.area2x2 ? 1 : 0;
+      }
+      if (!upload_geo(1 + idx, g, err)) return false;
+    }
+    ++own_sizes_[idx].refs;
+  }
+  src_size_[source] = idx;
+  // host-buffer API staging holds max_batch frames of the largest size (grown: synchronises and drops the graphs)
+  const size_t B = (size_t)max_batch_, px = (size_t)std::max(sources_out_px_max(), (long)W_ * H_);
+  if (!ensure((void**)&d_out_, &out_cap_, B * px * 3, err)) return false;
+  if (!ensure((void**)&d_yuyv_, &yuyv_cap_, B * px * 2, err)) return false;
   return true;
 }
 

@@ -80,7 +80,7 @@ struct Call {
   const uint8_t* in = nullptr;
   size_t pitch = 0, uv = 0, stride = 0;   // row pitch, NV12's UV plane offset inside a frame (else 0), frame stride
   const int* ids = nullptr;          // HOST array: frame b belongs to source ids[b] (n distinct ids); null: a plain call
-  uint8_t* out = nullptr; size_t out_stride = 0;       // BGR composite, out_w x out_h, rows out_w*3 bytes
+  uint8_t* out = nullptr; size_t out_stride = 0;       // BGR composite, out_w x out_h (sources: the frame's own), rows out_w*3 bytes
   uint8_t* video = nullptr; size_t video_stride = 0;   // tightly packed YUYV, or NV12 when the input is NV12
   uint8_t* mask = nullptr; size_t mask_stride = 0;     // W x H
   bool callbacks = false;            // fire the stage callbacks (the call then runs eagerly, synchronised at each stage)
@@ -126,6 +126,14 @@ class Engine {
   // mirroring of one source: -1 follows set_output's flips, 0..3 its own (bit 0 horizontal, bit 1 vertical).  Host
   // bookkeeping only: the flip reaches the device through the per-frame table of each call.
   bool set_source_flip(int source, int flip, std::string* err);
+  // virtual-camera size of one source: out_w <= 0 and out_h <= 0 follow set_output's size, else both in 1..16384
+  bool set_source_output(int source, int out_w, int out_h, std::string* err);
+  // the effective size of source s (its own, or the context's); false when s is not a source
+  bool source_output_size(int s, int* out_w, int* out_h) const;
+  // the largest effective size (w * h) among the sources, which bounds every frame of a sources call
+  long sources_out_px_max() const;
+  // the frames of sources call c with an own size: each fits its output strides, and an NV12 output is even-sized
+  bool check_source_outputs(const Call& c, std::string* err) const;
   // device staging of max_batch NV12 output frames (host-buffer API), grown on demand; nullptr on error
   uint8_t* nv12_staging(std::string* err);
   int n_sources() const { return n_sources_; }
@@ -155,8 +163,7 @@ class Engine {
     for (const Step& s : steps_) n += s.launches();
     if (bgblur_k_ && !has_bg_) n += 2;
     if (bg_count_ > 1 && bg_advance_) n += 1;
-    const bool resized = out_w_ != W_ || out_h_ != H_;
-    if (flip_h_ || flip_v_ || resized) n += (flip_h_ || flip_v_ ? 1 : 0) + (resized ? 1 : 0) + 1;   // + stand-alone YUYV
+    if (flip_h_ || flip_v_ || out_w_ != W_ || out_h_ != H_) n += 1;   // k_tail
     return n;
   }
   long get_tensor(int t, int frame, float* out, long cap, std::string* err);
@@ -190,21 +197,21 @@ class Engine {
     unsigned gclass = 0;             // sources: the Gaussian launch classes of the camera-blur frames (GAUSS_FUSED | GAUSS_SEPARABLE)
     bool all_blur = false;           // sources: every frame blurs its camera frame (the BGR frames are materialised)
     bool flipped = false;            // sources: some frame is mirrored (the table's flip row is not all 0)
-    bool flip_tail = false;          // ... and the tail mirrors them (k_flip_u8c3_frames): the call resizes or its post kernel
-                                     // is not k_post_tma
+    bool resized = false;            // sources: some frame's output size is not W x H (the table's geometry row)
+    bool flip_tail = false;          // ... and the tail mirrors them (k_tail): the call resizes or its post kernel is not k_post_tma
     bool native = false;             // the post stage reads the camera frames (YUYV or NV12) in place, no BGR frame is materialised
-    bool nv12_staged = false;        // the NV12 output is converted from a YUYV output staged in d_yuyv_ (k_yuyv_to_nv12)
+    bool nv12_staged = false;        // the NV12 output is converted from a YUYV output staged in d_yuyv_ (k_yuyv_to_nv12): an
+                                     // NV12 call whose post kernel reads BGR frames, without a tail
   };
   // flip_tail, native and nv12_staged (and the tail's staging); false with *err when a buffer cannot be grown
   bool plan_launch(const Call& c, Plan* p, std::string* err);
   void enqueue_pre(const Call& c);
   PostArgs post_args(const Call& c, const Plan& p) const;
   bool yuyv_native(const Call& c, Plan p) const;
-  // the call ends with a stand-alone tail (post -> stage -> flip -> resize -> YUYV): plain calls with a context flip or
-  // resize; sources calls with a resize, or with mirrored frames the post kernel cannot mirror in place
+  // the call ends with k_tail (post -> stage -> flip, resize, YUYV / NV12): plain calls with a context flip or resize;
+  // sources calls with a frame not at W x H, or with mirrored frames the post kernel cannot mirror in place
   bool call_tail(const Plan& p) const {
-    const bool resized = out_w_ != W_ || out_h_ != H_;
-    return p.mode == CALL_PLAIN ? (flip_h_ || flip_v_ || resized) : (resized || p.flip_tail);
+    return p.mode == CALL_PLAIN ? (flip_h_ || flip_v_ || out_w_ != W_ || out_h_ != H_) : (p.resized || p.flip_tail);
   }
   // false (nothing more enqueued) only when the post kernel cannot write a call's mirrored frames
   bool enqueue_all(const Call& c, const Plan& p);
@@ -303,7 +310,7 @@ class Engine {
   size_t bg_eff_cap_ = 0, bg_frames_cap_ = 0, gauss_tmp_cap_ = 0;
   bool flip_h_ = false, flip_v_ = false;
   int out_w_ = 0, out_h_ = 0;
-  uint8_t* d_stage_a_ = nullptr, *d_stage_b_ = nullptr, *d_stage_c_ = nullptr;
+  uint8_t* d_stage_a_ = nullptr;     // [B][H][W][3] unflipped composites that k_tail reads
   int2* d_tile_geo_ = nullptr;       // k_post_tma patch geometry per tile row | per 64-wide tile column | per 128-wide tile column
   int geo_nty_ = 0, geo_ntx64_ = 0;
   uint8_t* d_bg_yuyv_ = nullptr;     // YUYV of the effective background (ring): all-background tiles are copies
@@ -316,14 +323,23 @@ class Engine {
   uint8_t* d_nv12_ = nullptr;        // host-buffer API staging of the NV12 output
   size_t nv12_cap_ = 0;
   int last_call_launches_ = 0;
-  size_t stage_a_cap_ = 0, stage_b_cap_ = 0, stage_c_cap_ = 0, out_cap_ = 0, yuyv_cap_ = 0;
+  size_t stage_a_cap_ = 0, out_cap_ = 0, yuyv_cap_ = 0;
 
   // ---- independent sources (calls with ids) ----
   int n_sources_ = 0;
   uint8_t* src_state_ = nullptr;     // [n_sources][oh*ow] smoother state per source
-  // [4][max_batch]: source id of frame b | background-bank slot of frame b | camera-blur strength of frame b (0 = none) |
-  // flip code of frame b (bit 0 horizontal, bit 1 vertical; the source's own, or the context's), written before each launch
+  // [5][max_batch]: source id of frame b | background-bank slot of frame b | camera-blur strength of frame b (0 = none) |
+  // flip code of frame b (bit 0 horizontal, bit 1 vertical; the source's own, or the context's) | geometry slot of frame b
+  // (d_geo_ index), written before each launch
   int* d_src_tab_ = nullptr;
+  // Output geometries k_tail reads, [1 + n_sources]: slot 0 the context's (set_output), slot 1 + i own size i.  Each own
+  // size is kept once, however many sources use it; a slot no source uses any more is reused by the next new size.
+  TailGeo* d_geo_ = nullptr;
+  struct OwnSize { int w = 0, h = 0, refs = 0; DevResizeTab tab; };
+  std::vector<OwnSize> own_sizes_;
+  std::vector<int> src_size_;        // per source: -1 = the context's size, else an index into own_sizes_
+  TailGeo ctx_geo() const;
+  bool upload_geo(int slot, const TailGeo& g, std::string* err);
   // background bank, one base + one stride for the post kernel: [max_batch] camera-blur slots | [1] the context's effective
   // background | [n_sources] source slots; d_bank_yuyv_ is its YUYV and d_bank_nv12_ its NV12 (the camera-blur slots'
   // are written by the Gaussian of the call, in the call's video format)
@@ -352,16 +368,20 @@ class Engine {
   // Everything a captured launch sequence bakes into its kernel arguments: the call's buffers and layouts (the stride of
   // an absent output does not matter), and the plan's mode (a plain and a sources graph over the same buffers are
   // different graphs), Gaussian classes (strengths within them replay), all-blur and flipped (which frames flip is table
-  // data).  The rest of the plan is decided from these.
+  // data), resized and the largest output size of the sources, which the tail's grid covers (which frame has which size
+  // is table data too).  The rest of the plan is decided from these.
   struct GraphKey {
     int n, fmt; const void* in; size_t pitch, uv, stride;
     const void* out; const void* video; const void* mask; size_t ostride, vstride, mstride;
-    int mode; unsigned gclass; bool all_blur, flipped;
-    GraphKey(const Call& c, const Plan& p)
+    int mode; unsigned gclass; bool all_blur, flipped, resized; long out_px_max;
+    GraphKey(const Call& c, const Plan& p, long px_max)
         : n(c.n), fmt(c.fmt), in(c.in), pitch(c.pitch), uv(c.uv), stride(c.stride), out(c.out), video(c.video), mask(c.mask),
           ostride(c.out ? c.out_stride : 0), vstride(c.video ? c.video_stride : 0), mstride(c.mask ? c.mask_stride : 0),
-          mode(p.mode), gclass(p.gclass), all_blur(p.all_blur), flipped(p.flipped) {}
-    auto tie() const { return std::tie(n, fmt, in, pitch, uv, stride, out, video, mask, ostride, vstride, mstride, mode, gclass, all_blur, flipped); }
+          mode(p.mode), gclass(p.gclass), all_blur(p.all_blur), flipped(p.flipped), resized(p.resized), out_px_max(px_max) {}
+    auto tie() const {
+      return std::tie(n, fmt, in, pitch, uv, stride, out, video, mask, ostride, vstride, mstride, mode, gclass, all_blur, flipped, resized,
+                      out_px_max);
+    }
     bool operator<(const GraphKey& r) const { return tie() < r.tie(); }
   };
 #ifndef BSB_EMU

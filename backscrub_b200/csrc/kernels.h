@@ -288,8 +288,23 @@ bool launch_gauss_frames(cudaStream_t s, int n, const GaussSrc& cam, const int* 
                          uint8_t* dst, uint8_t* dst_yuyv, uint8_t* dst_nv12, int W, int H);
 // app/deepseg.cc:667-673: cv::flip on n packed frames
 void launch_flip_u8c3(cudaStream_t s, int n, const uint8_t* src, size_t sstride, uint8_t* dst, size_t dstride, int W, int H, bool flip_h, bool flip_v);
-// the same per frame: frame b flipped by flip[b] (DEVICE [n]; bit 0 horizontally, bit 1 vertically), copied when it is 0
-void launch_flip_u8c3_frames(cudaStream_t s, int n, const uint8_t* src, size_t sstride, uint8_t* dst, size_t dstride, int W, int H, const int* flip);
+// app/deepseg.cc:667-681 in one launch, the tail of a call whose frames are mirrored or resized outside the post kernel:
+// cv::flip, then cv::resize to the frame's virtual-camera geometry, then the YUYV (or NV12) conversion, from the staged
+// W x H BGR composites.  The flip mirrors each tap's source coordinate and keeps the weights; ow == W and oh == H is a
+// mirrored copy.  Bit-exact against the chain k_flip_u8c3 -> k_resize_u8c3 -> k_rgb_to_yuyv (-> k_yuyv_to_nv12).
+struct TailGeo { int ow, oh; ResizeTab tab; int area2x2; };   // tab: INTER_LINEAR tables W x H -> ow x oh
+struct TailArgs {
+  int n, W, H;
+  const uint8_t* src; size_t src_stride;   // staged composites, rows W*3 bytes
+  uint8_t* out; size_t out_stride;         // may be null: BGR, tightly packed rows ow*3 bytes
+  uint8_t* video; size_t video_stride;     // may be null: tightly packed YUYV (floor(ow*oh/2) flat pixel pairs), or NV12
+  int nv12;                                //   (ow, oh even; Y plane, UV plane at byte ow*oh) when nv12 != 0
+  TailGeo geo; int flip;                   // every frame's geometry and flip code (bit 0 horizontal, bit 1 vertical) ...
+  const int* slot; const TailGeo* geos;    // ... unless set: frame b's geometry is geos[slot[b]] (DEVICE)
+  const int* flips;                        // ... and its flip code flips[b] (DEVICE)
+};
+// max_px: the largest ow * oh a frame of the call can have (the grid covers it; smaller frames' extra CTAs exit)
+void launch_tail(cudaStream_t s, const TailArgs& a, long max_px);
 
 // cv::cvtColor(COLOR_YUV2BGR_YUYV): camera YUYV frames -> BGR (what cv::VideoCapture does for the
 // reference, app/deepseg.cc:553).  n frames of W x H, tightly packed.

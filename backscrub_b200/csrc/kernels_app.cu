@@ -188,21 +188,6 @@ BSB_D void gauss_fused_bc(uint8_t* P, uint16_t* Ht, const GaussFast& g, int rows
   }
 }
 
-// convert_rgb_to_yuyv of one pixel pair (6 BGR bytes) as the word (Y0, V, Y1, U): what the post kernel produces for
-// mask 255, i.e. the cached YUYV of a background slot
-BSB_D unsigned yuyv_pair_word(const uint8_t* s) {
-  int Y0, U0, V0, Y1, U1, V1;
-  rgb2yuv(s[0], s[1], s[2], Y0, U0, V0);
-  rgb2yuv(s[3], s[4], s[5], Y1, U1, V1);
-  return (unsigned)Y0 | ((unsigned)((V0 + V1) / 2) << 8) | ((unsigned)Y1 << 16) | ((unsigned)((U0 + U1) / 2) << 24);
-}
-// the NV12 of one 2x2 block from the YUYV words of its two rows: Y copied, UV the truncating row-pair average
-BSB_D void nv12_block(unsigned w0, unsigned w1, uint8_t* y0, int W, uint8_t* uv) {
-  y0[0] = (uint8_t)w0; y0[1] = (uint8_t)(w0 >> 16); y0[W] = (uint8_t)w1; y0[W + 1] = (uint8_t)(w1 >> 16);
-  uv[0] = (uint8_t)((((w0 >> 8) & 255u) + ((w1 >> 8) & 255u)) >> 1);
-  uv[1] = (uint8_t)(((w0 >> 24) + (w1 >> 24)) >> 1);
-}
-
 // yuyv / nv12 (may be null; W even, NV12 also H even): [n] W*H*2 / W*H*3/2-byte frames that receive the blurred frame's
 // YUYV / NV12, written from the output tile in stage D
 __global__ void __launch_bounds__(256) k_gauss_fused(const uint8_t* src, size_t spitch, size_t sstride, uint8_t* dst, size_t dpitch,
@@ -461,24 +446,6 @@ void launch_flip_u8c3(cudaStream_t s, int n, const uint8_t* src, size_t sstride,
   const size_t npix = (size_t)W * H;
   BSB_LAUNCH(k_flip_u8c3, dim3((unsigned)((npix + 255) / 256), (unsigned)n), dim3(256), 0, s, src, sstride, dst, dstride, W, H,
              flip_h ? 1 : 0, flip_v ? 1 : 0);
-  count_launch();
-}
-
-// per-frame variant (sources calls): frame b flipped by flip[b], copied when 0, so the resize that follows sees every frame
-__global__ void __launch_bounds__(256) k_flip_u8c3_frames(const uint8_t* src, size_t sstride, uint8_t* dst, size_t dstride, int W, int H,
-                                                          const int* flip) {
-  const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (p >= (size_t)W * H) return;
-  const int fl = __ldg(flip + blockIdx.y);
-  const int x = (int)(p % W), y = (int)(p / W);
-  const uint8_t* sp = src + (size_t)blockIdx.y * sstride + ((size_t)((fl & 2) ? H - 1 - y : y) * W + ((fl & 1) ? W - 1 - x : x)) * 3;
-  uint8_t* dp = dst + (size_t)blockIdx.y * dstride + 3 * p;
-  dp[0] = sp[0]; dp[1] = sp[1]; dp[2] = sp[2];
-}
-
-void launch_flip_u8c3_frames(cudaStream_t s, int n, const uint8_t* src, size_t sstride, uint8_t* dst, size_t dstride, int W, int H, const int* flip) {
-  const size_t npix = (size_t)W * H;
-  BSB_LAUNCH(k_flip_u8c3_frames, dim3((unsigned)((npix + 255) / 256), (unsigned)n), dim3(256), 0, s, src, sstride, dst, dstride, W, H, flip);
   count_launch();
 }
 

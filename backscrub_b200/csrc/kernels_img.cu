@@ -766,6 +766,34 @@ bool launch_post(cudaStream_t s, const PostArgs& a_in) {
 // ---------------------------------------------------------------------------
 // cv::resize(src -> dst) 8UC3 (background provider).  One thread = one dst pixel.
 // ---------------------------------------------------------------------------
+// One output pixel (dx, dy) of cv::resize 8UC3 of the sw x sh image `src` (rows spitch bytes apart): the exact 2x
+// INTER_AREA mean (a+b+c+d+2)>>2 when area2x2, else INTER_LINEAR through the tables.  flip (bit 0 horizontally, bit 1
+// vertically) mirrors the image before the resize (app/deepseg.cc:667-679): each tap's source coordinate is mirrored and
+// its weight kept, which is not the same as mirroring the resized image (the fixed-point tables need not be symmetric).
+BSB_D void resize_px(const uint8_t* src, int sw, int sh, size_t spitch, const ResizeTab& t, bool area2x2, int flip, int dx, int dy,
+                     uint8_t* d) {
+  if (area2x2) {
+    int x0 = 2 * dx, x1 = 2 * dx + 1, y0 = 2 * dy, y1 = 2 * dy + 1;
+    if (flip & 1) { x0 = sw - 1 - x0; x1 = sw - 1 - x1; }
+    if (flip & 2) { y0 = sh - 1 - y0; y1 = sh - 1 - y1; }
+    const uint8_t* s0 = src + (size_t)y0 * spitch;
+    const uint8_t* s1 = src + (size_t)y1 * spitch;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) d[c] = (uint8_t)((s0[3 * x0 + c] + s0[3 * x1 + c] + s1[3 * x0 + c] + s1[3 * x1 + c] + 2) >> 2);
+    return;
+  }
+  int sx = __ldg(t.xofs + dx), sx1 = min(sx + 1, sw - 1);
+  int y0 = __ldg(t.yofs0 + dy), y1 = __ldg(t.yofs1 + dy);
+  if (flip & 1) { sx = sw - 1 - sx; sx1 = sw - 1 - sx1; }
+  if (flip & 2) { y0 = sh - 1 - y0; y1 = sh - 1 - y1; }
+  const int a0 = __ldg(t.xw + 2 * dx), a1 = __ldg(t.xw + 2 * dx + 1);
+  const int b0 = __ldg(t.yw + 2 * dy), b1 = __ldg(t.yw + 2 * dy + 1);
+  const uint8_t* r0 = src + (size_t)y0 * spitch;
+  const uint8_t* r1 = src + (size_t)y1 * spitch;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) d[c] = lin_v(lin_h(r0, sx, sx1, 3, c, a0, a1), lin_h(r1, sx, sx1, 3, c, a0, a1), b0, b1);
+}
+
 __global__ void __launch_bounds__(256) k_resize_u8c3(const uint8_t* src, int sw, int sh, size_t spitch,
                                                      uint8_t* dst, int dw, int dh, size_t dpitch, ResizeTab t, bool area2x2,
                                                      size_t sstride, size_t dstride) {
@@ -773,22 +801,7 @@ __global__ void __launch_bounds__(256) k_resize_u8c3(const uint8_t* src, int sw,
   if (idx >= (long)dw * dh) return;
   src += (size_t)blockIdx.y * sstride; dst += (size_t)blockIdx.y * dstride;
   const int dx = (int)(idx % dw), dy = (int)(idx / dw);
-  uint8_t* d = dst + (size_t)dy * dpitch + (size_t)dx * 3;
-  if (area2x2) {
-    const uint8_t* s0 = src + (size_t)(2 * dy) * spitch + (size_t)(2 * dx) * 3;
-    const uint8_t* s1 = s0 + spitch;
-#pragma unroll
-    for (int c = 0; c < 3; ++c) d[c] = (uint8_t)((s0[c] + s0[3 + c] + s1[c] + s1[3 + c] + 2) >> 2);
-    return;
-  }
-  const int sx = __ldg(t.xofs + dx), sx1 = min(sx + 1, sw - 1);
-  const int a0 = __ldg(t.xw + 2 * dx), a1 = __ldg(t.xw + 2 * dx + 1);
-  const int b0 = __ldg(t.yw + 2 * dy), b1 = __ldg(t.yw + 2 * dy + 1);
-  const uint8_t* r0 = src + (size_t)__ldg(t.yofs0 + dy) * spitch;
-  const uint8_t* r1 = src + (size_t)__ldg(t.yofs1 + dy) * spitch;
-#pragma unroll
-  for (int c = 0; c < 3; ++c) d[c] = lin_v(lin_h(r0, sx, sx1, 3, c, a0, a1), lin_h(r1, sx, sx1, 3, c, a0, a1), b0, b1);
-  (void)sh;
+  resize_px(src, sw, sh, spitch, t, area2x2, 0, dx, dy, dst + (size_t)dy * dpitch + (size_t)dx * 3);
 }
 
 void launch_resize_u8c3(cudaStream_t s, const uint8_t* src, int sw, int sh, size_t spitch,
@@ -874,12 +887,9 @@ __global__ void __launch_bounds__(256) k_rgb_to_yuyv(const uint8_t* rgb, uint8_t
   const size_t p = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (p >= npairs) return;
   rgb += (size_t)blockIdx.y * rgb_stride; yuyv += (size_t)blockIdx.y * yuyv_stride;
-  const uint8_t* s = rgb + 6 * p;
-  int Y0, U0, V0, Y1, U1, V1;
-  rgb2yuv(s[0], s[1], s[2], Y0, U0, V0);
-  rgb2yuv(s[3], s[4], s[5], Y1, U1, V1);
+  const unsigned w = yuyv_pair_word(rgb + 6 * p);
   uint8_t* d = yuyv + 4 * p;
-  d[0] = (uint8_t)Y0; d[1] = (uint8_t)((V0 + V1) / 2); d[2] = (uint8_t)Y1; d[3] = (uint8_t)((U0 + U1) / 2);
+  d[0] = (uint8_t)w; d[1] = (uint8_t)(w >> 8); d[2] = (uint8_t)(w >> 16); d[3] = (uint8_t)(w >> 24);
 }
 
 void launch_rgb_to_yuyv(cudaStream_t s, const uint8_t* rgb, uint8_t* yuyv, size_t npix, int n, size_t rgb_stride, size_t yuyv_stride) {
@@ -937,6 +947,75 @@ __global__ void __launch_bounds__(256) k_yuyv_to_nv12(const uint8_t* yuyv, size_
 void launch_yuyv_to_nv12(cudaStream_t s, int n, const uint8_t* yuyv, size_t yuyv_stride, uint8_t* nv12, size_t nv12_stride, int W, int H) {
   const long blocks = ((long)(W / 2) * (H / 2) + 255) / 256;
   BSB_LAUNCH(k_yuyv_to_nv12, dim3((unsigned)blocks, (unsigned)n), dim3(256), 0, s, yuyv, yuyv_stride, nv12, nv12_stride, W, H);
+  count_launch();
+}
+
+// ---------------------------------------------------------------------------
+// The call's tail (app/deepseg.cc:667-681): flip -> resize -> YUYV / NV12 of the staged composites, frames along
+// blockIdx.y.  YUYV: one thread = one flat pixel pair of the packed output (convert_rgb_to_yuyv walks total(), so with an
+// odd width a pair spans a row end; a last odd pixel has no pair).  NV12: one thread = one 2x2 block, whose two YUYV
+// words give its Y bytes and UV pair directly.
+// ---------------------------------------------------------------------------
+// pixel (x, y) of frame geometry g: the mirrored copy when g is the staged size, else the mirrored resize
+BSB_D void tail_px(const uint8_t* src, int W, int H, const TailGeo& g, int flip, int x, int y, uint8_t* d) {
+  if (g.ow == W && g.oh == H) {
+    const uint8_t* s = src + ((size_t)((flip & 2) ? H - 1 - y : y) * W + ((flip & 1) ? W - 1 - x : x)) * 3;
+    d[0] = s[0]; d[1] = s[1]; d[2] = s[2];
+  } else {
+    resize_px(src, W, H, (size_t)W * 3, g.tab, g.area2x2 != 0, flip, x, y, d);
+  }
+}
+
+__global__ void __launch_bounds__(256) k_tail(TailArgs a) {
+  const int b = blockIdx.y;
+  const TailGeo g = a.slot ? a.geos[__ldg(a.slot + b)] : a.geo;
+  const int fl = a.flips ? __ldg(a.flips + b) : a.flip;
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  const long npx = (long)g.ow * g.oh;
+  const uint8_t* src = a.src + (size_t)b * a.src_stride;
+  uint8_t* out = a.out ? a.out + (size_t)b * a.out_stride : nullptr;
+  uint8_t* vid = a.video ? a.video + (size_t)b * a.video_stride : nullptr;
+  if (a.nv12) {
+    if (i >= npx / 4) return;
+    const int hw = g.ow / 2, x = (int)(i % hw) * 2, y = (int)(i / hw) * 2;
+    uint8_t px[12];                                   // (x, y) (x+1, y) | (x, y+1) (x+1, y+1)
+    tail_px(src, a.W, a.H, g, fl, x, y, px);
+    tail_px(src, a.W, a.H, g, fl, x + 1, y, px + 3);
+    tail_px(src, a.W, a.H, g, fl, x, y + 1, px + 6);
+    tail_px(src, a.W, a.H, g, fl, x + 1, y + 1, px + 9);
+    if (out) {
+      uint8_t* o = out + ((size_t)y * g.ow + x) * 3;
+#pragma unroll
+      for (int k = 0; k < 6; ++k) { o[k] = px[k]; o[(size_t)g.ow * 3 + k] = px[6 + k]; }
+    }
+    if (vid) nv12_block(yuyv_pair_word(px), yuyv_pair_word(px + 6), vid + (size_t)y * g.ow + x, g.ow, vid + npx + (size_t)(y / 2) * g.ow + x);
+    return;
+  }
+  const long p = 2 * i;
+  if (p >= npx) return;
+  const bool pair = p + 1 < npx;
+  uint8_t px[6];
+  tail_px(src, a.W, a.H, g, fl, (int)(p % g.ow), (int)(p / g.ow), px);
+  if (pair) tail_px(src, a.W, a.H, g, fl, (int)((p + 1) % g.ow), (int)((p + 1) / g.ow), px + 3);
+  if (out) {
+    uint8_t* o = out + 3 * p;
+    o[0] = px[0]; o[1] = px[1]; o[2] = px[2];
+    if (pair) { o[3] = px[3]; o[4] = px[4]; o[5] = px[5]; }
+  }
+  if (vid && pair) {
+    const unsigned w = yuyv_pair_word(px);
+    uint8_t* v = vid + 4 * i;
+    if ((reinterpret_cast<uintptr_t>(v) & 3) == 0) {
+      *reinterpret_cast<unsigned*>(v) = w;
+    } else {
+      v[0] = (uint8_t)w; v[1] = (uint8_t)(w >> 8); v[2] = (uint8_t)(w >> 16); v[3] = (uint8_t)(w >> 24);
+    }
+  }
+}
+
+void launch_tail(cudaStream_t s, const TailArgs& a, long max_px) {
+  const long threads = (max_px + 1) / 2;
+  BSB_LAUNCH(k_tail, dim3((unsigned)((threads + 255) / 256), (unsigned)a.n), dim3(256), 0, s, a);
   count_launch();
 }
 

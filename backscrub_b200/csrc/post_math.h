@@ -88,6 +88,21 @@ BSB_D void rgb2yuv(int R, int G, int Bc, int& Y, int& U, int& V) {
   U = U < 0 ? 0 : (U > 255 ? 255 : U);
   V = V < 0 ? 0 : (V > 255 ? 255 : V);
 }
+// convert_rgb_to_yuyv of one pixel pair (two 3-byte BGR pixels) as the word (Y0, V, Y1, U) (app/deepseg.cc:87-106)
+BSB_D unsigned yuyv_pair_word(const uint8_t* p0, const uint8_t* p1) {
+  int Y0, U0, V0, Y1, U1, V1;
+  rgb2yuv(p0[0], p0[1], p0[2], Y0, U0, V0);
+  rgb2yuv(p1[0], p1[1], p1[2], Y1, U1, V1);
+  return (unsigned)Y0 | ((unsigned)((V0 + V1) / 2) << 8) | ((unsigned)Y1 << 16) | ((unsigned)((U0 + U1) / 2) << 24);
+}
+BSB_D unsigned yuyv_pair_word(const uint8_t* s) { return yuyv_pair_word(s, s + 3); }
+// the NV12 of one 2x2 block from the YUYV words of its two rows (W bytes apart in the Y plane): Y copied, UV the
+// truncating row-pair average (include/backscrub_b200.h)
+BSB_D void nv12_block(unsigned w0, unsigned w1, uint8_t* y0, int W, uint8_t* uv) {
+  y0[0] = (uint8_t)w0; y0[1] = (uint8_t)(w0 >> 16); y0[W] = (uint8_t)w1; y0[W + 1] = (uint8_t)(w1 >> 16);
+  uv[0] = (uint8_t)((((w0 >> 8) & 255u) + ((w1 >> 8) & 255u)) >> 1);
+  uv[1] = (uint8_t)(((w0 >> 24) + (w1 >> 24)) >> 1);
+}
 
 // one pixel from its Y byte and the U / V bytes it shares (the arithmetic of yuyv8_to_bgr24)
 BSB_D void yuv_px_to_bgr(int y, int u8, int v8, int* bgr) {

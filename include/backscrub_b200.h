@@ -110,7 +110,7 @@ BSB_API int bsb_set_bgblur(bsb_ctx* ctx, int ksize);
 /* `-H`/`-V` cv::flip of the composited frame (:667-673) and cv::resize to the virtual-camera geometry when it
  * differs from the capture geometry (:677-679); both before the YUYV conversion.  out_w/out_h <= 0 = frame size.
  * After this call `out` buffers are out_w x out_h x 3 and `out_yuyv` out_w x out_h x 2; the mask stays W x H.
- * The flips are the default of every source of a sources call (bsb_set_source_flip); the output size is per context. */
+ * The flips and the size are the default of every source of a sources call (bsb_set_source_flip, bsb_set_source_output). */
 BSB_API int bsb_set_output(bsb_ctx* ctx, int flip_h, int flip_v, int out_w, int out_h);
 BSB_API int bsb_output_size(bsb_ctx* ctx, int* out_w, int* out_h);
 
@@ -184,8 +184,8 @@ BSB_API int bsb_composite_nv12(bsb_ctx* ctx, int n_frames, const uint8_t* nv12, 
  * background (bsb_set_background, or the green default), blurred when bgblur is on; else, with
  * bgblur on and no background of either kind, its own blurred camera frame (app/deepseg.cc:652-658).
  * That is the default effect of every source; bsb_set_source_effect changes it per source.
- * bsb_set_output's size applies to every frame, its flips to every source without its own
- * (bsb_set_source_flip); callbacks do not fire; the context
+ * bsb_set_output's size and flips apply to every source without its own
+ * (bsb_set_source_output, bsb_set_source_flip); callbacks do not fire; the context
  * background must not be a ring of more than one image.  Plain calls never touch the per-source
  * states and sources calls never touch the plain smoother state, so both can be mixed on one
  * context.  A violated rule returns 0 with a bsb_last_error() message and leaves the context usable. */
@@ -206,8 +206,7 @@ BSB_API int bsb_set_source_background(bsb_ctx* ctx, int source, const uint8_t* b
  *                                     the strength is > 0, else plain green (the source's own image is kept,
  *                                     unused, until DEFAULT again).
  * bgblur:     -1 = follow the context (bsb_set_bgblur, including later changes), 0 = off, odd 1..255.
- * bsb_set_sources resets every source to (DEFAULT, -1).  The output size of bsb_set_output and the camera-blur mode
- * of plain calls stay per context.  An unknown background, an even / out-of-range strength, a source id out of range or no
+ * bsb_set_sources resets every source to (DEFAULT, -1).  The camera-blur mode of plain calls stays per context.  An unknown background, an even / out-of-range strength, a source id out of range or no
  * bsb_set_sources yet return 0 with a bsb_last_error() message.
  * Cost: bsb_set_background and bsb_set_bgblur refresh the still background of every source except one with its own
  * image at a fixed strength (a Gaussian for each such source with a strength > 0; nothing is cached by strength). */
@@ -219,11 +218,26 @@ BSB_API int bsb_set_source_effect(bsb_ctx* ctx, int source, int background, int 
  * NV12 output and mask of a plain context set up the same way plus bsb_set_output(flip_h_s, flip_v_s, out_w, out_h).
  * The mask is never flipped.  bsb_set_sources resets every source to -1.  Host bookkeeping only (no device work, no
  * synchronisation), so it may be called per frame; the flips reach the device with the call's source table.  Without a
- * resize, where the TMA post kernel takes the geometry, it writes the mirrored frames in place; otherwise they are
- * flipped between the post kernel and the resize.  A flip outside -1..3, a source id out of range or no
+ * resize in the call, where the TMA post kernel takes the geometry, it writes the mirrored frames in place; otherwise one
+ * tail kernel flips, resizes and converts the staged frames.  A flip outside -1..3, a source id out of range or no
  * bsb_set_sources yet return 0 with a bsb_last_error() message. */
 enum { BSB_FLIP_H = 1, BSB_FLIP_V = 2 };
 BSB_API int bsb_set_source_flip(bsb_ctx* ctx, int source, int flip);
+/* Virtual-camera size of one source (cv::resize after the flip, before the YUYV / NV12 conversion, app/deepseg.cc:667-681).
+ * out_w <= 0 and out_h <= 0: follow bsb_set_output's size, including later changes; otherwise both in 1..16384.
+ * Frame b of a sources call, from source s, gives exactly the composite, YUYV / NV12 output and mask of a plain context
+ * set up the same way plus bsb_set_output(flip_h_s, flip_v_s, out_w_s, out_h_s).  The mask stays W x H.
+ * Output layout of a sources call: frame b's composite is tightly packed at its own size (rows out_w_b*3 bytes) at
+ * out + b*out_stride, its YUYV / NV12 tightly packed at video + b*video_stride; the strides must hold the largest frame of
+ * the call.  A call refuses, before any launch, a frame of its own size whose bytes do not fit its stride, an NV12 output
+ * for a frame of odd own width or height, and (host buffers) a YUYV output for a frame of odd own width.
+ * bsb_set_sources resets every source to follow.  No bsb_set_sources yet, a source id out of range or a size out of range
+ * or half given return 0 with a bsb_last_error() message.  Each distinct size keeps one set of resize tables on the
+ * device; replacing tables a queued call may read waits for the context's stream, and the host-buffer staging grows to
+ * the largest size (dropping the captured graphs) when a size exceeds it. */
+BSB_API int bsb_set_source_output(bsb_ctx* ctx, int source, int out_w, int out_h);
+/* the effective size of one source (its own, or the context's) */
+BSB_API int bsb_source_output_size(bsb_ctx* ctx, int source, int* out_w, int* out_h);
 /* HOST buffers, BGR frames, laid out as in bsb_composite (out rows tightly packed, `out_stride` bytes
  * per frame).  Any of out / out_yuyv / out_mask may be NULL. */
 BSB_API int bsb_composite_sources(bsb_ctx* ctx, int n_frames, const int* source_ids, const uint8_t* frames, size_t frame_pitch,
