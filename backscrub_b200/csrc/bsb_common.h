@@ -95,12 +95,30 @@ BSB_HD float bsb_logistic(float v) {
   return bsb_div(1.f, 1.f + bsb_expf(-v));
 }
 
+// v / 6, correctly rounded (the bits of bsb_div(v, 6.f) under FTZ / DAZ), without the IEEE divide subroutine: the
+// product by RN(1/6) is within one ulp of the quotient, its residual v - 6q is exact in one fmaf, and one correction
+// step rounds to nearest.  The residual of a tiny v would be flushed, the product sends -0 to +0 and +-inf to NaN, so
+// non-finite v and nonzero |v| < 2^-100 take the division; zero (hard-swish of x <= -3) stays on the fast path and
+// copysignf restores its sign.  tests/test_chain_overhead.py compares every float32 bit pattern against the division,
+// on the CPU under FTZ + DAZ and on the GPU against __fdiv_rn.
+BSB_HD float bsb_div6(float v) {
+  const float a = fabsf(v);
+  if (!((a >= 0x1p-100f && a <= 0x1.fffffep127f) || v == 0.f)) return bsb_div(v, 6.f);
+  const float q = v * 0x1.555556p-3f;             // RN(1/6)
+  const float r = fmaf(-q, 6.f, v);
+  return copysignf(fmaf(r, 0x1.555556p-3f, q), v);
+}
+
 // reference hard_swish.h:45-56: x * min(6, max(0, x + 3)) / 6
 BSB_HD float bsb_hard_swish(float x) {
   float t = x + 3.f;
   t = t < 0.f ? 0.f : t;
   t = t > 6.f ? 6.f : t;
+#if defined(__CUDA_ARCH__)
+  return bsb_div6(x * t);
+#else
   return bsb_div(x * t, 6.f);
+#endif
 }
 
 BSB_HD float bsb_act(float x, int act) {

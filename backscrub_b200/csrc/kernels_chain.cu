@@ -22,6 +22,17 @@ namespace bsb {
 
 void count_launch();
 
+#ifdef BSB_EMU
+// the kernel-logic emulator build only (tests/emu, set by the tests through ctypes): nonzero runs every geometry on the
+// runtime-shape instantiations (Meet lite reaches the two-per-SM one anyway; no bundled graph reaches the one-per-SM one)
+extern "C" {
+int bsb_emu_chain_runtime_shape = 0;
+}
+static bool chain_fixed_shape() { return !bsb_emu_chain_runtime_shape; }
+#else
+constexpr bool chain_fixed_shape() { return true; }
+#endif
+
 namespace {
 
 constexpr int CH_T = 512;            // threads per CTA of the one-frame-per-SM instantiation
@@ -203,53 +214,90 @@ BSB_D void chain_dw_slice(const float* E, const float* wds, const ChainOp& op, i
   else chain_dw_slice_t<KS, -1, ELD>(E, wds, op, c0, cw, h, w, es, D);
 }
 
+// CH_DWG: depthwise KS x KS, stride op.s, SAME, from the global tensor op.gin into D[p][c]; taps from shared `wsm`
+// ([KS*KS][C]).  A thread computes 4 channels of one pixel; each window row's KS input loads are issued together before
+// its fmafs.  Out-of-image taps load +0 instead of being skipped: the accumulator starts at +0 and can never become -0
+// (fmaf rounds an exact zero sum to +0), so fmaf(+0, w, acc) leaves it unchanged bit for bit and every output keeps
+// the oracle's fmaf chain over the in-image taps in (fy, fx) order.
+template <int KS>
+BSB_D void chain_dwg(const ChainOp& op, const float* wsm, float* D, int b, int P, int w) {
+  const float* gin = op.gin + (size_t)b * op.gin_frame;
+  const int C = op.cin, groups = C / 4, ld = op.gin_ld, ih = op.ih, iw = op.iw, st = op.s;
+  for (int i = threadIdx.x; i < P * groups; i += blockDim.x) {
+    const int p = i / groups, c0 = (i - p * groups) * 4;
+    const int oy = p / w, ox = p - oy * w;
+    const int iy0 = oy * st - op.pt, ix0 = ox * st - op.pl;
+    const int g0 = (iy0 * iw + ix0) * ld + c0;      // element offset of the window origin (may lie outside the image)
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 1
+    for (int fy = 0; fy < KS; ++fy) {                // one row's loads in flight at a time: more do not fit 80 registers
+      const bool row_in = (unsigned)(iy0 + fy) < (unsigned)ih;
+      float4 v[KS];
+#pragma unroll
+      for (int fx = 0; fx < KS; ++fx)
+        v[fx] = row_in && (unsigned)(ix0 + fx) < (unsigned)iw ? __ldg(reinterpret_cast<const float4*>(gin + g0 + (fy * iw + fx) * ld))
+                                                               : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+      for (int fx = 0; fx < KS; ++fx) {
+        const float4 wv = *reinterpret_cast<const float4*>(wsm + (fy * KS + fx) * C + c0);
+        acc.x = fmaf(v[fx].x, wv.x, acc.x); acc.y = fmaf(v[fx].y, wv.y, acc.y);
+        acc.z = fmaf(v[fx].z, wv.z, acc.z); acc.w = fmaf(v[fx].w, wv.w, acc.w);
+      }
+    }
+    const float4 bv = op.bd ? __ldg(reinterpret_cast<const float4*>(op.bd + c0)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    float* d = D + (size_t)p * CH_DLD + c0;
+    d[0] = chain_act2(acc.x + bv.x, op.dact1, op.dact2);
+    d[1] = chain_act2(acc.y + bv.y, op.dact1, op.dact2);
+    d[2] = chain_act2(acc.z + bv.z, op.dact1, op.dact2);
+    d[3] = chain_act2(acc.w + bv.w, op.dact1, op.dact2);
+  }
+}
+
 }  // namespace
 
+// The op descriptors are copied into shared memory, one op ahead: the loops then read their fields (k, strides, channel
+// counts, weight pointers) from a uniform shared address instead of from global memory behind every barrier.
+constexpr int CH_OP_WORDS = (int)(sizeof(ChainOp) / sizeof(int));
+static_assert(sizeof(ChainOp) % sizeof(int) == 0 && CH_OP_WORDS <= CH_T2, "one thread per ChainOp word");
+constexpr size_t CH_OP_SMEM = 2 * sizeof(ChainOp);   // static shared memory of k_chain: the double-buffered descriptor
+
+BSB_D void chain_fetch_op(int* dst, const ChainOp* src) {
+  if ((int)threadIdx.x < CH_OP_WORDS) dst[threadIdx.x] = __ldg(reinterpret_cast<const int*>(src) + threadIdx.x);
+}
+
 // R: rows per thread tile of the GEMMs; ELD: E slice width; NT, MIN_CTAS: threads per CTA and CTAs per SM.
-// es = chain_estride(w, ELD) comes in as a parameter: read from the constant bank, it costs no register.
-template <int R, int ELD, int NT, int MIN_CTAS>
-__global__ void __launch_bounds__(NT, MIN_CTAS) k_chain(const ChainOp* ops, int n_ops, int h, int w, int es) {
+// HC x WC: the geometry fixed at compile time (pixel counts, strides, strip and tile counts become constants, index
+// divisions by them become multiplies and shifts); HC = WC = 0 takes h, w and es = chain_estride(w, ELD) at run time
+// (read from the constant bank, they cost no register).
+template <int R, int ELD, int NT, int MIN_CTAS, int HC, int WC>
+__global__ void __launch_bounds__(NT, MIN_CTAS) k_chain(const ChainOp* ops, int n_ops, int h_rt, int w_rt, int es_rt) {
   // expand GEMM into a 16-column slice: (P / 2) x 4 thread tiles (Meet: 288 of the 384 threads)
   constexpr int RE = ELD == 16 ? 2 : R;
+  const int h = HC ? HC : h_rt, w = WC ? WC : w_rt, es = HC ? chain_estride(WC, ELD) : es_rt;
   BSB_DYN_SMEM(smem_raw);
+  __shared__ __align__(16) int op_sm[2][CH_OP_WORDS];
   float* sm = reinterpret_cast<float*>(smem_raw);
   const int P = h * w;
   const ChainLayout L = chain_layout(h, w, ELD);
   float* X = sm + L.off_x; float* D = sm + L.off_d; float* E = sm + L.off_e;
   float* w1s = sm + L.off_w1; float* wds = sm + L.off_wd;
   float* v0 = sm + L.off_vec; float* v1 = v0 + 128; float* sv = v1 + 128;
-  const int tid = threadIdx.x, T = blockDim.x;
+  const int tid = threadIdx.x, T = NT;                  // launched with NT threads
   const int b = blockIdx.x;
 
+  chain_fetch_op(op_sm[0], ops);
   for (int oi = 0; oi < n_ops; ++oi) {
-    const ChainOp& op = ops[oi];
-    __syncthreads();                                      // the previous op's results are complete
+    __syncthreads();                                      // the previous op's results (and op_sm[oi & 1]) are complete
+    if (oi + 1 < n_ops) chain_fetch_op(op_sm[(oi + 1) & 1], ops + oi + 1);   // its buffer was last read by op oi - 1
+    const ChainOp& op = *reinterpret_cast<const ChainOp*>(op_sm[oi & 1]);
     switch (op.type) {
       case CH_DWG: {
-        // depthwise k x k, stride s, SAME padding, straight from the global input tensor into D[p][c]
-        const float* gin = op.gin + (size_t)b * op.gin_frame;
-        const int C = op.cin, groups = C / 4;
-        for (int i = tid; i < P * groups; i += T) {
-          const int p = i / groups, c0 = (i - p * groups) * 4;
-          const int oy = p / w, ox = p - oy * w;
-          float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
-          for (int fy = 0; fy < op.k; ++fy) {
-            const int iy = oy * op.s - op.pt + fy;
-            if (iy < 0 || iy >= op.ih) continue;
-            for (int fx = 0; fx < op.k; ++fx) {
-              const int ix = ox * op.s - op.pl + fx;
-              if (ix < 0 || ix >= op.iw) continue;
-              const float4 v = __ldg(reinterpret_cast<const float4*>(gin + ((size_t)iy * op.iw + ix) * op.gin_ld + c0));
-              const float4 wv = __ldg(reinterpret_cast<const float4*>(op.wd + (size_t)(fy * op.k + fx) * C + c0));
-              acc.x = fmaf(v.x, wv.x, acc.x); acc.y = fmaf(v.y, wv.y, acc.y); acc.z = fmaf(v.z, wv.z, acc.z); acc.w = fmaf(v.w, wv.w, acc.w);
-            }
-          }
-          float* d = D + (size_t)p * CH_DLD + c0;
-          d[0] = chain_act2(acc.x + (op.bd ? __ldg(op.bd + c0) : 0.f), op.dact1, op.dact2);
-          d[1] = chain_act2(acc.y + (op.bd ? __ldg(op.bd + c0 + 1) : 0.f), op.dact1, op.dact2);
-          d[2] = chain_act2(acc.z + (op.bd ? __ldg(op.bd + c0 + 2) : 0.f), op.dact1, op.dact2);
-          d[3] = chain_act2(acc.w + (op.bd ? __ldg(op.bd + c0 + 3) : 0.f), op.dact1, op.dact2);
-        }
+        // depthwise k x k, stride s, SAME padding, straight from the global input tensor into D[p][c].  The taps
+        // (k * k * C <= 25 * 128 floats, Engine::detect_chain) are staged in E, which is free here.
+        chain_stage(E, op.wd, op.k * op.k * op.cin);
+        __syncthreads();
+        if (op.k == 5) chain_dwg<5>(op, E, D, b, P, w);
+        else chain_dwg<3>(op, E, D, b, P, w);
         break;
       }
       case CH_EXPAND_DW: {
@@ -357,7 +405,7 @@ ChainConfig chain_config(int h, int w) {
       per_sm = 0;
     }
 #endif
-    if (2 * (bytes + (size_t)reserved) <= (size_t)per_sm) return {true, bytes};
+    if (2 * (bytes + CH_OP_SMEM + (size_t)reserved) <= (size_t)per_sm) return {true, bytes};
   }
   return {false, (size_t)chain_layout(h, w, 32).total * sizeof(float)};
 }
@@ -371,26 +419,47 @@ size_t chain_smem_bytes(int h, int w) {
   return bytes <= 226 * 1024 ? bytes : 0;
 }
 
+namespace {
+
+// two 384-thread CTAs per SM, 16-channel E slices
+template <int HC, int WC>
+void launch_chain_two(cudaStream_t s, int B, int h, int w, size_t smem, const ChainOp* d_ops, int n_ops) {
+  auto k = k_chain<3, 16, CH_T2, 2, HC, WC>;
+  ensure_dyn_smem(reinterpret_cast<const void*>(k), smem);
+#ifndef BSB_EMU
+  // the whole unified L1 / shared array as shared memory: room for the two CTAs (set once per device and instantiation)
+  static std::once_flag carveout[64];
+  int dev = 0;
+  if (cudaGetDevice(&dev) == cudaSuccess && dev < 64)
+    std::call_once(carveout[dev], [&] {
+      if (cudaFuncSetAttribute(reinterpret_cast<const void*>(k), cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess)
+        cudaGetLastError();
+    });
+#endif
+  BSB_LAUNCH(k, dim3((unsigned)B), dim3(CH_T2), smem, s, d_ops, n_ops, h, w, chain_estride(w, 16));
+}
+
+// one 512-thread CTA per SM, 32-channel E slices
+template <int HC, int WC>
+void launch_chain_one(cudaStream_t s, int B, int h, int w, size_t smem, const ChainOp* d_ops, int n_ops) {
+  auto k = k_chain<4, 32, CH_T, 1, HC, WC>;
+  ensure_dyn_smem(reinterpret_cast<const void*>(k), smem);
+  BSB_LAUNCH(k, dim3((unsigned)B), dim3(CH_T), smem, s, d_ops, n_ops, h, w, chain_estride(w, 32));
+}
+
+}  // namespace
+
+// Meet full (9x16) and MLKit (16x16) run instantiations with the shape fixed at compile time; any other shape
+// chain_smem_bytes accepts, Meet lite's 6x10 among them, runs the runtime-shape one of its configuration (a 6x10
+// instantiation needs one register more than the 80 that two CTAs per SM allow, and would spill).
 void launch_chain(cudaStream_t s, int B, int h, int w, const ChainOp* d_ops, int n_ops) {
   const ChainConfig cfg = chain_config(h, w);
   if (cfg.two_per_sm) {
-    auto k = k_chain<3, 16, CH_T2, 2>;
-    ensure_dyn_smem(reinterpret_cast<const void*>(k), cfg.smem);
-#ifndef BSB_EMU
-    // the whole unified L1 / shared array as shared memory: room for the two CTAs (set once per device)
-    static std::once_flag carveout[64];
-    int dev = 0;
-    if (cudaGetDevice(&dev) == cudaSuccess && dev < 64)
-      std::call_once(carveout[dev], [&] {
-        if (cudaFuncSetAttribute(reinterpret_cast<const void*>(k), cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared) != cudaSuccess)
-          cudaGetLastError();
-      });
-#endif
-    BSB_LAUNCH(k, dim3((unsigned)B), dim3(CH_T2), cfg.smem, s, d_ops, n_ops, h, w, chain_estride(w, 16));
+    if (chain_fixed_shape() && h == 9 && w == 16) launch_chain_two<9, 16>(s, B, h, w, cfg.smem, d_ops, n_ops);
+    else launch_chain_two<0, 0>(s, B, h, w, cfg.smem, d_ops, n_ops);
   } else {
-    auto k = k_chain<4, 32, CH_T, 1>;
-    ensure_dyn_smem(reinterpret_cast<const void*>(k), cfg.smem);
-    BSB_LAUNCH(k, dim3((unsigned)B), dim3(CH_T), cfg.smem, s, d_ops, n_ops, h, w, chain_estride(w, 32));
+    if (chain_fixed_shape() && h == 16 && w == 16) launch_chain_one<16, 16>(s, B, h, w, cfg.smem, d_ops, n_ops);
+    else launch_chain_one<0, 0>(s, B, h, w, cfg.smem, d_ops, n_ops);
   }
   count_launch();
 }

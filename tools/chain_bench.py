@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """SM time of the low-resolution chain kernel (k_chain, kernels_chain.cu) per Meet frame.
 
-    python tools/chain_bench.py --out DIR [--calls 30] [--warmup 5]
+    python tools/chain_bench.py --out DIR [--calls 30] [--warmup 5] [--lib PATH]
 
 One Meet full context (segm_full_v679, 1280x720 camera YUYV frames resident on the device) with max_batch = 2 x SMs.
 For n = SMs and n = 2 x SMs frames per call: `warmup` calls, then `calls` calls captured with torch.profiler (CUDA
@@ -9,7 +9,9 @@ activities only), one capture per n, written to DIR/chain_bench_n<n>.pt.trace.js
 min and max k_chain duration per call, and the chain's SM time per frame = median x SMs / n.
 
 With one CTA per SM the 2 x SMs call takes about twice the SMs call; with two co-resident CTAs per SM it takes
-clearly less.  Prints one JSON line, with the GPU name and power limit read in the same run."""
+clearly less.  With --lib (the library of another build, e.g. the parent of a chain change) that library is timed
+instead of the package's, so two builds can be run alternately in one session.  Prints one JSON line, with the GPU name
+and power limit read in the same run."""
 import argparse
 import json
 import os
@@ -40,6 +42,7 @@ def main():
     ap.add_argument("--calls", type=int, default=30)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--lib", default=None, help="library of another build (default: the package's)")
     args = ap.parse_args()
     if args.calls < 20:
         raise SystemExit("--calls must be >= 20")
@@ -48,7 +51,9 @@ def main():
     from torch.profiler import ProfilerActivity, profile
 
     import backscrub_b200 as bs
+    from backscrub_b200 import api
     from tests import synth
+    from tools.source_effects_bench import bind_older
     from tools.sources_bench import gpu_info
 
     if bs.device_count() <= 0:
@@ -64,7 +69,8 @@ def main():
     d_out = torch.empty((n_max, H, W, 3), dtype=torch.uint8, device=cuda)
     d_yuyv = torch.empty((n_max, H, W, 2), dtype=torch.uint8, device=cuda)
     d_mask = torch.empty((n_max, H, W), dtype=torch.uint8, device=cuda)
-    g = bs.bs_maskgen_new(os.path.join(ROOT, "models", MODEL), 2, W, H, device=dev, max_batch=n_max)
+    lib = bind_older(args.lib) if args.lib else bs.lib()
+    g = api.MaskGen(lib, os.path.join(ROOT, "models", MODEL), W, H, device=dev, max_batch=n_max)
     g.set_background(synth.background())
 
     def call(n):
@@ -79,7 +85,8 @@ def main():
             for _ in range(args.calls):
                 call(n)
             torch.cuda.synchronize()
-        path = os.path.join(args.out, f"chain_bench_n{n}.pt.trace.json")
+        tag = "_" + os.path.splitext(os.path.basename(args.lib))[0] if args.lib else ""
+        path = os.path.join(args.out, f"chain_bench{tag}_n{n}.pt.trace.json")
         prof.export_chrome_trace(path)
         durs, names = chain_durations_us(path)
         if len(durs) != args.calls:
@@ -89,7 +96,7 @@ def main():
                     "k_chain_us_median": round(med, 2), "k_chain_us_min": round(min(durs), 2), "k_chain_us_max": round(max(durs), 2),
                     "chain_sm_us_per_frame": round(med * sms / n, 3), "trace": os.path.basename(path)})
     g.close()
-    out = {"tool": "chain_bench", **gpu_info(dev), "sms": sms, "model": MODEL, "frame": f"{W}x{H}",
+    out = {"tool": "chain_bench", "lib": args.lib or "package", **gpu_info(dev), "sms": sms, "model": MODEL, "frame": f"{W}x{H}",
            "input": "device-resident camera YUYV", "warmup_calls": args.warmup, "results": res,
            "ratio_2x_sms_over_sms_call": round(res[1]["k_chain_us_median"] / res[0]["k_chain_us_median"], 3)}
     print(json.dumps(out))
