@@ -16,6 +16,7 @@ STAGE_CB = C.CFUNCTYPE(None, C.c_void_p)
 BG_READ_CB = C.CFUNCTYPE(C.c_int, C.c_void_p, C.POINTER(C.c_void_p), i32p, i32p, C.POINTER(C.c_size_t))
 BG_REWIND_CB = C.CFUNCTYPE(C.c_int, C.c_void_p)
 
+FEED_LOGITS, FEED_MASK = 1, 2
 FLAG_KEEP_TENSORS, FLAG_NO_GRAPH, FLAG_TENSOR_CORES, FLAG_FUSE_BLOCKS, FLAG_EXACT = 1, 2, 4, 8, 16
 
 # every symbol include/backscrub_b200.h declares (tests check the .so exports all of them)
@@ -34,6 +35,7 @@ SYMBOLS = [
     "bsb_set_sources", "bsb_reset_source", "bsb_set_source_background", "bsb_composite_sources", "bsb_composite_sources_yuyv_device",
     "bsb_composite_nv12", "bsb_composite_nv12_device", "bsb_composite_sources_nv12_device", "bsb_convert_nv12_to_bgr",
     "bsb_set_source_effect", "bsb_set_source_flip", "bsb_set_source_output", "bsb_source_output_size",
+    "bsb_test_feed_shape", "bsb_test_feed",
 ]
 
 
@@ -145,5 +147,8 @@ def bind(path: str) -> C.CDLL:
                                             C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int]
     L.bsb_composite_sources_nv12_device.argtypes = [C.c_void_p, C.c_int, i32p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_size_t, C.c_void_p,
                                                     C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int]
+    L.bsb_test_feed_shape.restype = C.c_long
+    L.bsb_test_feed_shape.argtypes = [C.c_void_p, C.c_int, i32p]
+    L.bsb_test_feed.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t]
     L.bsb_convert_nv12_to_bgr.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
     return L

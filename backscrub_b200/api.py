@@ -405,6 +405,22 @@ class MaskGen:
             self._fail("bsb_get_stage_u8")
         return buf.reshape(shape)
 
+    def feed_shape(self, stage: int):
+        """(h, w, c) of one frame of the tensor a feed of `stage` (_binding.FEED_LOGITS / FEED_MASK) replaces"""
+        hwc = (C.c_int * 3)()
+        if self._lib.bsb_test_feed_shape(self._h, int(stage), hwc) < 0:
+            self._fail("bsb_test_feed_shape")
+        return tuple(hwc)
+
+    def feed(self, stage: int, array: np.ndarray):
+        """Test entry point (bsb_test_feed): the next composite call takes `array` as the tensor of `stage` instead of
+        computing it — FEED_LOGITS: float32 [n, h, w, c] logits the decision reads; FEED_MASK: uint8 [n, oh, ow] smoother
+        output.  That call must have n frames."""
+        dt = np.float32 if stage == B.FEED_LOGITS else np.uint8
+        a = np.ascontiguousarray(array, dt)
+        if not self._lib.bsb_test_feed(self._h, int(stage), int(a.shape[0]), _ptr(a), a.nbytes):
+            self._fail("bsb_test_feed")
+
     def reset_state(self):
         if not self._lib.bsb_reset_state(self._h):
             self._fail("bsb_reset_state")

@@ -164,6 +164,12 @@ cudaError_t copy_out_sized(const bsb::Call& h, const bsb::Call& d, const Engine*
   return cudaSuccess;
 }
 
+// A feed armed by bsb_test_feed is consumed by the next composite call, also when that call is refused before it runs
+struct FeedConsumed {
+  Engine* e;
+  ~FeedConsumed() { if (e->feed_armed()) e->disarm_feed(); }
+};
+
 // Every host-buffer composite call.  `h` describes the caller's host buffers: every row is packed except BGR input rows
 // (h.pitch bytes apart) and, where given, output rows (*out_pitch bytes apart).  The frames are copied into the context
 // staging (MJPG: `jpegs` decoded there instead), the call runs on it, and each requested output is copied back before
@@ -173,6 +179,7 @@ int host_call(bsb_ctx* ctx, const bsb::Call& h, const char* what, const size_t* 
   if (!check_ctx(ctx)) return 0;
   const bsb::Callbacks* cbp = &ctx->cb;
   Engine* e = ctx->eng;
+  const FeedConsumed consumed{e};
   const bool bgr = h.fmt == bsb::IN_BGR, nv12 = h.fmt == bsb::IN_NV12;
   const size_t W = e->W(), H = e->H(), orow = (size_t)e->out_w() * 3, cpx = (size_t)e->out_w() * e->out_h();
   // sources calls: the staging holds frames of the largest size any source has; `sized`: some frame's size is its own
@@ -211,6 +218,10 @@ int host_call(bsb_ctx* ctx, const bsb::Call& h, const char* what, const size_t* 
   // that: cap.read -> CalcMask -> write); results are identical, only the schedule changes.
   const int chunk = bsb::tuning().e2e_chunk;
   const bool piped = h.fmt == bsb::IN_YUYV && chunk > 0 && h.n >= 2 * chunk && (h.n + chunk - 1) / chunk <= bsb_ctx::kMaxChunks;
+  if (piped && e->feed_armed()) {
+    report(cbp, std::string("error: ") + what + "a fed call runs as one launch, and this call would be split into chunks (e2e_chunk)");
+    return 0;
+  }
   if (piped && !ctx->pipe_ready) {
     API_CUDA(cudaStreamCreateWithFlags(&ctx->s_in, cudaStreamNonBlocking));
     API_CUDA(cudaStreamCreateWithFlags(&ctx->s_out, cudaStreamNonBlocking));
@@ -258,6 +269,7 @@ int device_call(bsb_ctx* ctx, bsb::Call c, int sync) {
   if (!check_ctx(ctx)) return 0;
   const bsb::Callbacks* cbp = &ctx->cb;
   Engine* e = ctx->eng;
+  const FeedConsumed consumed{e};
   if (c.fmt == bsb::IN_BGR) c.pitch = (size_t)e->W() * 3;
   if (c.fmt == bsb::IN_YUYV) { c.pitch = (size_t)e->W() * 2; c.stride = c.pitch * e->H(); }
   // the engine checks an NV12 call's frames and output with their layout
@@ -272,6 +284,7 @@ int device_call(bsb_ctx* ctx, bsb::Call c, int sync) {
 // sources entry points refuse a null id table first (a Call without ids is a plain call)
 bool null_ids(bsb_ctx* ctx, const int* ids) {
   if (ids || !check_ctx(ctx)) return false;
+  const FeedConsumed consumed{ctx->eng};
   report(&ctx->cb, "error: null source id table");
   return true;
 }
@@ -829,6 +842,21 @@ long bsb_get_stage_u8(bsb_ctx* ctx, int which, int frame, uint8_t* out, long cap
   long n = ctx->eng->get_stage_u8(which, frame, out, capacity, &err);
   if (n < 0) report(&ctx->cb, "error: " + err);
   return n;
+}
+
+long bsb_test_feed_shape(bsb_ctx* ctx, int stage, int hwc[3]) {
+  if (!check_ctx(ctx)) return -1;
+  int h = 0, w = 0, c = 0;
+  if (!ctx->eng->feed_shape(stage, &h, &w, &c)) { report(&ctx->cb, "error: unknown feed stage"); return -1; }
+  if (hwc) { hwc[0] = h; hwc[1] = w; hwc[2] = c; }
+  return (long)h * w * c * (stage == BSB_FEED_LOGITS ? (long)sizeof(float) : 1L);
+}
+
+int bsb_test_feed(bsb_ctx* ctx, int stage, int n_frames, const void* data, size_t bytes) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->arm_feed(stage, n_frames, data, bytes, &err)) { report(&ctx->cb, "error: bsb_test_feed: " + err); return 0; }
+  return 1;
 }
 
 int bsb_reset_state(bsb_ctx* ctx) {

@@ -1315,19 +1315,70 @@ bool Engine::enqueue_all(const Call& c, const Plan& p) {
   const int n = c.n;
   if (c.fmt == IN_NV12 && !p.native) launch_nv12_to_bgr(stream_, n, c.in, c.pitch, c.uv, c.stride, d_frames_, W_, H_);
   if (c.fmt == IN_YUYV && !p.native) launch_yuyv_to_bgr(stream_, c.in, d_frames_, (size_t)n * W_ * H_);
-  enqueue_pre(c);
-  if (c.callbacks && cb_.onprep) { cudaStreamSynchronize(stream_); cb_.onprep(cb_.caller_ctx); }
-  enqueue_cnn(n, true);
-  if (c.callbacks && cb_.oninfer) { cudaStreamSynchronize(stream_); cb_.oninfer(cb_.caller_ctx); }
-  enqueue_decision(n, p.mode != CALL_PLAIN);
-  if (c.callbacks && cb_.onmask) { cudaStreamSynchronize(stream_); cb_.onmask(cb_.caller_ctx); }
+  if (fed_) {
+    enqueue_feed(*fed_);
+    if (fed_->stage == FEED_LOGITS) enqueue_decision(n, p.mode != CALL_PLAIN);
+  } else {
+    enqueue_pre(c);
+    if (c.callbacks && cb_.onprep) { cudaStreamSynchronize(stream_); cb_.onprep(cb_.caller_ctx); }
+    enqueue_cnn(n, true);
+    if (c.callbacks && cb_.oninfer) { cudaStreamSynchronize(stream_); cb_.oninfer(cb_.caller_ctx); }
+    enqueue_decision(n, p.mode != CALL_PLAIN);
+    if (c.callbacks && cb_.onmask) { cudaStreamSynchronize(stream_); cb_.onmask(cb_.caller_ctx); }
+  }
   if (!enqueue_post(c, p)) return false;
   if (p.nv12_staged) launch_yuyv_to_nv12(stream_, n, d_yuyv_, (size_t)W_ * H_ * 2, c.video, c.video_stride, W_, H_);
   last_call_launches_ = (int)(thread_launch_count() - l0);
   return true;
 }
 
+bool Engine::feed_shape(int stage, int* h, int* w, int* c) const {
+  if (stage == FEED_MASK) { *h = oh_; *w = ow_; *c = 1; return true; }
+  if (stage != FEED_LOGITS) return false;
+  const TensorInfo& I = tinfo_[dec_up_step_ >= 0 ? steps_[dec_up_step_].in : g_.output];
+  *h = I.h; *w = I.w; *c = I.c;
+  return true;
+}
+
+bool Engine::arm_feed(int stage, int n, const void* data, size_t bytes, std::string* err) {
+  feed_ = Feed{};
+  int h = 0, w = 0, ch = 0;
+  if (!feed_shape(stage, &h, &w, &ch)) { *err = "unknown feed stage"; return false; }
+  if (n < 1 || n > max_batch_) { *err = "n_frames out of range (1..max_batch)"; return false; }
+  const size_t need = (size_t)n * h * w * ch * (stage == FEED_LOGITS ? sizeof(float) : 1);
+  if (!data || bytes != need) { *err = "feed size differs from n_frames times the stage's frame size"; return false; }
+  feed_.stage = stage; feed_.n = n;
+  feed_.data.assign((const uint8_t*)data, (const uint8_t*)data + bytes);
+  return true;
+}
+
+void Engine::enqueue_feed(const Feed& f) {
+  const int n = f.n;
+  if (f.stage == FEED_MASK) {
+    cudaMemcpy2DAsync(ofinal_, opitch_, f.data.data(), ow_, ow_, (size_t)n * oh_, cudaMemcpyHostToDevice, stream_);
+    return;
+  }
+  // the layout the decision kernels read: [n][h][w][ld] floats, the first c of each pixel's ld
+  const int t = dec_up_step_ >= 0 ? steps_[dec_up_step_].in : g_.output;
+  const TensorInfo& I = tinfo_[t];
+  cudaMemcpy2DAsync(tptr(t), (size_t)I.ld * 4, f.data.data(), (size_t)I.c * 4, (size_t)I.c * 4, (size_t)n * I.h * I.w,
+                    cudaMemcpyHostToDevice, stream_);
+}
+
+// A call with an armed feed: eager (the captured graphs are neither used nor changed), the feed consumed whatever the outcome
+bool Engine::run_fed(const Call& c, std::string* err) {
+  Feed f;
+  std::swap(f, feed_);
+  if (c.n != f.n) { *err = "the call's n_frames differs from the armed feed's"; return false; }
+  fed_ = &f;
+  const bool ok = run(c, err);
+  fed_ = nullptr;
+  if (ok) CUDA_OK(cudaStreamSynchronize(stream_));    // the feed's host copy is read by the queued copy
+  return ok;
+}
+
 bool Engine::run(const Call& c, std::string* err) {
+  if (feed_.stage != FEED_NONE) return run_fed(c, err);
   const int n = c.n;
   if (c.fmt == IN_NV12) {
     if ((W_ & 1) || (H_ & 1)) { *err = "NV12 needs an even frame width and height"; return false; }
@@ -1380,7 +1431,7 @@ bool Engine::run(const Call& c, std::string* err) {
     CUDA_OK(cudaMemcpyAsync(d_src_tab_, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, stream_));
   }
   const bool cbs = c.callbacks && (cb_.onprep || cb_.oninfer || cb_.onmask);
-  bool eager = cbs || (flags_ & 2u);
+  bool eager = cbs || (flags_ & 2u) || fed_;
 #ifdef BSB_EMU
   eager = true;
 #endif

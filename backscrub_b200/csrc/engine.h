@@ -139,6 +139,17 @@ class Engine {
   int n_sources() const { return n_sources_; }
   double time_stage(int stage, int n, int iters, std::string* err);
 
+  // Test entry point (include/backscrub_b200.h, bsb_test_feed): the next call takes the tensor a stage reads from the
+  // caller instead of computing it.  FEED_LOGITS: the fp32 tensor the decision reads, [n][h][w][c] packed (pre-processing
+  // and the CNN are skipped); FEED_MASK: the smoother output ofinal, [n][oh][ow] bytes (the decision is skipped too, and
+  // no smoother state changes).  The fed call runs eagerly and consumes the feed whatever its outcome.
+  enum { FEED_NONE = 0, FEED_LOGITS = 1, FEED_MASK = 2 };
+  // h, w, c of one frame of a stage's tensor; false for an unknown stage
+  bool feed_shape(int stage, int* h, int* w, int* c) const;
+  bool arm_feed(int stage, int n, const void* data, size_t bytes, std::string* err);
+  bool feed_armed() const { return feed_.stage != FEED_NONE; }
+  void disarm_feed() { feed_ = Feed{}; }
+
   // accessors
   int W() const { return W_; }
   int H() const { return H_; }
@@ -215,6 +226,12 @@ class Engine {
   }
   // false (nothing more enqueued) only when the post kernel cannot write a call's mirrored frames
   bool enqueue_all(const Call& c, const Plan& p);
+  struct Feed { int stage = FEED_NONE, n = 0; std::vector<uint8_t> data; };
+  Feed feed_;                        // armed by arm_feed for the next call
+  const Feed* fed_ = nullptr;        // the feed of the call being enqueued (run_fed), else null
+  bool run_fed(const Call& c, std::string* err);
+  // the fed tensor into the place the skipped stages write (ofinal_, or the tensor the decision reads)
+  void enqueue_feed(const Feed& f);
   bool refresh_bg_yuyv(std::string* err);
   void enqueue_cnn(int n, bool from_u8);
   void enqueue_decision(int n, bool sources);

@@ -355,6 +355,24 @@ BSB_API int bsb_tc_steps(bsb_ctx* ctx, int* rows, int capacity);
 /* stage buffers of the last call, frame `frame`: which = 0 model-sized RGB u8 (after resize +
  * BGR2RGB), 1 bilateral-filtered u8, 2 ofinal (IIR state after that frame) */
 BSB_API long bsb_get_stage_u8(bsb_ctx* ctx, int which, int frame, uint8_t* out, long capacity);
+/* Test entry point: feed chosen values to the decision or the post stage of the next composite call, so that their
+ * kernels can be checked on constructed inputs (ties, overflows, thresholds, single-pixel masks) rather than on what the
+ * CNN makes of a frame.
+ *   BSB_FEED_LOGITS: float32 values of the tensor the decision stage reads, [n][h][w][c] packed (DeepLab: the low-
+ *                    resolution tensor of the resize the decision kernel folds in); pre-processing and the CNN are skipped.
+ *                    The smoother states advance as in a real call.
+ *   BSB_FEED_MASK:   the smoother output (`ofinal`) bytes, [n][oh][ow] packed; the decision is skipped too, and neither
+ *                    the plain nor any source's smoother state changes.
+ * bsb_test_feed copies `bytes` bytes (n_frames times the stage's frame size) and arms them for the next composite call on
+ * the context, of any kind (plain, YUYV, NV12, device or host buffers, sources), which must have n_frames frames.  That
+ * call runs eagerly (the captured CUDA graphs are neither used nor changed) and is synchronous; the YUYV / NV12 -> BGR
+ * conversion and everything from the post stage on run as in any call.  The next composite call consumes the feed
+ * whatever its outcome.  A wrong size, an unknown stage, a call of another frame count or a host call that would be
+ * split into chunks (e2e_chunk) returns 0 with a bsb_last_error() message and leaves the context usable.
+ * bsb_test_feed_shape: h, w, c of one frame of a stage's tensor into hwc; returns its bytes, -1 for an unknown stage. */
+enum { BSB_FEED_LOGITS = 1, BSB_FEED_MASK = 2 };
+BSB_API long bsb_test_feed_shape(bsb_ctx* ctx, int stage, int hwc[3]);
+BSB_API int bsb_test_feed(bsb_ctx* ctx, int stage, int n_frames, const void* data, size_t bytes);
 /* reset the temporal IIR state to zero (start of a new stream) */
 BSB_API int bsb_reset_state(bsb_ctx* ctx);
 /* kernel launches per n-frame call (graph nodes) and launches issued so far by this process */
