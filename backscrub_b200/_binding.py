@@ -35,6 +35,7 @@ SYMBOLS = [
     "bsb_set_sources", "bsb_reset_source", "bsb_set_source_background", "bsb_composite_sources", "bsb_composite_sources_yuyv_device",
     "bsb_composite_nv12", "bsb_composite_nv12_device", "bsb_composite_sources_nv12_device", "bsb_convert_nv12_to_bgr",
     "bsb_set_source_effect", "bsb_set_source_flip", "bsb_set_source_output", "bsb_source_output_size",
+    "bsb_set_source_background_ring", "bsb_set_source_background_cursor",
     "bsb_test_feed_shape", "bsb_test_feed",
 ]
 
@@ -133,6 +134,8 @@ def bind(path: str) -> C.CDLL:
     L.bsb_set_sources.argtypes = [C.c_void_p, C.c_int]
     L.bsb_reset_source.argtypes = [C.c_void_p, C.c_int]
     L.bsb_set_source_background.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_size_t]
+    L.bsb_set_source_background_ring.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_size_t, C.c_size_t, C.c_int]
+    L.bsb_set_source_background_cursor.argtypes = [C.c_void_p, C.c_int, C.c_int]
     L.bsb_set_source_effect.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
     L.bsb_set_source_flip.argtypes = [C.c_void_p, C.c_int, C.c_int]
     L.bsb_set_source_output.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]

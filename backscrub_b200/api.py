@@ -264,6 +264,21 @@ class MaskGen:
         if not ok:
             self._fail("bsb_set_source_background")
 
+    def set_source_background_ring(self, source: int, frames: np.ndarray, advance: int = 1):
+        """Animated background of one source: frames [count, bh, bw, 3] -> the source's device-resident ring (resized like
+        set_background_ring, blurred at the source's strength).  Each sources call carrying a frame of the source blends
+        ring image `cursor`, then moves the cursor on by `advance`; advance 0 leaves pacing to
+        set_source_background_cursor.  set_source_background(source, None) clears it."""
+        frames = np.ascontiguousarray(frames, np.uint8)
+        c, bh, bw, _ = frames.shape
+        if not self._lib.bsb_set_source_background_ring(self._h, int(source), _ptr(frames), c, bw, bh, bw * 3, bh * bw * 3, int(advance)):
+            self._fail("bsb_set_source_background_ring")
+
+    def set_source_background_cursor(self, source: int, index: int):
+        """the ring image the next call carrying a frame of `source` blends (host bookkeeping only)"""
+        if not self._lib.bsb_set_source_background_cursor(self._h, int(source), int(index)):
+            self._fail("bsb_set_source_background_cursor")
+
     def set_source_effect(self, source: int, background: str = "default", bgblur: int = -1):
         """background effect of one source: background "default" (its own image, else the context's) or "none" (no
         image: the blurred camera frame when the strength is > 0, else green); bgblur -1 = follow set_bgblur, 0 = off,

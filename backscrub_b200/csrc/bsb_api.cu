@@ -491,6 +491,25 @@ int bsb_set_source_background(bsb_ctx* ctx, int source, const uint8_t* bg_raw, i
   return 1;
 }
 
+int bsb_set_source_background_ring(bsb_ctx* ctx, int source, const uint8_t* frames, int count, int bg_w, int bg_h, size_t bg_pitch,
+                                   size_t frame_stride, int advance) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!frames) { report(&ctx->cb, "error: invalid background (null frames; bsb_set_source_background(NULL) clears a source's background)"); return 0; }
+  if (!ctx->eng->set_source_ring(source, frames, count, bg_w, bg_h, bg_pitch, frame_stride, advance, &err)) {
+    report(&ctx->cb, "error: " + err);
+    return 0;
+  }
+  return 1;
+}
+
+int bsb_set_source_background_cursor(bsb_ctx* ctx, int source, int index) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_source_cursor(source, index, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
 int bsb_set_source_effect(bsb_ctx* ctx, int source, int background, int bgblur) {
   if (!check_ctx(ctx)) return 0;
   std::string err;

@@ -1406,11 +1406,10 @@ bool Engine::run(const Call& c, std::string* err) {
         if (c.ids[j] == id) { *err = "source ids must be distinct within one call"; return false; }
       tab[b] = id;
       int k = 0;
-      const int from = source_bg(id, &k);
-      int slot = max_batch_;
-      if (from == SRC_FROM_SLOT) slot = max_batch_ + 1 + id;
-      else if (from == SRC_FROM_CAMBLUR) { slot = b; tab[2 * (size_t)max_batch_ + b] = k; p.gclass |= (unsigned)gauss_class(k); ++n_blur; }
-      tab[(size_t)max_batch_ + b] = slot;
+      size_t slot = 0;
+      const int from = source_bg(id, &k, &slot);
+      if (from == SRC_FROM_CAMBLUR) { slot = b; tab[2 * (size_t)max_batch_ + b] = k; p.gclass |= (unsigned)gauss_class(k); ++n_blur; }
+      tab[(size_t)max_batch_ + b] = (int)slot;
       const int fl = src_flip_[id] < 0 ? ctx_flip : src_flip_[id];
       tab[3 * (size_t)max_batch_ + b] = fl;
       p.flipped = p.flipped || fl != 0;
@@ -1441,6 +1440,7 @@ bool Engine::run(const Call& c, std::string* err) {
     last_native_ = p.native;
     if (!enqueue_all(c, p)) { *err = kNoMirror; return false; }
     CUDA_OK(cudaGetLastError());
+    move_cursors(c);
     return true;
   }
 #ifndef BSB_EMU
@@ -1476,8 +1476,19 @@ bool Engine::run(const Call& c, std::string* err) {
   }
   last_call_launches_ = it->second.launches;
   CUDA_OK(cudaGraphLaunch(it->second.exec, stream_));
+  move_cursors(c);
 #endif
   return true;
+}
+
+// after a sources call is enqueued: the ring of every source with a frame in it moves on, blended or not (a video keeps
+// playing while a source shows no image or its blurred camera frame).  The next call's table carries the new slots.
+void Engine::move_cursors(const Call& c) {
+  if (!c.ids) return;
+  for (int b = 0; b < c.n; ++b) {
+    SrcRing& r = src_ring_[c.ids[b]];
+    if (r.count > 1) r.cursor = (int)(((long)r.cursor + r.advance) % r.count);
+  }
 }
 
 uint8_t* Engine::nv12_staging(std::string* err) {
@@ -1541,7 +1552,7 @@ bool Engine::set_background_ring(const uint8_t* frames, int count, int bw, int b
   if (!refresh_bg_blur(err)) return false;
   if (!refresh_bg_yuyv(err)) return false;
   if (!refresh_bank_ctx(err)) return false;
-  if (!refresh_bank_sources_after_ctx(err)) return false;
+  if (!refresh_bank_sources_after_ctx(false, err)) return false;
   CUDA_OK(cudaStreamSynchronize(stream_));
   CUDA_OK(cudaGetLastError());
   return true;
@@ -1602,7 +1613,7 @@ bool Engine::set_bgblur(int k, std::string* err) {
   if (!refresh_bg_blur(err)) return false;
   if (!refresh_bg_yuyv(err)) return false;
   if (!refresh_bank_ctx(err)) return false;
-  if (!refresh_bank_sources_after_ctx(err)) return false;
+  if (!refresh_bank_sources_after_ctx(true, err)) return false;
   CUDA_OK(cudaStreamSynchronize(stream_));
   return true;
 }
@@ -1645,10 +1656,12 @@ bool Engine::reset_state(std::string* err) {
 // independent sources
 // ---------------------------------------------------------------------------
 void Engine::free_sources() {
-  for (void* p : {(void*)src_state_, (void*)d_bank_, (void*)d_bank_yuyv_, (void*)d_bank_nv12_, (void*)d_src_bg_, (void*)d_green_}) if (p) cudaFree(p);
-  src_state_ = nullptr; d_bank_ = nullptr; d_bank_yuyv_ = nullptr; d_bank_nv12_ = nullptr; d_src_bg_ = nullptr; d_green_ = nullptr;
+  for (void* p : {(void*)src_state_, (void*)d_bank_, (void*)d_bank_yuyv_, (void*)d_bank_nv12_, (void*)d_src_bg_, (void*)d_pool_bg_, (void*)d_green_})
+    if (p) cudaFree(p);
+  src_state_ = nullptr; d_bank_ = nullptr; d_bank_yuyv_ = nullptr; d_bank_nv12_ = nullptr; d_src_bg_ = nullptr; d_pool_bg_ = nullptr; d_green_ = nullptr;
   n_sources_ = 0;
-  src_has_bg_.clear();
+  pool_slots_ = 0;
+  src_ring_.clear();
   src_fx_.clear();
   src_flip_.clear();
   src_size_.clear();
@@ -1690,7 +1703,7 @@ bool Engine::set_sources(int n_sources, std::string* err) {
     CUDA_OK(cudaMemcpy(d_green_, green.data(), fbytes, cudaMemcpyHostToDevice));
   }
   n_sources_ = n_sources;
-  src_has_bg_.assign((size_t)n_sources, 0);
+  src_ring_.assign((size_t)n_sources, SrcRing{});
   src_fx_.assign((size_t)n_sources, SrcEffect{});
   src_flip_.assign((size_t)n_sources, -1);
   src_size_.assign((size_t)n_sources, -1);
@@ -1724,13 +1737,21 @@ bool Engine::refresh_bank_ctx(std::string* err) {
   return true;
 }
 
-int Engine::source_bg(int s, int* k) const {
+int Engine::source_bg(int s, int* k, size_t* slot) const {
   const SrcEffect& f = src_fx_[s];
+  const SrcRing& r = src_ring_[s];
   *k = f.k < 0 ? bgblur_k_ : f.k;
-  if (f.bg == SRC_BG_DEFAULT && src_has_bg_[s]) return SRC_FROM_SLOT;                          // its own image, blurred with k
-  if (f.bg == SRC_BG_DEFAULT && has_bg_) return *k == bgblur_k_ ? SRC_FROM_CTX : SRC_FROM_SLOT;  // the context image at k
-  if (*k) return SRC_FROM_CAMBLUR;                                                            // no image: its blurred camera frame
-  return has_bg_ ? SRC_FROM_SLOT : SRC_FROM_CTX;         // green (the context slot is green while there is no context image)
+  int from;
+  if (f.bg == SRC_BG_DEFAULT && r.count) from = SRC_FROM_SLOT;                                // its own image, blurred with k
+  else if (f.bg == SRC_BG_DEFAULT && has_bg_) from = *k == bgblur_k_ ? SRC_FROM_CTX : SRC_FROM_SLOT;   // the context image at k
+  else if (*k) from = SRC_FROM_CAMBLUR;                                                       // no image: its blurred camera frame
+  else from = has_bg_ ? SRC_FROM_SLOT : SRC_FROM_CTX;    // green (the context slot is green while there is no context image)
+  if (slot) {
+    if (from == SRC_FROM_CTX) *slot = (size_t)max_batch_;
+    else if (f.bg == SRC_BG_DEFAULT && r.count > 1) *slot = pool0() + r.base + (size_t)r.cursor;   // its ring's current image
+    else *slot = (size_t)max_batch_ + 1 + (size_t)s;
+  }
+  return from;
 }
 
 // d_gauss_tmp_ (16-bit row sums of the row / column Gaussian) for max_batch frames
@@ -1738,35 +1759,46 @@ bool Engine::ensure_gauss_tmp(std::string* err) {
   return ensure((void**)&d_gauss_tmp_, &gauss_tmp_cap_, (size_t)max_batch_ * W_ * H_ * 3 * sizeof(uint16_t), err);
 }
 
-// bank slot of source s when its still background differs from the context slot: its own image, the context image or
-// green, blurred with the source's strength; then its YUYV / NV12
+// bank slots of source s when its still background differs from the context slot: its own image (every image of its
+// ring), the context image or green, blurred with the source's strength; then their YUYV / NV12.  A ring of more than
+// one image fills its pool slots max_batch images at a time (the Gaussian's row sums hold max_batch frames).
 bool Engine::refresh_bank_source(int s, std::string* err) {
   int k = 0;
-  if (source_bg(s, &k) != SRC_FROM_SLOT) return true;
+  size_t slot_i = 0;
+  if (source_bg(s, &k, &slot_i) != SRC_FROM_SLOT) return true;
   const SrcEffect& f = src_fx_[s];
-  const size_t fbytes = (size_t)W_ * H_ * 3, npix = (size_t)W_ * H_, slot_i = (size_t)max_batch_ + 1 + (size_t)s;
-  const uint8_t* src = f.bg != SRC_BG_DEFAULT ? d_green_ : src_has_bg_[s] ? d_src_bg_ + (size_t)s * fbytes : has_bg_ ? d_bg_ : d_green_;
+  const SrcRing& r = src_ring_[s];
+  const size_t fbytes = (size_t)W_ * H_ * 3, npix = (size_t)W_ * H_;
+  const bool own = f.bg == SRC_BG_DEFAULT && r.count, pooled = own && r.count > 1;
+  const int n = pooled ? r.count : 1;
+  if (pooled) slot_i = pool0() + r.base;
+  const uint8_t* src = !own ? (f.bg == SRC_BG_DEFAULT && has_bg_ ? d_bg_ : d_green_)
+                            : pooled ? d_pool_bg_ + r.base * fbytes : d_src_bg_ + (size_t)s * fbytes;
   uint8_t* slot = d_bank_ + slot_i * fbytes;
   if (k) {
     GaussTaps t{};
     gauss_taps(k, &t);
     if (gauss_class(k) == GAUSS_SEPARABLE && !ensure_gauss_tmp(err)) return false;
-    launch_gauss_blur(stream_, 1, src, (size_t)W_ * 3, fbytes, d_gauss_tmp_, slot, (size_t)W_ * 3, fbytes, W_, H_, t);
+    for (int i = 0; i < n; i += max_batch_)
+      launch_gauss_blur(stream_, std::min(max_batch_, n - i), src + (size_t)i * fbytes, (size_t)W_ * 3, fbytes, d_gauss_tmp_, slot + (size_t)i * fbytes,
+                        (size_t)W_ * 3, fbytes, W_, H_, t);
   } else {
-    CUDA_OK(cudaMemcpyAsync(slot, src, fbytes, cudaMemcpyDeviceToDevice, stream_));
+    CUDA_OK(cudaMemcpyAsync(slot, src, (size_t)n * fbytes, cudaMemcpyDeviceToDevice, stream_));
   }
-  if (d_bank_yuyv_) launch_rgb_to_yuyv(stream_, slot, d_bank_yuyv_ + slot_i * npix * 2, npix);
-  if (d_bank_nv12_) launch_yuyv_to_nv12(stream_, 1, d_bank_yuyv_ + slot_i * npix * 2, 0, d_bank_nv12_ + slot_i * npix * 3 / 2, 0, W_, H_);
+  if (d_bank_yuyv_) launch_rgb_to_yuyv(stream_, slot, d_bank_yuyv_ + slot_i * npix * 2, npix, n, fbytes, npix * 2);
+  if (d_bank_nv12_)
+    launch_yuyv_to_nv12(stream_, n, d_bank_yuyv_ + slot_i * npix * 2, npix * 2, d_bank_nv12_ + slot_i * npix * 3 / 2, npix * 3 / 2, W_, H_);
   CUDA_OK(cudaGetLastError());
   return true;
 }
 
-// after a new context background or strength: every source slot except an own image at a fixed strength depends on them
-// (one Gaussian per such source with a strength > 0)
-bool Engine::refresh_bank_sources_after_ctx(std::string* err) {
+// after a new context background or strength: every source slot except an own image (still or ring) at a fixed strength
+// depends on them (one Gaussian per such source image with a strength > 0); own images that follow the context's strength
+// only when it changed
+bool Engine::refresh_bank_sources_after_ctx(bool strength, std::string* err) {
   for (int s = 0; s < n_sources_; ++s) {
     const SrcEffect& f = src_fx_[s];
-    if (f.bg == SRC_BG_DEFAULT && src_has_bg_[s] && f.k >= 0) continue;
+    if (f.bg == SRC_BG_DEFAULT && src_ring_[s].count && (f.k >= 0 || !strength)) continue;
     if (!refresh_bank_source(s, err)) return false;
   }
   return true;
@@ -1883,39 +1915,114 @@ bool Engine::set_source_output(int source, int out_w, int out_h, std::string* er
   return true;
 }
 
-bool Engine::set_source_background(int source, const uint8_t* bg_raw, int bw, int bh, size_t pitch, std::string* err) {
+// Every new source background goes through here (a still is the ring of one image at advance 0).  Checked first, then
+// each buffer the ring needs is allocated before anything is changed, so an error leaves every source as it was.
+bool Engine::set_source_ring(int source, const uint8_t* frames, int count, int bw, int bh, size_t pitch, size_t frame_stride, int advance,
+                             std::string* err) {
   if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
   if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
-  if (!bg_raw) {                                               // later calls blend the context background again
+  SrcRing& r = src_ring_[source];
+  if (!frames) {                                               // later calls blend the context background again
     CUDA_OK(cudaSetDevice(device_));
-    src_has_bg_[source] = 0;
+    if (r.count > 1 && !resize_pool(source, 0, err)) return false;
+    r = SrcRing{};
     if (!refresh_bank_source(source, err)) return false;
     CUDA_OK(cudaStreamSynchronize(stream_));
     return true;
   }
+  if (count < 1) { *err = "background count must be >= 1"; return false; }
   if (bw <= 0 || bh <= 0 || pitch < (size_t)bw * 3) { *err = "invalid background"; return false; }
+  if (count > 1 && frame_stride < pitch * (size_t)(bh - 1) + (size_t)bw * 3) { *err = "background frame stride is smaller than one image"; return false; }
+  if (advance < 0) { *err = "background advance must be >= 0"; return false; }
   CUDA_OK(cudaSetDevice(device_));
+  // decoded images are staged and resized max_batch at a time
+  const int chunk = std::min(count, max_batch_);
   const size_t raw = (size_t)bw * bh * 3, fbytes = (size_t)W_ * H_ * 3;
-  if (raw > src_raw_cap_) {
+  if ((size_t)chunk * raw > src_raw_cap_) {
     CUDA_OK(cudaStreamSynchronize(stream_));
     if (d_src_raw_) cudaFree(d_src_raw_);
     d_src_raw_ = nullptr; src_raw_cap_ = 0;
-    CUDA_OK(cudaMalloc((void**)&d_src_raw_, raw));
-    src_raw_cap_ = raw;
+    CUDA_OK(cudaMalloc((void**)&d_src_raw_, (size_t)chunk * raw));
+    src_raw_cap_ = (size_t)chunk * raw;
   }
   if (bw != src_bg_w_ || bh != src_bg_h_) {
     CUDA_OK(cudaStreamSynchronize(stream_));
+    src_bg_w_ = src_bg_h_ = 0;                                 // until the new tables are in place
     if (!upload_resize_tab(build_resize_tab(bw, bh, W_, H_), &tab_src_, err)) return false;
     src_bg_w_ = bw; src_bg_h_ = bh;
   }
-  CUDA_OK(cudaMemcpy2DAsync(d_src_raw_, (size_t)bw * 3, bg_raw, pitch, (size_t)bw * 3, (size_t)bh, cudaMemcpyHostToDevice, stream_));
-  // app/background.cc:178-194: cv::resize(raw, out, Size(width, height))
-  launch_resize_u8c3(stream_, d_src_raw_, bw, bh, (size_t)bw * 3, d_src_bg_ + (size_t)source * fbytes, W_, H_, (size_t)W_ * 3, tab_src_.tab,
-                     tab_src_.area2x2);
-  src_has_bg_[source] = 1;
+  // a ring of the same count rewrites its slots in place, in stream order; any other change of the pool reallocates it
+  if ((count > 1 || r.count > 1) && count != r.count && !resize_pool(source, count, err)) return false;
+  uint8_t* dst = count > 1 ? d_pool_bg_ + r.base * fbytes : d_src_bg_ + (size_t)source * fbytes;
+  for (int i = 0; i < count; i += chunk) {
+    const int n = std::min(chunk, count - i);
+    for (int j = 0; j < n; ++j)
+      CUDA_OK(cudaMemcpy2DAsync(d_src_raw_ + (size_t)j * raw, (size_t)bw * 3, frames + (size_t)(i + j) * frame_stride, pitch, (size_t)bw * 3,
+                                (size_t)bh, cudaMemcpyHostToDevice, stream_));
+    // app/background.cc:178-194: cv::resize(raw, out, Size(width, height))
+    launch_resize_u8c3(stream_, d_src_raw_, bw, bh, (size_t)bw * 3, dst + (size_t)i * fbytes, W_, H_, (size_t)W_ * 3, tab_src_.tab, tab_src_.area2x2,
+                       n, raw, fbytes);
+  }
+  r.count = count; r.advance = advance; r.cursor = 0;
   if (!refresh_bank_source(source, err)) return false;
   CUDA_OK(cudaStreamSynchronize(stream_));
   CUDA_OK(cudaGetLastError());
+  return true;
+}
+
+bool Engine::set_source_cursor(int source, int index, std::string* err) {
+  if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
+  if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
+  const SrcRing& r = src_ring_[source];
+  if (!r.count) { *err = "the source has no background of its own"; return false; }
+  if (index < 0 || index >= r.count) { *err = "background index out of range"; return false; }
+  src_ring_[source].cursor = index;
+  return true;
+}
+
+bool Engine::resize_pool(int s, int count, std::string* err) {
+  const size_t fbytes = (size_t)W_ * H_ * 3, npix = (size_t)W_ * H_, fixed = pool0();
+  std::vector<size_t> base((size_t)n_sources_, 0);
+  size_t total = 0;
+  for (int i = 0; i < n_sources_; ++i) {
+    const int c = i == s ? count : src_ring_[i].count;
+    if (c > 1) { base[i] = total; total += (size_t)c; }
+  }
+  const size_t slots = fixed + total;
+  uint8_t* bank = nullptr, *yuyv = nullptr, *nv12 = nullptr, *pool = nullptr;
+  cudaError_t e = cudaMalloc((void**)&bank, slots * fbytes);
+  if (e == cudaSuccess && d_bank_yuyv_) e = cudaMalloc((void**)&yuyv, slots * npix * 2);
+  if (e == cudaSuccess && d_bank_nv12_) e = cudaMalloc((void**)&nv12, slots * npix * 3 / 2);
+  if (e == cudaSuccess && total) e = cudaMalloc((void**)&pool, total * fbytes);
+  if (e != cudaSuccess) {
+    for (void* p : {(void*)bank, (void*)yuyv, (void*)nv12, (void*)pool}) if (p) cudaFree(p);
+    cudaGetLastError();
+    *err = std::string("cannot allocate the background bank (") + std::to_string(slots) + " images): " + cudaGetErrorString(e);
+    return false;
+  }
+  // in stream order, behind every queued call that reads the old bank
+  auto copy = [&](uint8_t* dst, const uint8_t* src, size_t bytes, size_t to, size_t from, size_t n) {
+    return cudaMemcpyAsync(dst + to * bytes, src + from * bytes, n * bytes, cudaMemcpyDeviceToDevice, stream_);
+  };
+  CUDA_OK(copy(bank, d_bank_, fbytes, 0, 0, fixed));
+  if (yuyv) CUDA_OK(copy(yuyv, d_bank_yuyv_, npix * 2, 0, 0, fixed));
+  if (nv12) CUDA_OK(copy(nv12, d_bank_nv12_, npix * 3 / 2, 0, 0, fixed));
+  for (int i = 0; i < n_sources_; ++i) {
+    const SrcRing& r = src_ring_[i];
+    if (i == s || r.count < 2) continue;
+    const size_t n = (size_t)r.count;
+    CUDA_OK(copy(bank, d_bank_, fbytes, fixed + base[i], fixed + r.base, n));
+    if (yuyv) CUDA_OK(copy(yuyv, d_bank_yuyv_, npix * 2, fixed + base[i], fixed + r.base, n));
+    if (nv12) CUDA_OK(copy(nv12, d_bank_nv12_, npix * 3 / 2, fixed + base[i], fixed + r.base, n));
+    CUDA_OK(copy(pool, d_pool_bg_, fbytes, base[i], r.base, n));
+  }
+  CUDA_OK(cudaStreamSynchronize(stream_));
+  drop_graphs();                                  // captured launches hold the old bank's base and tensor maps
+  for (void* p : {(void*)d_bank_, (void*)d_bank_yuyv_, (void*)d_bank_nv12_, (void*)d_pool_bg_}) if (p) cudaFree(p);
+  d_bank_ = bank; d_bank_yuyv_ = yuyv; d_bank_nv12_ = nv12; d_pool_bg_ = pool;
+  pool_slots_ = total;
+  for (int i = 0; i < n_sources_; ++i) src_ring_[i].base = base[i];
+  src_ring_[s].count = std::max(count, 0); src_ring_[s].cursor = 0;   // the layout's count; the caller fills the images
   return true;
 }
 

@@ -117,8 +117,18 @@ class Engine {
   // states and the per-source background bank (again: everything reallocated and zeroed, graphs dropped).
   bool set_sources(int n_sources, std::string* err);
   bool reset_source(int source, std::string* err);
-  // cv::resize(raw -> W x H) into the source's bank slot (+ bgblur, + its YUYV); bg_raw == nullptr clears the slot
-  bool set_source_background(int source, const uint8_t* bg_raw, int bw, int bh, size_t pitch, std::string* err);
+  // cv::resize(raw -> W x H) into the source's bank slot (+ bgblur, + its YUYV); bg_raw == nullptr clears the slot.  The
+  // ring of one image at advance 0.
+  bool set_source_background(int source, const uint8_t* bg_raw, int bw, int bh, size_t pitch, std::string* err) {
+    return set_source_ring(source, bg_raw, 1, bw, bh, pitch, 0, 0, err);
+  }
+  // animated background of one source (app/background.cc:126-194): `count` decoded images resized into the bank (one: the
+  // source's own slot; more: the ring pool), blurred at the source's strength; each call carrying a frame of the source
+  // blends ring image `cursor`, then moves the cursor on by `advance`.  frames == nullptr clears the source's background.
+  bool set_source_ring(int source, const uint8_t* frames, int count, int bw, int bh, size_t pitch, size_t frame_stride, int advance,
+                       std::string* err);
+  // host bookkeeping only: the cursor reaches the device with the next call's source table
+  bool set_source_cursor(int source, int index, std::string* err);
   // background effect of one source (include/backscrub_b200.h): background SRC_BG_DEFAULT / SRC_BG_NONE, bgblur -1 (follow
   // the context), 0 or odd 1..255
   enum { SRC_BG_DEFAULT = 0, SRC_BG_NONE = 1 };
@@ -358,27 +368,41 @@ class Engine {
   TailGeo ctx_geo() const;
   bool upload_geo(int slot, const TailGeo& g, std::string* err);
   // background bank, one base + one stride for the post kernel: [max_batch] camera-blur slots | [1] the context's effective
-  // background | [n_sources] source slots; d_bank_yuyv_ is its YUYV and d_bank_nv12_ its NV12 (the camera-blur slots'
-  // are written by the Gaussian of the call, in the call's video format)
+  // background | [n_sources] source slots | [pool_slots_] the ring pool, the images of every source ring of more than one
+  // image; d_bank_yuyv_ is its YUYV and d_bank_nv12_ its NV12 (the camera-blur slots' are written by the Gaussian of the
+  // call, in the call's video format)
   uint8_t* d_bank_ = nullptr, *d_bank_yuyv_ = nullptr, *d_bank_nv12_ = nullptr;
   uint8_t* d_src_bg_ = nullptr;      // [n_sources] resized, unblurred source backgrounds (re-blurred when their strength changes)
+  uint8_t* d_pool_bg_ = nullptr;     // [pool_slots_] the same for the ring pool
+  size_t pool_slots_ = 0;
   uint8_t* d_green_ = nullptr;       // one plain green frame (the still background of a source without an image)
   uint8_t* d_src_raw_ = nullptr;     // staging of one decoded source background
   size_t src_raw_cap_ = 0;
   DevResizeTab tab_src_;
   int src_bg_w_ = 0, src_bg_h_ = 0;
-  std::vector<char> src_has_bg_;
+  // own background of source s: count 0 none, 1 a still in its own slot, more a ring in the pool from bank slot
+  // pool0() + base; it blends ring image `cursor`, and every call carrying a frame of s moves the cursor on by `advance`
+  struct SrcRing { int count = 0, advance = 0, cursor = 0; size_t base = 0; };
+  std::vector<SrcRing> src_ring_;
+  size_t pool0() const { return (size_t)max_batch_ + 1 + (size_t)n_sources_; }
+  // the pool with source s's ring replaced by one of `count` images (none when count <= 1); false with *err, and nothing
+  // changed, when an allocation is refused
+  bool resize_pool(int s, int count, std::string* err);
+  void move_cursors(const Call& c);
   struct SrcEffect { int bg = SRC_BG_DEFAULT, k = -1; };
   std::vector<SrcEffect> src_fx_;
   std::vector<signed char> src_flip_;   // per source: -1 = the context's flips (flip_h_ / flip_v_), else 0..3
   // Where source s's background comes from: the context slot, its own bank slot (its effective still background differs
-  // from the context's), or its camera frame blurred at strength *k
+  // from the context's) or the slot of its ring's current image, or its camera frame blurred at strength *k.  *slot: the
+  // bank slot the source blends now (not set for camera blur, whose slot is the frame's)
   enum SrcBg { SRC_FROM_CTX = 0, SRC_FROM_SLOT = 1, SRC_FROM_CAMBLUR = 2 };
-  int source_bg(int s, int* k) const;
-  int bank_slots() const { return max_batch_ + 1 + n_sources_; }
+  int source_bg(int s, int* k, size_t* slot = nullptr) const;
+  int bank_slots() const { return (int)(pool0() + pool_slots_); }
   bool refresh_bank_ctx(std::string* err);
   bool refresh_bank_source(int s, std::string* err);
-  bool refresh_bank_sources_after_ctx(std::string* err);   // every source slot that depends on the context background / strength
+  // every source slot that depends on the context background / strength (strength: the context's strength changed, so
+  // own images that follow it are re-blurred too)
+  bool refresh_bank_sources_after_ctx(bool strength, std::string* err);
   bool ensure_gauss_tmp(std::string* err);
   void free_sources();
 

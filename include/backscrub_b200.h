@@ -195,9 +195,40 @@ BSB_API int bsb_set_sources(bsb_ctx* ctx, int n_sources);
 /* Zeroes one source's smoother state: the source starts over as a new camera. */
 BSB_API int bsb_reset_source(bsb_ctx* ctx, int source);
 /* bsb_set_background for one source: cv::resize(raw -> W x H) on the GPU (app/background.cc:178-194) into
- * the source's slot, blurred once if bgblur is on.  bg_raw NULL clears the slot (the source blends the
- * context background again).  Video backgrounds: call again for each decoded frame. */
+ * the source's slot, blurred once if bgblur is on.  bg_raw NULL clears the slot, or the source's ring (the source blends
+ * the context background again).  The ring of one image at advance 0 (bsb_set_source_background_ring).  Video
+ * backgrounds: bsb_set_source_background_ring. */
 BSB_API int bsb_set_source_background(bsb_ctx* ctx, int source, const uint8_t* bg_raw, int bg_w, int bg_h, size_t bg_pitch);
+/* Animated background of one source: bsb_set_background_ring for one camera of a sources context.  `count` decoded images,
+ * `frame_stride` bytes apart, are resized to W x H on the GPU (app/background.cc:178-194), blurred at the source's
+ * effective strength, and kept on the device with their YUYV / NV12.  The source's cursor starts at 0.  Each sources call
+ * that carries a frame of the source blends ring image cursor, then moves the cursor on by `advance` (mod count).
+ * advance 0 leaves pacing to the caller (bsb_set_source_background_cursor), as the reference paces by wall clock.
+ * Frame b of a sources call, from source s with its own ring, gives exactly the composite, YUYV / NV12 output and mask of a
+ * plain batch-1 context set up with bsb_set_background_ring(same frames, same advance), bsb_set_bgblur(k_s) and
+ * bsb_set_output(flip_s, size_s), with the same cursor moves.  The rules:
+ *   - the cursor moves only for a call that carries a frame of the source and is enqueued; a refused call moves none;
+ *   - the cursor keeps moving while the ring is not blended (BSB_SOURCE_BG_NONE, camera blur), as a video keeps playing;
+ *     back to BSB_SOURCE_BG_DEFAULT, the source resumes at the advanced cursor;
+ *   - the ring follows the source's effective strength: bsb_set_source_effect with a new strength re-blurs it, and
+ *     bsb_set_bgblur re-blurs every ring whose source follows the context (one Gaussian per image);
+ *   - bsb_set_source_background(s, img) is the ring of one image at advance 0 (kept in the source's own bank slot);
+ *     bsb_set_source_background(s, NULL) clears a ring of any count;
+ *   - a ring replaced by one of the same count rewrites its images in place, in stream order (no reallocation, the
+ *     captured graphs are kept): the way to stream decoded frames into a fixed ring.  Any other change of the ring pool (a
+ *     new ring, another count, a cleared ring) allocates the new bank before freeing the old one, copies the other rings
+ *     over, synchronises the context's stream and drops the captured graphs;
+ *   - bsb_reset_source leaves the cursor; bsb_set_sources frees every ring.
+ * Device memory: W*H*6.5 bytes per image (BGR, YUYV and NV12 of the blurred image) plus W*H*3 (the unblurred image kept
+ * for re-blurring).  No bsb_set_sources yet, a source id out of range, NULL frames, count < 1, bg_w / bg_h <= 0,
+ * bg_pitch < bg_w*3, a frame_stride too small for count > 1, advance < 0 or a refused device allocation return 0 with a
+ * bsb_last_error() message and leave the context and every source's background and cursor as they were. */
+BSB_API int bsb_set_source_background_ring(bsb_ctx* ctx, int source, const uint8_t* frames, int count, int bg_w, int bg_h,
+                                           size_t bg_pitch, size_t frame_stride, int advance);
+/* Host bookkeeping only (no device work, no synchronisation), so it may be called per frame: the index reaches the device
+ * with the call's source table.  index in 0..count-1 of the source's own background; a source without an image of its
+ * own, an index out of range, a source id out of range or no bsb_set_sources yet return 0 with a bsb_last_error() message. */
+BSB_API int bsb_set_source_background_cursor(bsb_ctx* ctx, int source, int index);
 /* Background effect of one source.  Frame b of a sources call, from source s, gives exactly the bytes a plain
  * context gives for that camera's stream when set up with the background s would blend (its own image, else the
  * context image, else none) and bsb_set_bgblur(k), k = s's effective strength.
@@ -208,8 +239,9 @@ BSB_API int bsb_set_source_background(bsb_ctx* ctx, int source, const uint8_t* b
  * bgblur:     -1 = follow the context (bsb_set_bgblur, including later changes), 0 = off, odd 1..255.
  * bsb_set_sources resets every source to (DEFAULT, -1).  The camera-blur mode of plain calls stays per context.  An unknown background, an even / out-of-range strength, a source id out of range or no
  * bsb_set_sources yet return 0 with a bsb_last_error() message.
- * Cost: bsb_set_background and bsb_set_bgblur refresh the still background of every source except one with its own
- * image at a fixed strength (a Gaussian for each such source with a strength > 0; nothing is cached by strength). */
+ * Cost: bsb_set_background and bsb_set_bgblur refresh the background of every source except one with its own image (or
+ * ring) at a fixed strength, and bsb_set_background leaves own images that follow the context's strength too: a Gaussian
+ * for each such source image with a strength > 0, every image of a ring (nothing is cached by strength). */
 enum { BSB_SOURCE_BG_DEFAULT = 0, BSB_SOURCE_BG_NONE = 1 };
 BSB_API int bsb_set_source_effect(bsb_ctx* ctx, int source, int background, int bgblur);
 /* Mirroring of one source (cv::flip, app/deepseg.cc:667-673, toggled at run time by the `h` / `v` keys, :785-790).
