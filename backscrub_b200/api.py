@@ -107,6 +107,12 @@ class MaskGen:
         self._lib.bsb_output_size(self._h, C.byref(w), C.byref(h))
         self.out_width, self.out_height = w.value, h.value
 
+    def set_filter(self, active: bool):
+        """the filter switch (the `s` key, app/deepseg.cc:624,639-664): False passes the camera frame through, flipped,
+        resized and converted as usual; the mask is still computed and written and the smoother still advances."""
+        if not self._lib.bsb_set_filter(self._h, int(bool(active))):
+            self._fail("bsb_set_filter")
+
     def background(self) -> np.ndarray:
         out = np.empty((self.height, self.width, 3), np.uint8)
         if not self._lib.bsb_get_background(self._h, _ptr(out), self.width * 3):
@@ -296,6 +302,13 @@ class MaskGen:
         flip = -1 if flip_h is None and flip_v is None else (1 if flip_h else 0) | (2 if flip_v else 0)
         if not self._lib.bsb_set_source_flip(self._h, int(source), flip):
             self._fail("bsb_set_source_flip")
+
+    def set_source_filter(self, source: int, active=None):
+        """filter switch of one source: None = follow set_filter, including later changes; otherwise the source's own
+        (False: its camera frame passes through; its mask and smoother are unaffected)."""
+        v = -1 if active is None else int(bool(active))
+        if not self._lib.bsb_set_source_filter(self._h, int(source), v):
+            self._fail("bsb_set_source_filter")
 
     def set_source_output(self, source: int, out_size=None):
         """virtual-camera size of one source (cv::resize after the flip, app/deepseg.cc:677-679): out_size = (w, h), or

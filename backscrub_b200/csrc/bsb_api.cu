@@ -381,6 +381,13 @@ int bsb_set_output(bsb_ctx* ctx, int flip_h, int flip_v, int out_w, int out_h) {
   return 1;
 }
 
+int bsb_set_filter(bsb_ctx* ctx, int active) {
+  if (!check_ctx(ctx)) return 0;
+  if (active != 0 && active != 1) { report(&ctx->cb, "error: filter must be 0 (off) or 1 (on)"); return 0; }
+  ctx->eng->set_filter(active != 0);
+  return 1;
+}
+
 int bsb_output_size(bsb_ctx* ctx, int* out_w, int* out_h) {
   if (!check_ctx(ctx)) return 0;
   if (out_w) *out_w = ctx->eng->out_w();
@@ -521,6 +528,13 @@ int bsb_set_source_flip(bsb_ctx* ctx, int source, int flip) {
   if (!check_ctx(ctx)) return 0;
   std::string err;
   if (!ctx->eng->set_source_flip(source, flip, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
+int bsb_set_source_filter(bsb_ctx* ctx, int source, int active) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_source_filter(source, active, &err)) { report(&ctx->cb, "error: " + err); return 0; }
   return 1;
 }
 

@@ -894,6 +894,9 @@ bool Engine::upload(std::string* err) {
     bg_cap_ = fpx * 3;
     CUDA_OK(cudaMalloc((void**)&d_bg_cursor_, sizeof(int)));
     CUDA_OK(cudaMemset(d_bg_cursor_, 0, sizeof(int)));
+    const std::vector<int> ones(B, 1);
+    CUDA_OK(cudaMalloc((void**)&d_pass_all_, B * sizeof(int)));
+    CUDA_OK(cudaMemcpy(d_pass_all_, ones.data(), B * sizeof(int), cudaMemcpyHostToDevice));
   }
   out_w_ = W_; out_h_ = H_;
   out_cap_ = B * fpx * 3; yuyv_cap_ = B * fpx * 2;
@@ -940,7 +943,7 @@ Engine::~Engine() {
     if (p) cudaFree(p);
   for (ChainPlan& cp : chains_) if (cp.d_ops) cudaFree(cp.d_ops);
   free_sources();
-  for (void* p : {(void*)d_src_tab_, (void*)d_src_raw_, tab_src_.blob}) if (p) cudaFree(p);
+  for (void* p : {(void*)d_src_tab_, (void*)d_src_raw_, tab_src_.blob, (void*)d_pass_all_}) if (p) cudaFree(p);
   if (h_mask_) cudaFreeHost(h_mask_);
   if (stream_) cudaStreamDestroy(stream_);
 }
@@ -1188,7 +1191,7 @@ PostArgs Engine::post_args(const Call& c, const Plan& p) const {
   if (has_bg_) {
     if (bgblur_k_) a.bg = d_bg_eff_;                       // blurred once, when the background / strength was set
     if (bg_count_ > 1) { a.bg_stride = fbytes; a.bg_cursor = d_bg_cursor_; a.bg_count = bg_count_; a.bg_advance = bg_advance_; }
-  } else if (bgblur_k_ && want_rgb) {
+  } else if (bgblur_k_ && want_rgb && !p.passed) {
     a.bg = d_bg_frames_; a.bg_stride = fbytes;            // the blurred camera frame itself (filled by enqueue_post)
   }
   if (bg_yuyv_valid_ && !(bgblur_k_ && !has_bg_)) { a.bg_yuyv = d_bg_yuyv_; a.bg_nv12 = bg_nv12_valid_ ? d_bg_nv12_ : nullptr; }
@@ -1223,6 +1226,9 @@ PostArgs Engine::post_args(const Call& c, const Plan& p) const {
     a.yuyv = nullptr; a.yuyv_stride = 0;
   }
   a.mask = c.mask; a.mask_stride = c.mask_stride;
+  // frames whose filter is off (app/deepseg.cc:639-664): the post kernel passes their camera frame through.  A call without
+  // any passes no table, and its post kernel runs as before.
+  if (p.passed) a.pass = p.mode == CALL_PLAIN ? d_pass_all_ : d_src_tab_ + 5 * (size_t)max_batch_;
   a.geo_rows = d_tile_geo_; a.geo_cols64 = d_tile_geo_ + geo_nty_; a.geo_cols128 = d_tile_geo_ + geo_nty_ + geo_ntx64_;
   return a;
 }
@@ -1247,7 +1253,7 @@ bool Engine::enqueue_post(const Call& c, const Plan& p) {
     uint8_t* nv = (!p.all_blur && nv12_in) ? d_bank_nv12_ : nullptr;
     launch_gauss_frames(stream_, n, cam, d_src_tab_ + 2 * (size_t)max_batch_, p.gclass, const_cast<uint8_t*>(a.frames), d_gauss_tmp_,
                         d_bank_, yv, nv, W_, H_);
-  } else if (p.mode == CALL_PLAIN && !has_bg_ && bgblur_k_ && want_rgb)
+  } else if (p.mode == CALL_PLAIN && !has_bg_ && bgblur_k_ && want_rgb && !p.passed)
     launch_gauss_blur(stream_, n, a.frames, a.frame_pitch, a.frame_stride, d_gauss_tmp_, d_bg_frames_, (size_t)W_ * 3, fbytes, W_, H_, taps_);
   if (!launch_post(stream_, a)) return false;
   if (ring && bg_advance_) launch_advance_cursor(stream_, d_bg_cursor_, (int)(((long)n * bg_advance_) % bg_count_), bg_count_);
@@ -1275,8 +1281,9 @@ bool Engine::enqueue_post(const Call& c, const Plan& p) {
 // (a sources call's Gaussian reads the wire format itself).  Decided on the call's own outputs.
 bool Engine::yuyv_native(const Call& c, Plan p) const {
   // a sources call whose every frame blurs its camera frame converts every frame to BGR for the Gaussian anyway, and the
-  // post kernel reads BGR frames faster than it converts the wire format
-  const bool camblur = p.mode == CALL_PLAIN ? (bgblur_k_ && !has_bg_) : p.all_blur;
+  // post kernel reads BGR frames faster than it converts the wire format.  A plain call with the filter off has no
+  // Gaussian.
+  const bool camblur = p.mode == CALL_PLAIN ? (bgblur_k_ && !has_bg_ && !p.passed) : p.all_blur;
   if (c.fmt == IN_BGR || camblur) return false;
   p.native = true; p.nv12_staged = false;
   return post_tma_eligible(post_args(c, p));
@@ -1391,12 +1398,16 @@ bool Engine::run(const Call& c, std::string* err) {
   if (c.ids && !n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
   if (n < 1 || n > max_batch_) { *err = "n_frames out of range (1..max_batch)"; return false; }
   Plan p;
+  // a call without a composite or video output is the same whatever the filter switches say (the mask is unaffected)
+  const bool want_rgb = c.out || c.video;
+  p.passed = want_rgb && !c.ids && !filter_;
   std::vector<int> tab;
   if (c.ids) {
     if (has_bg_ && bg_count_ > 1) { *err = "sources calls need a still context background (animate a source with bsb_set_source_background)"; return false; }
     // frame b: state of source ids[b]; background (source_bg) = the context slot, the source's slot, or its camera frame
-    // blurred at the source's strength into camera-blur slot b; flip and geometry = the source's own, else the context's
-    tab.assign(5 * (size_t)max_batch_, 0);
+    // blurred at the source's strength into camera-blur slot b; flip, geometry and filter switch = the source's own, else
+    // the context's.  A frame whose filter is off blends nothing: it adds no Gaussian class and is no camera-blur frame.
+    tab.assign(6 * (size_t)max_batch_, 0);
     int n_blur = 0;
     const int ctx_flip = (flip_h_ ? 1 : 0) | (flip_v_ ? 2 : 0);
     for (int b = 0; b < n; ++b) {
@@ -1407,8 +1418,12 @@ bool Engine::run(const Call& c, std::string* err) {
       tab[b] = id;
       int k = 0;
       size_t slot = 0;
+      const bool off = want_rgb && (src_filter_[id] < 0 ? !filter_ : src_filter_[id] == 0);
+      tab[5 * (size_t)max_batch_ + b] = off ? 1 : 0;
+      p.passed = p.passed || off;
       const int from = source_bg(id, &k, &slot);
-      if (from == SRC_FROM_CAMBLUR) { slot = b; tab[2 * (size_t)max_batch_ + b] = k; p.gclass |= (unsigned)gauss_class(k); ++n_blur; }
+      if (from == SRC_FROM_CAMBLUR) slot = b;
+      if (from == SRC_FROM_CAMBLUR && !off) { tab[2 * (size_t)max_batch_ + b] = k; p.gclass |= (unsigned)gauss_class(k); ++n_blur; }
       tab[(size_t)max_batch_ + b] = (int)slot;
       const int fl = src_flip_[id] < 0 ? ctx_flip : src_flip_[id];
       tab[3 * (size_t)max_batch_ + b] = fl;
@@ -1472,9 +1487,10 @@ bool Engine::run(const Call& c, std::string* err) {
     const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
     cudaGraphDestroy(graph);
     if (ie != cudaSuccess) { cudaGetLastError(); *err = std::string("cudaGraphInstantiate failed: ") + cudaGetErrorString(ie); return false; }
-    it = graphs_.emplace(key, CapturedCall{exec, last_call_launches_}).first;
+    it = graphs_.emplace(key, CapturedCall{exec, last_call_launches_, last_native_}).first;
   }
   last_call_launches_ = it->second.launches;
+  last_native_ = it->second.native;
   CUDA_OK(cudaGraphLaunch(it->second.exec, stream_));
   move_cursors(c);
 #endif
@@ -1664,6 +1680,7 @@ void Engine::free_sources() {
   src_ring_.clear();
   src_fx_.clear();
   src_flip_.clear();
+  src_filter_.clear();
   src_size_.clear();
   for (OwnSize& o : own_sizes_) if (o.tab.blob) cudaFree(o.tab.blob);
   own_sizes_.clear();
@@ -1680,8 +1697,8 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   const size_t fbytes = (size_t)W_ * H_ * 3, npix = (size_t)W_ * H_, opx = (size_t)oh_ * ow_;
   const size_t slots = (size_t)max_batch_ + 1 + (size_t)n_sources;
   if (!d_src_tab_) {
-    CUDA_OK(cudaMalloc((void**)&d_src_tab_, 5 * (size_t)max_batch_ * sizeof(int)));
-    CUDA_OK(cudaMemset(d_src_tab_, 0, 5 * (size_t)max_batch_ * sizeof(int)));
+    CUDA_OK(cudaMalloc((void**)&d_src_tab_, 6 * (size_t)max_batch_ * sizeof(int)));
+    CUDA_OK(cudaMemset(d_src_tab_, 0, 6 * (size_t)max_batch_ * sizeof(int)));
   }
   CUDA_OK(cudaMalloc((void**)&src_state_, (size_t)n_sources * opx));
   CUDA_OK(cudaMemset(src_state_, 0, (size_t)n_sources * opx));
@@ -1706,6 +1723,7 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   src_ring_.assign((size_t)n_sources, SrcRing{});
   src_fx_.assign((size_t)n_sources, SrcEffect{});
   src_flip_.assign((size_t)n_sources, -1);
+  src_filter_.assign((size_t)n_sources, -1);
   src_size_.assign((size_t)n_sources, -1);
   CUDA_OK(cudaMalloc((void**)&d_geo_, (1 + (size_t)n_sources) * sizeof(TailGeo)));
   if (!upload_geo(0, ctx_geo(), err)) return false;
@@ -1826,6 +1844,14 @@ bool Engine::set_source_flip(int source, int flip, std::string* err) {
   if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
   if (flip < -1 || flip > 3) { *err = "source flip must be -1 (follow the context) or 0..3 (BSB_FLIP_H | BSB_FLIP_V)"; return false; }
   src_flip_[source] = (signed char)flip;
+  return true;
+}
+
+bool Engine::set_source_filter(int source, int active, std::string* err) {
+  if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
+  if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
+  if (active < -1 || active > 1) { *err = "source filter must be -1 (follow the context), 0 (off) or 1 (on)"; return false; }
+  src_filter_[source] = (signed char)active;
   return true;
 }
 

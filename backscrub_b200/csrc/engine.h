@@ -110,6 +110,11 @@ class Engine {
   bool set_bgblur(int k, std::string* err);
   // app/deepseg.cc:667-679: cv::flip and cv::resize to the virtual-camera size before the YUYV conversion
   bool set_output(bool flip_h, bool flip_v, int out_w, int out_h, std::string* err);
+  // app/deepseg.cc:624,639-664 (the `s` key): off, a call's composite is the camera frame, flipped, resized and converted as
+  // usual; the mask is still computed and written and the smoother still advances.  Host state only: the switch is part of
+  // the captured call, so toggling replays once both states have been captured.
+  void set_filter(bool active) { filter_ = active; }
+  bool filter() const { return filter_; }
   bool sync(std::string* err);
   bool reset_state(std::string* err);
 
@@ -136,6 +141,9 @@ class Engine {
   // mirroring of one source: -1 follows set_output's flips, 0..3 its own (bit 0 horizontal, bit 1 vertical).  Host
   // bookkeeping only: the flip reaches the device through the per-frame table of each call.
   bool set_source_flip(int source, int flip, std::string* err);
+  // filter switch of one source: -1 follows set_filter, 0 off, 1 on.  Host bookkeeping only: which frames are filtered off
+  // reaches the device through the per-frame table of each call.
+  bool set_source_filter(int source, int active, std::string* err);
   // virtual-camera size of one source: out_w <= 0 and out_h <= 0 follow set_output's size, else both in 1..16384
   bool set_source_output(int source, int out_w, int out_h, std::string* err);
   // the effective size of source s (its own, or the context's); false when s is not a source
@@ -182,7 +190,7 @@ class Engine {
     if (last_call_launches_ > 0) return last_call_launches_;
     int n = 4;
     for (const Step& s : steps_) n += s.launches();
-    if (bgblur_k_ && !has_bg_) n += 2;
+    if (bgblur_k_ && !has_bg_ && filter_) n += 2;
     if (bg_count_ > 1 && bg_advance_) n += 1;
     if (flip_h_ || flip_v_ || out_w_ != W_ || out_h_ != H_) n += 1;   // k_tail
     return n;
@@ -219,6 +227,8 @@ class Engine {
     bool all_blur = false;           // sources: every frame blurs its camera frame (the BGR frames are materialised)
     bool flipped = false;            // sources: some frame is mirrored (the table's flip row is not all 0)
     bool resized = false;            // sources: some frame's output size is not W x H (the table's geometry row)
+    bool passed = false;             // some frame's filter is off (plain: the context's switch; sources: the table's filter
+                                     // row is not all 0); only calls with a composite or video output have one
     bool flip_tail = false;          // ... and the tail mirrors them (k_tail): the call resizes or its post kernel is not k_post_tma
     bool native = false;             // the post stage reads the camera frames (YUYV or NV12) in place, no BGR frame is materialised
     bool nv12_staged = false;        // the NV12 output is converted from a YUYV output staged in d_yuyv_ (k_yuyv_to_nv12): an
@@ -337,6 +347,8 @@ class Engine {
   size_t bg_eff_cap_ = 0, bg_frames_cap_ = 0, gauss_tmp_cap_ = 0;
   bool flip_h_ = false, flip_v_ = false;
   int out_w_ = 0, out_h_ = 0;
+  bool filter_ = true;
+  int* d_pass_all_ = nullptr;        // [max_batch] ones: the filter table of a plain call with the filter off
   uint8_t* d_stage_a_ = nullptr;     // [B][H][W][3] unflipped composites that k_tail reads
   int2* d_tile_geo_ = nullptr;       // k_post_tma patch geometry per tile row | per 64-wide tile column | per 128-wide tile column
   int geo_nty_ = 0, geo_ntx64_ = 0;
@@ -355,9 +367,9 @@ class Engine {
   // ---- independent sources (calls with ids) ----
   int n_sources_ = 0;
   uint8_t* src_state_ = nullptr;     // [n_sources][oh*ow] smoother state per source
-  // [5][max_batch]: source id of frame b | background-bank slot of frame b | camera-blur strength of frame b (0 = none) |
+  // [6][max_batch]: source id of frame b | background-bank slot of frame b | camera-blur strength of frame b (0 = none) |
   // flip code of frame b (bit 0 horizontal, bit 1 vertical; the source's own, or the context's) | geometry slot of frame b
-  // (d_geo_ index), written before each launch
+  // (d_geo_ index) | 1 when frame b's filter is off (the source's own switch, or the context's), written before each launch
   int* d_src_tab_ = nullptr;
   // Output geometries k_tail reads, [1 + n_sources]: slot 0 the context's (set_output), slot 1 + i own size i.  Each own
   // size is kept once, however many sources use it; a slot no source uses any more is reused by the next new size.
@@ -392,6 +404,7 @@ class Engine {
   struct SrcEffect { int bg = SRC_BG_DEFAULT, k = -1; };
   std::vector<SrcEffect> src_fx_;
   std::vector<signed char> src_flip_;   // per source: -1 = the context's flips (flip_h_ / flip_v_), else 0..3
+  std::vector<signed char> src_filter_; // per source: -1 = the context's switch (filter_), else 0 (off) or 1 (on)
   // Where source s's background comes from: the context slot, its own bank slot (its effective still background differs
   // from the context's) or the slot of its ring's current image, or its camera frame blurred at strength *k.  *slot: the
   // bank slot the source blends now (not set for camera blur, whose slot is the frame's)
@@ -408,25 +421,27 @@ class Engine {
 
   // Everything a captured launch sequence bakes into its kernel arguments: the call's buffers and layouts (the stride of
   // an absent output does not matter), and the plan's mode (a plain and a sources graph over the same buffers are
-  // different graphs), Gaussian classes (strengths within them replay), all-blur and flipped (which frames flip is table
-  // data), resized and the largest output size of the sources, which the tail's grid covers (which frame has which size
-  // is table data too).  The rest of the plan is decided from these.
+  // different graphs), Gaussian classes (strengths within them replay), all-blur, flipped and passed (which frames flip or
+  // are filtered off is table data), resized and the largest output size of the sources, which the tail's grid covers
+  // (which frame has which size is table data too).  The rest of the plan is decided from these.
   struct GraphKey {
     int n, fmt; const void* in; size_t pitch, uv, stride;
     const void* out; const void* video; const void* mask; size_t ostride, vstride, mstride;
-    int mode; unsigned gclass; bool all_blur, flipped, resized; long out_px_max;
+    int mode; unsigned gclass; bool all_blur, flipped, resized, passed; long out_px_max;
     GraphKey(const Call& c, const Plan& p, long px_max)
         : n(c.n), fmt(c.fmt), in(c.in), pitch(c.pitch), uv(c.uv), stride(c.stride), out(c.out), video(c.video), mask(c.mask),
           ostride(c.out ? c.out_stride : 0), vstride(c.video ? c.video_stride : 0), mstride(c.mask ? c.mask_stride : 0),
-          mode(p.mode), gclass(p.gclass), all_blur(p.all_blur), flipped(p.flipped), resized(p.resized), out_px_max(px_max) {}
+          mode(p.mode), gclass(p.gclass), all_blur(p.all_blur), flipped(p.flipped), resized(p.resized), passed(p.passed),
+          out_px_max(px_max) {}
     auto tie() const {
       return std::tie(n, fmt, in, pitch, uv, stride, out, video, mask, ostride, vstride, mstride, mode, gclass, all_blur, flipped, resized,
-                      out_px_max);
+                      passed, out_px_max);
     }
     bool operator<(const GraphKey& r) const { return tie() < r.tie(); }
   };
 #ifndef BSB_EMU
-  struct CapturedCall { cudaGraphExec_t exec; int launches; };
+  // a replay restores the launch count and the native flag of its graph: toggling the filter switch alternates graphs
+  struct CapturedCall { cudaGraphExec_t exec; int launches; bool native; };
   std::map<GraphKey, CapturedCall> graphs_;
 #endif
 };

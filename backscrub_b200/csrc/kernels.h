@@ -253,6 +253,10 @@ struct PostArgs {
   // TMA path only: non-null (DEVICE [B]): frame b's out / YUYV / NV12 are written mirrored by flip[b] (bit 0 horizontally,
   // bit 1 vertically; 0 = as is).  The mask is never mirrored.  launch_post refuses it where k_post_tma cannot run.
   const int* flip;
+  // non-null (DEVICE [B]): frame b with pass[b] != 0 has its filter switched off (app/deepseg.cc:624,639-664): its
+  // composite is the camera frame (blend weight 0) and no background is read; its mask is stored as for any frame.  Every
+  // post kernel honours it; each compiles it into separate instantiations, so a call without it runs as before.
+  const int* pass;
 };
 // false (nothing launched) when a.flip is set and k_post_tma cannot take the arguments
 bool launch_post(cudaStream_t s, const PostArgs& a);

@@ -449,13 +449,16 @@ BSB_D void load48(const uint8_t* p, bool fast, Px16& r) {
   }
 }
 
+// PASS: the launch has a filter table (PostArgs::pass), as k_post_fast
+template <bool PASS>
 __global__ void __launch_bounds__(256) k_post(PostArgs a) {
   __shared__ __align__(16) uint8_t Us[PT_UH * PT_US];
   __shared__ __align__(16) unsigned short Vs[PT_H * PT_UW];
   const int b = blockIdx.z;
   const int tx0 = blockIdx.x * PT_W, ty0 = blockIdx.y * PT_H;
   const int tid = threadIdx.x;
-  const bool hits_roi = tx0 < a.roi_x + a.roi_w && tx0 + PT_W > a.roi_x && ty0 < a.roi_y + a.roi_h && ty0 + PT_H > a.roi_y;
+  const bool pass = PASS && __ldg(a.pass + b) != 0;
+  const bool hits_roi = (!pass || a.mask) && tx0 < a.roi_x + a.roi_w && tx0 + PT_W > a.roi_x && ty0 < a.roi_y + a.roi_h && ty0 + PT_H > a.roi_y;
 
   if (hits_roi) {
     // ---- A: upsampled mask tile with halo, reflect-101 at the ROI border ----
@@ -508,21 +511,32 @@ __global__ void __launch_bounds__(256) k_post(PostArgs a) {
 
   // ---- D: blend (+ YUYV, + mask) ----
   const size_t fo = (size_t)b * a.frame_stride + (size_t)y * a.frame_pitch + (size_t)x0 * 3;
-  const size_t bo = bg_frame_offset(a, b) + (size_t)y * a.bg_pitch + (size_t)x0 * 3;
   const bool full = npx == PT_PX;
-  const bool fast_in = full && ((reinterpret_cast<uintptr_t>(a.frames + fo) | reinterpret_cast<uintptr_t>(a.bg + bo)) & 15) == 0;
   Px16 f, g, o;
-  if (full) { load48(a.frames + fo, fast_in, f); load48(a.bg + bo, fast_in, g); }
-  else {
-    uint8_t* fd = reinterpret_cast<uint8_t*>(&f); uint8_t* gd = reinterpret_cast<uint8_t*>(&g);
-    for (int i = 0; i < npx * 3; ++i) { fd[i] = a.frames[fo + i]; gd[i] = a.bg[bo + i]; }
+  if (pass) {
+    // filter off: the camera frame alone, blended at weight 0
+    const bool fast_in = full && (reinterpret_cast<uintptr_t>(a.frames + fo) & 15) == 0;
+    if (full) load48(a.frames + fo, fast_in, f);
+    else {
+      uint8_t* fd = reinterpret_cast<uint8_t*>(&f);
+      for (int i = 0; i < npx * 3; ++i) fd[i] = a.frames[fo + i];
+    }
+    g = f;
+  } else {
+    const size_t bo = bg_frame_offset(a, b) + (size_t)y * a.bg_pitch + (size_t)x0 * 3;
+    const bool fast_in = full && ((reinterpret_cast<uintptr_t>(a.frames + fo) | reinterpret_cast<uintptr_t>(a.bg + bo)) & 15) == 0;
+    if (full) { load48(a.frames + fo, fast_in, f); load48(a.bg + bo, fast_in, g); }
+    else {
+      uint8_t* fd = reinterpret_cast<uint8_t*>(&f); uint8_t* gd = reinterpret_cast<uint8_t*>(&g);
+      for (int i = 0; i < npx * 3; ++i) { fd[i] = a.frames[fo + i]; gd[i] = a.bg[bo + i]; }
+    }
   }
   const uint8_t* fb = reinterpret_cast<const uint8_t*>(&f);
   const uint8_t* gb = reinterpret_cast<const uint8_t*>(&g);
   uint8_t* ob = reinterpret_cast<uint8_t*>(&o);
 #pragma unroll
   for (int i = 0; i < PT_PX; ++i) {
-    const unsigned aw = m[i], bw = 255u - aw;
+    const unsigned aw = blend_weight(pass, m[i]), bw = 255u - aw;
 #pragma unroll
     for (int c = 0; c < 3; ++c) ob[3 * i + c] = (uint8_t)bsb_div255((unsigned)gb[3 * i + c] * aw + (unsigned)fb[3 * i + c] * bw);
   }
@@ -569,7 +583,8 @@ __global__ void __launch_bounds__(256) k_post(PostArgs a) {
 //       16-byte streaming loads / stores.
 // ---------------------------------------------------------------------------
 
-template <bool OUT, bool YUYV>
+// PASS: the launch has a filter table (PostArgs::pass); without one the kernel is compiled without the pass-through
+template <bool OUT, bool YUYV, bool PASS>
 __global__ void __launch_bounds__(256, 4) k_post_fast(PostArgs a) {
   __shared__ __align__(16) unsigned short Hs[PF_RMAX * PF_US];
   __shared__ __align__(16) unsigned short Us[PF_UH * PF_US];
@@ -579,7 +594,9 @@ __global__ void __launch_bounds__(256, 4) k_post_fast(PostArgs a) {
   const int b = blockIdx.z;
   const int tx0 = blockIdx.x * PF_W, ty0 = blockIdx.y * PF_H;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const bool hits_roi = tx0 < a.roi_x + a.roi_w && tx0 + PF_W > a.roi_x && ty0 < a.roi_y + a.roi_h && ty0 + PF_H > a.roi_y;
+  // a frame whose filter is off reads no background, and computes its mask only when the call stores it
+  const bool pass = PASS && __ldg(a.pass + b) != 0;
+  const bool hits_roi = (!pass || a.mask) && tx0 < a.roi_x + a.roi_w && tx0 + PF_W > a.roi_x && ty0 < a.roi_y + a.roi_h && ty0 + PF_H > a.roi_y;
   int tile_const = -1;                       // 255 / 0 when the whole mask tile is known to be constant
   {
     // pull this thread's 48 bytes of camera frame into L2 while the mask tile is being built
@@ -689,7 +706,7 @@ __global__ void __launch_bounds__(256, 4) k_post_fast(PostArgs a) {
     for (int k = 0; k < 3; ++k) {
       const uint4 t = a.frame_l1 ? __ldg(reinterpret_cast<const uint4*>(fp + 16 * k)) : ldg_stream(fp + 16 * k);
       f[4 * k] = t.x; f[4 * k + 1] = t.y; f[4 * k + 2] = t.z; f[4 * k + 3] = t.w;
-      const uint4 s = __ldg(reinterpret_cast<const uint4*>(gp + 16 * k));
+      const uint4 s = pass ? t : __ldg(reinterpret_cast<const uint4*>(gp + 16 * k));
       g[4 * k] = s.x; g[4 * k + 1] = s.y; g[4 * k + 2] = s.z; g[4 * k + 3] = s.w;
     }
   }
@@ -708,6 +725,10 @@ __global__ void __launch_bounds__(256, 4) k_post_fast(PostArgs a) {
     stg_stream(a.mask + (size_t)b * a.mask_stride + (size_t)y * a.W + x0, mv);
   }
   if (!(OUT || YUYV)) return;
+  if (pass) {
+#pragma unroll
+    for (int i = 0; i < PF_PX; ++i) m[i] = blend_weight(true, m[i]);
+  }
 
   // ---- D: blend (+ RGB->YUV) ----
   unsigned o[12], yy[8];
@@ -742,6 +763,14 @@ static bool post_fast_ok(const PostArgs& a) {
 
 bool launch_post_tma(cudaStream_t s, const PostArgs& a);   // kernels_post.cu
 
+template <bool PASS>
+static void launch_post_fast(cudaStream_t s, dim3 grid, const PostArgs& a) {
+  if (a.yuyv && a.out) { auto k = k_post_fast<true, true, PASS>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  else if (a.yuyv) { auto k = k_post_fast<false, true, PASS>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  else if (a.out) { auto k = k_post_fast<true, false, PASS>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  else { auto k = k_post_fast<false, false, PASS>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+}
+
 bool launch_post(cudaStream_t s, const PostArgs& a_in) {
   if (launch_post_tma(s, a_in)) return true;
   // only k_post_tma writes mirrored frames: a flip table it could not take is an error, never unmirrored output
@@ -750,15 +779,14 @@ bool launch_post(cudaStream_t s, const PostArgs& a_in) {
   a.frame_l1 = tuning().post_l1;                 // measurement switch: frame loads allocate in L1
   if (post_fast_ok(a)) {
     dim3 grid((unsigned)ceil_div(a.W, PF_W), (unsigned)ceil_div(a.H, PF_H), (unsigned)a.B);
-    if (a.yuyv && a.out) { auto k = k_post_fast<true, true>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
-    else if (a.yuyv) { auto k = k_post_fast<false, true>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
-    else if (a.out) { auto k = k_post_fast<true, false>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
-    else { auto k = k_post_fast<false, false>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+    if (a.pass) launch_post_fast<true>(s, grid, a);
+    else launch_post_fast<false>(s, grid, a);
     count_launch();
     return true;
   }
   dim3 grid((unsigned)ceil_div(a.W, PT_W), (unsigned)ceil_div(a.H, PT_H), (unsigned)a.B);
-  BSB_LAUNCH(k_post, grid, dim3(256), 0, s, a);
+  if (a.pass) { auto k = k_post<true>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  else { auto k = k_post<false>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
   count_launch();
   return true;
 }

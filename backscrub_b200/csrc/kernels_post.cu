@@ -14,7 +14,9 @@
 //       mixed tile:       the k_post_fast arithmetic on shared-memory operands;
 //   * results are staged in shared memory and leave with TMA stores;
 //   * a frame with a flip code (PostArgs::flip, sources calls) is written mirrored: each thread puts its 16 pixels,
-//     reversed, into the mirrored slot of the staging tiles, and the stores go to the mirrored box.
+//     reversed, into the mirrored slot of the staging tiles, and the stores go to the mirrored box;
+//   * a frame whose filter is off (PostArgs::pass) loads no background: every tile loads the camera tile and takes the
+//     person-tile path, and the mask patch is loaded and classified only when the call stores the mask.
 // Arithmetic is shared with k_post_fast through post_math.h, so both kernels produce the oracle's bits.
 #include "kernels.h"
 #include "post_math.h"
@@ -135,8 +137,9 @@ template <int TW> struct PtL {
 };
 
 // FMT: IN_BGR / IN_YUYV frames with YUYV video output, or IN_NV12 frames with NV12 video output.  FLIP: the launch has a
-// flip table (sources calls); without one the kernel is compiled without the mirroring paths.
-template <int FMT, int TW, bool FLIP>
+// flip table (sources calls); without one the kernel is compiled without the mirroring paths.  PASS: the launch has a
+// filter table; without one the kernel is compiled without the pass-through paths.
+template <int FMT, int TW, bool FLIP, bool PASS>
 __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const __grid_constant__ PostMapsOf<FMT> tm, const PostArgs a, const PostTmaCfg cfg) {
   using L = PtL<TW>;
   constexpr bool IN_YUYV = FMT == InFmt::IN_YUYV, NV12 = FMT == InFmt::IN_NV12;
@@ -159,6 +162,8 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
   const int ty0 = blockIdx.y * PF_H, tx0 = blockIdx.x * TW;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   int* geo = reinterpret_cast<int*>(smem + L::OFF_GEO);                 // tile geometry, published by thread 0
+  // geo[9]: the frame's flip code, and with PASS its filter-off flag in bit 2
+  auto flip_code = [&]() -> int { return FLIP ? (PASS ? (geo[9] & 3) : geo[9]) : 0; };
 
   // ---- thread 0: geometry of the tile and ALL the loads, before anybody else does anything.  The geometry is uniform
   //      over the CTA: computing it once and publishing it through shared memory takes ~25 instructions off every other
@@ -166,7 +171,9 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
   if (tid == 0) {
     tma::mbar_init(barP, 1); tma::mbar_init(barB, 1); tma::mbar_init(barF, 1);
     tma::fence_barrier_init();
-    const bool hit = tx0 < a.roi_x + a.roi_w && tx0 + TW > a.roi_x && ty0 < a.roi_y + a.roi_h && ty0 + PF_H > a.roi_y;
+    // a filtered-off frame needs the mask patch only for the mask output
+    const bool pass = PASS && __ldg(a.pass + b) != 0;
+    const bool hit = (!pass || cfg.has_mask) && tx0 < a.roi_x + a.roi_w && tx0 + TW > a.roi_x && ty0 < a.roi_y + a.roi_h && ty0 + PF_H > a.roi_y;
     // the patch of the small mask this tile touches comes from two per-context tables (engine.cu): two independent
     // loads whose addresses need nothing but the block index, then the patch request — the head of the CTA's critical
     // path — goes out first ...
@@ -186,19 +193,22 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
     else if (a.bg_cursor) bgi = (int)(((unsigned)__ldg(a.bg_cursor) + (unsigned)b * (unsigned)a.bg_advance) % (unsigned)a.bg_count);
     else if (a.bg_stride) bgi = b;
     if (FLIP) geo[9] = __ldg(a.flip + b);             // the frame's flip code, read by every thread after the first barrier
-    tma::mbar_expect_tx(barB, (unsigned)L::F_BYTES + (cfg.has_bgy ? (NV12 ? (unsigned)L::N_BYTES : (unsigned)L::Y_BYTES) : 0u));
-    tma::load_3d(sB, &tm.bg, blockIdx.x * (TW * 3 / 4), ty0, bgi, barB);
-    if constexpr (NV12) {
-      if (cfg.has_bgy) {
-        tma::load_3d(sY, &tm.bgy, blockIdx.x * (TW / 4), ty0, bgi, barB);
-        tma::load_3d(sY + TW * PF_H, &tm.bgy_uv, blockIdx.x * (TW / 4), ty0 / 2, bgi, barB);
+    if (PASS) geo[9] = (FLIP ? geo[9] : 0) | (pass ? 4 : 0);
+    if (!pass) {                                       // (a filtered-off frame arms no background barrier, nor waits on it)
+      tma::mbar_expect_tx(barB, (unsigned)L::F_BYTES + (cfg.has_bgy ? (NV12 ? (unsigned)L::N_BYTES : (unsigned)L::Y_BYTES) : 0u));
+      tma::load_3d(sB, &tm.bg, blockIdx.x * (TW * 3 / 4), ty0, bgi, barB);
+      if constexpr (NV12) {
+        if (cfg.has_bgy) {
+          tma::load_3d(sY, &tm.bgy, blockIdx.x * (TW / 4), ty0, bgi, barB);
+          tma::load_3d(sY + TW * PF_H, &tm.bgy_uv, blockIdx.x * (TW / 4), ty0 / 2, bgi, barB);
+        }
+      } else {
+        if (cfg.has_bgy) tma::load_3d(sY, &tm.bgy, blockIdx.x * (TW / 2), ty0, bgi, barB);
       }
-    } else {
-      if (cfg.has_bgy) tma::load_3d(sY, &tm.bgy, blockIdx.x * (TW / 2), ty0, bgi, barB);
     }
-    // ... and the camera tile when the tile can contain a person at all: waiting for the classification first would put a
-    // second memory round trip on the critical path of every person / mixed tile
-    if (hit) {
+    // ... and the camera tile when the tile can contain a person at all (every tile of a filtered-off frame): waiting for
+    // the classification first would put a second memory round trip on the critical path of every person / mixed tile
+    if (hit || pass) {
       if constexpr (NV12) {
         tma::mbar_expect_tx(barF, (unsigned)L::N_BYTES);
         tma::load_3d(sF, &tm.frame, blockIdx.x * (TW / 4), ty0, b, barF);
@@ -216,6 +226,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
   __syncthreads();
   const int4 g0 = *reinterpret_cast<const int4*>(geo), g1 = *reinterpret_cast<const int4*>(geo + 4);
   const bool hits_roi = g0.x != 0;
+  const bool pz = PASS && (geo[9] & 4) != 0;            // the frame's filter is off
   const int gy_lo = g0.y, gx_lo = g0.z, rmin = g0.w, nrows = g1.x, cmin = g1.y, ncols = g1.z, coff = g1.w;
 
   const int lx = (tid % (TW / PF_PX)) * PF_PX, ly = tid / (TW / PF_PX);
@@ -316,14 +327,15 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
   // a background tile with a cached YUYV copy is moved by the copy engine alone: only thread 0 (which issues the stores)
   // waits for the background tiles, and for the (speculatively loaded, unused) camera tile after the stores are on their
   // way — shared memory must be quiet when the CTA exits.  A mirrored frame's background tile is reversed by the threads.
-  const bool bg_copy = kind == 0 && !(cfg.has_yuyv && !cfg.has_bgy);
-  const bool engine_only = bg_copy && !(FLIP && geo[9]);
-  if (!engine_only) tma::mbar_wait(barB, 0);
-  if (hits_roi && kind != 0) tma::mbar_wait(barF, 0);
-  if (kind == 0) {
+  // A filtered-off frame's tiles all take the person-tile path on the camera tile, which every one of them loaded.
+  const bool bg_copy = kind == 0 && !pz && !(cfg.has_yuyv && !cfg.has_bgy);
+  const bool engine_only = bg_copy && !(FLIP && flip_code());
+  if (!engine_only && !pz) tma::mbar_wait(barB, 0);
+  if ((hits_roi && kind != 0) || pz) tma::mbar_wait(barF, 0);
+  if (kind == 0 && !pz) {
     // ---- background tile: out = background tile, YUYV = cached YUYV tile, mask = 255.  No per-pixel arithmetic ----
     if (cfg.has_mask) *mdst = make_uint4(0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu);
-    const int fl = FLIP ? geo[9] : 0;
+    const int fl = flip_code();
     if (fl) {
       // mirrored frame: every thread reads its chunk of the staged tiles (the YUYV converted from the background when
       // there is no cached copy), and after a barrier writes it reversed to the mirrored slot — in place, since every
@@ -387,12 +399,13 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
       ydst[0] = make_uint4(yy[0], yy[1], yy[2], yy[3]); ydst[1] = make_uint4(yy[4], yy[5], yy[6], yy[7]);
     }
   } else {
+    // (a filtered-off frame: the mask of any kind of tile, computed only when it is stored; outside the ROI it is 255)
     unsigned m[PF_PX];
     if (kind == 1) {
 #pragma unroll
       for (int i = 0; i < PF_PX; ++i) m[i] = 0u;
-    } else {
-      const bool row_in = y >= a.roi_y && y < a.roi_y + a.roi_h;
+    } else if (!pz || cfg.has_mask) {
+      const bool row_in = (!PASS || hits_roi) && y >= a.roi_y && y < a.roi_y + a.roi_h;
       post_mask16(a, row_in, tile_const, x0, Vs + ly * US + lx, m);
     }
     unsigned f[12], gg[12];
@@ -416,7 +429,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
       f[0] = f0.x; f[1] = f0.y; f[2] = f0.z; f[3] = f0.w; f[4] = f1.x; f[5] = f1.y; f[6] = f1.z; f[7] = f1.w;
       f[8] = f2.x; f[9] = f2.y; f[10] = f2.z; f[11] = f2.w;
     }
-    if (kind == 2) {
+    if (kind == 2 && !pz) {
       const uint4* gq = reinterpret_cast<const uint4*>(sB + ly * (TW * 3) + lx * 3);
       const uint4 g0 = gq[0], g1 = gq[1], g2 = gq[2];
       gg[0] = g0.x; gg[1] = g0.y; gg[2] = g0.z; gg[3] = g0.w; gg[4] = g1.x; gg[5] = g1.y; gg[6] = g1.z; gg[7] = g1.w;
@@ -426,11 +439,14 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
       for (int i = 0; i < 12; ++i) gg[i] = f[i];
     }
     unsigned o[12], yy[8];
-    post_blend16<true, true>(f, gg, m, o, yy);
+    unsigned w[PF_PX];
+#pragma unroll
+    for (int i = 0; i < PF_PX; ++i) w[i] = blend_weight(pz, m[i]);
+    post_blend16<true, true>(f, gg, w, o, yy);
     // the YUYV camera tile is fully consumed before the (wider) BGR tile overwrites it, and a mirrored frame's camera tile
     // before any thread writes another's slot; the mask staging tile reuses Us, whose last readers (phase B) are behind a
     // barrier already
-    const int fl = FLIP ? geo[9] : 0;
+    const int fl = flip_code();
     if (IN_YUYV || NV12 || fl) __syncthreads();
     if (fl) {
       // mirrored frame: the thread's 16 pixels, reversed when horizontal, go to the mirrored slot
@@ -452,8 +468,9 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
       odst[0] = make_uint4(o[0], o[1], o[2], o[3]); odst[1] = make_uint4(o[4], o[5], o[6], o[7]); odst[2] = make_uint4(o[8], o[9], o[10], o[11]);
       ydst[0] = make_uint4(yy[0], yy[1], yy[2], yy[3]); ydst[1] = make_uint4(yy[4], yy[5], yy[6], yy[7]);
     }
-    *mdst = make_uint4(m[0] | (m[1] << 8) | (m[2] << 16) | (m[3] << 24), m[4] | (m[5] << 8) | (m[6] << 16) | (m[7] << 24),
-                       m[8] | (m[9] << 8) | (m[10] << 16) | (m[11] << 24), m[12] | (m[13] << 8) | (m[14] << 16) | (m[15] << 24));
+    if (!pz || cfg.has_mask)
+      *mdst = make_uint4(m[0] | (m[1] << 8) | (m[2] << 16) | (m[3] << 24), m[4] | (m[5] << 8) | (m[6] << 16) | (m[7] << 24),
+                         m[8] | (m[9] << 8) | (m[10] << 16) | (m[11] << 24), m[12] | (m[13] << 8) | (m[14] << 16) | (m[15] << 24));
     out_src = sF;
   }
   const uint8_t* nv_src = sY;          // NV12 calls: the tile the NV12 stores read (the cached background, else sN)
@@ -478,7 +495,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
   // H/2 - ty0/2 - 16).  x stays a multiple of 16 pixels (W % 16 == 0), so every box starts 16-byte aligned.  At ragged
   // edges the mirrored box starts at a negative coordinate: the threads store it, dropping exactly the rows / columns that
   // came from outside the frame.
-  const int fl = FLIP ? geo[9] : 0;
+  const int fl = flip_code();
   const int sx = (fl & 1) ? a.W - tx0 - TW : tx0, sy = (fl & 2) ? a.H - ty0 - PF_H : ty0;
   const bool clipped = FLIP && (sx < 0 || sy < 0);
   if (clipped) {
@@ -508,7 +525,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
     }
     if (cfg.has_mask) tma::store_3d(&tm.mask, sM, tx0, ty0, b);
     tma::store_commit();
-    if (hits_roi && kind == 0) tma::mbar_wait(barF, 0);
+    if (hits_roi && kind == 0 && !pz) tma::mbar_wait(barF, 0);
     tma::store_wait_read();            // shared memory may be handed to the next CTA only after the engine has read it
   }
 }
@@ -616,17 +633,21 @@ bool post_tma_eligible(const PostArgs& a) {
   return post_tma_shape_ok(a) && build_post_maps(a, &tm, post_tile_width(a), &tm);
 }
 
-template <int FMT, int TW, bool FLIP>
+template <int FMT, int TW, bool FLIP, bool PASS>
 static bool launch_post_tma_f(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
   using L = PtL<TW>;
-  if (!ensure_dyn_smem(reinterpret_cast<const void*>(k_post_tma<FMT, TW, FLIP>), L::SMEM)) return false;
+  if (!ensure_dyn_smem(reinterpret_cast<const void*>(k_post_tma<FMT, TW, FLIP, PASS>), L::SMEM)) return false;
   const dim3 grid((unsigned)ceil_div(a.W, TW), (unsigned)ceil_div(a.H, PF_H), (unsigned)a.B);
-  k_post_tma<FMT, TW, FLIP><<<grid, L::NT, L::SMEM, s>>>(tm, a, cfg);
+  k_post_tma<FMT, TW, FLIP, PASS><<<grid, L::NT, L::SMEM, s>>>(tm, a, cfg);
   return true;
+}
+template <int FMT, int TW, bool PASS>
+static bool launch_post_tma_p(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
+  return a.flip ? launch_post_tma_f<FMT, TW, true, PASS>(s, tm, a, cfg) : launch_post_tma_f<FMT, TW, false, PASS>(s, tm, a, cfg);
 }
 template <int FMT, int TW>
 static bool launch_post_tma_t(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
-  return a.flip ? launch_post_tma_f<FMT, TW, true>(s, tm, a, cfg) : launch_post_tma_f<FMT, TW, false>(s, tm, a, cfg);
+  return a.pass ? launch_post_tma_p<FMT, TW, true>(s, tm, a, cfg) : launch_post_tma_p<FMT, TW, false>(s, tm, a, cfg);
 }
 
 bool launch_post_tma(cudaStream_t s, const PostArgs& a) {

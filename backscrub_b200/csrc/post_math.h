@@ -159,6 +159,11 @@ BSB_D void post_mask16(const PostArgs& a, bool row_in, int tile_const, int x0, c
 
 }
 
+// the blend weight of a pixel with mask m: m, or 0 when its frame's filter is off (PostArgs::pass), so that alpha_blend
+// returns the camera byte exactly ((f * 255) / 255 == f) and post_blend16 takes its all-person path.  The stored mask
+// is m either way.
+BSB_D unsigned blend_weight(bool pass, unsigned m) { return pass ? 0u : m; }
+
 // 16 pixels: f / g = frame / background bytes (12 words each), m = masks; o = blended BGR (12 words), yy = YUYV (8 words)
 template <bool OUT, bool YUYV>
 BSB_D void post_blend16(const unsigned* f, const unsigned* g, const unsigned* m, unsigned* o, unsigned* yy) {

@@ -113,6 +113,16 @@ BSB_API int bsb_set_bgblur(bsb_ctx* ctx, int ksize);
  * The flips and the size are the default of every source of a sources call (bsb_set_source_flip, bsb_set_source_output). */
 BSB_API int bsb_set_output(bsb_ctx* ctx, int flip_h, int flip_v, int out_w, int out_h);
 BSB_API int bsb_output_size(bsb_ctx* ctx, int* out_w, int* out_h);
+/* The filter switch (app/deepseg.cc:624,639-664,782-784: the `s` key).  active: 1 = composite (the default), 0 = pass the
+ * camera frame through: the composite is the camera frame (as BGR; YUYV / NV12 frames converted as the fused path converts
+ * them), then the flip, the resize and the YUYV / NV12 conversion of bsb_set_output.  The mask is still computed and
+ * written, byte for byte as with the filter on, and the smoother still advances (:634 feeds every frame), so switching
+ * back on continues a stream that never stopped.  No background is read or blurred for such a frame; a background ring's
+ * cursor still moves.  Every composite entry point honours it (plain calls, and sources calls through the sources that
+ * follow the context, bsb_set_source_filter); bsb_maskgen_process and the bsb_calcmask_* front end produce masks only.
+ * Host state only: the switch is part of the captured call, so once both states of a call have run, toggling replays.
+ * active outside 0..1 returns 0 with a bsb_last_error() message and leaves the context as it was. */
+BSB_API int bsb_set_filter(bsb_ctx* ctx, int active);
 
 /* ---- fused per-frame path: one CUDA-graph launch per call ---------------------------
  * mask generation (bs_maskgen_process) + alpha_blend(bg, frame, mask)
@@ -255,6 +265,17 @@ BSB_API int bsb_set_source_effect(bsb_ctx* ctx, int source, int background, int 
  * bsb_set_sources yet return 0 with a bsb_last_error() message. */
 enum { BSB_FLIP_H = 1, BSB_FLIP_V = 2 };
 BSB_API int bsb_set_source_flip(bsb_ctx* ctx, int source, int flip);
+/* Filter switch of one source (app/deepseg.cc:624,639-664, toggled at run time by the `s` key, :782-784).
+ * active: -1 = follow bsb_set_filter, including later changes; 0 = off; 1 = on.  Frame b of a sources call, from source s,
+ * gives exactly the composite, YUYV / NV12 output and mask of a plain context set up the same way plus
+ * bsb_set_filter(active_s): with the filter off, the camera frame flipped, resized and converted, the mask still written
+ * and the source's smoother still advanced.  Switching one source changes no other frame's bytes.  A frame with its
+ * filter off blends nothing, so a camera-blur source that is off costs no Gaussian.  bsb_set_sources resets every source
+ * to -1.  Host bookkeeping only (no device work, no synchronisation), so it may be called per frame; which frames are off
+ * reaches the device with the call's source table, and a call with some frame off replays one of at most two graphs per
+ * buffer set.  active outside -1..1, a source id out of range or no bsb_set_sources yet return 0 with a bsb_last_error()
+ * message and leave the context as it was. */
+BSB_API int bsb_set_source_filter(bsb_ctx* ctx, int source, int active);
 /* Virtual-camera size of one source (cv::resize after the flip, before the YUYV / NV12 conversion, app/deepseg.cc:667-681).
  * out_w <= 0 and out_h <= 0: follow bsb_set_output's size, including later changes; otherwise both in 1..16384.
  * Frame b of a sources call, from source s, gives exactly the composite, YUYV / NV12 output and mask of a plain context
