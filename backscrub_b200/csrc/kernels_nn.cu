@@ -28,13 +28,20 @@ bool ensure_dyn_smem(const void* func, size_t bytes) {
   (void)func; (void)bytes;
   return true;
 #else
-  if (bytes <= 48 * 1024) return true;
   static std::mutex mu;
   static std::map<std::pair<int, const void*>, size_t> configured;
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return false;
   std::lock_guard<std::mutex> lock(mu);
-  size_t& have = configured[std::make_pair(dev, func)];
+  const auto key = std::make_pair(dev, func);
+  auto it = configured.find(key);
+  if (it == configured.end()) {
+    // without the opt-in attribute a block gets 48 KB of shared memory in all: the kernel's static share plus the dynamic
+    cudaFuncAttributes fa;
+    if (cudaFuncGetAttributes(&fa, func) != cudaSuccess) { cudaGetLastError(); return false; }
+    it = configured.emplace(key, 48 * 1024 - std::min<size_t>(fa.sharedSizeBytes, 48 * 1024)).first;
+  }
+  size_t& have = it->second;
   if (bytes <= have) return true;
   if (cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) != cudaSuccess) { cudaGetLastError(); return false; }
   have = bytes;
@@ -180,6 +187,8 @@ void launch_conv_direct(cudaStream_t s, int B, const float* in, int ih, int iw, 
              pad_t, pad_l, oh, ow, ld_out, to_dev(e)};
   const long total = (long)B * oh * ow * (a.oc4 / 4);
   const size_t smem = sizeof(float) * (size_t)kh * kw * ic * a.oc4;
+  // the planner admits up to 96 KB of weights (engine.cu); above 48 KB the kernel needs the opt-in attribute
+  ensure_dyn_smem(reinterpret_cast<const void*>(k_conv_direct), smem);
   BSB_LAUNCH(k_conv_direct, dim3((unsigned)((total + 255) / 256)), dim3(256), smem, s, a);
   count_launch();
 }
@@ -1187,6 +1196,7 @@ void launch_pool_fc(cudaStream_t s, int B, const float* inA, int cA, int ldA, co
     // one launch: enough blocks per frame to spread the row sums, the last one per frame does the tail
     const int per_frame = h * C;
     int bpf = std::min(ceil_div(per_frame, 256), std::max(1, (device_sms() * 8) / std::max(B, 1)));
+    ensure_dyn_smem(reinterpret_cast<const void*>(k_rowsum_fc), wbytes);
     BSB_LAUNCH(k_rowsum_fc, dim3((unsigned)bpf, (unsigned)B), dim3(256), wbytes, s, inA, cA, ldA, inB, cB, ldB, h, w, rowsum_scratch, counters,
                (float)(h * w), pool_act, n_fc, f[0], f[1], out, ld_out);
     count_launch();
