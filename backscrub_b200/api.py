@@ -47,6 +47,7 @@ class MaskGen:
             raise BackscrubError("".join(self._msgs).strip() or lib.bsb_last_error().decode())
         self.width, self.height, self.max_batch, self.device = width, height, max_batch, device
         self.out_width, self.out_height = width, height
+        self.out_channels = 3                        # bytes per pixel of the `out` frames: 3 (BGR), 4 (BGRA, set_out_format)
         self._n_sources, self._src_out = 0, {}       # sources with their own output size: source -> (w, h)
         r, i, o = (C.c_int * 4)(), (C.c_int * 4)(), (C.c_int * 4)()
         ih, oh = (C.c_int * 3)(), (C.c_int * 3)()
@@ -113,6 +114,17 @@ class MaskGen:
         if not self._lib.bsb_set_filter(self._h, int(bool(active))):
             self._fail("bsb_set_filter")
 
+    def set_out_format(self, fmt: str):
+        """format of the `out` frames of every composite call: "bgr" (the composite, the default) or "bgra" (the camera with
+        alpha 255 - mask, straight alpha, flipped and resized like the composite; the video output and the mask are
+        unchanged).  The wrappers then allocate out as [n, oh, ow, 4], and sources strides count 4 bytes per pixel."""
+        code = {"bgr": 0, "bgra": 1}.get(fmt, -1) if isinstance(fmt, str) else -1
+        if code < 0:
+            raise BackscrubError(f"unknown output format {fmt!r} (\"bgr\" or \"bgra\")")
+        if not self._lib.bsb_set_out_format(self._h, code):
+            self._fail("bsb_set_out_format")
+        self.out_channels = 3 + code
+
     def background(self) -> np.ndarray:
         out = np.empty((self.height, self.width, 3), np.uint8)
         if not self._lib.bsb_get_background(self._h, _ptr(out), self.width * 3):
@@ -128,11 +140,12 @@ class MaskGen:
             raise BackscrubError(f"frame shape {frames.shape[1:]} != {(self.height, self.width, 3)}")
         fb, npx = self.height * self.width * 3, self.height * self.width
         ow, oh = self.out_width, self.out_height
-        out = np.empty((n, oh, ow, 3), np.uint8) if want_out else None
+        oc = self.out_channels
+        out = np.empty((n, oh, ow, oc), np.uint8) if want_out else None
         yuyv = np.empty((n, oh, ow, 2), np.uint8) if want_yuyv else None
         mask = np.empty((n, self.height, self.width), np.uint8) if want_mask else None
         ok = self._lib.bsb_composite(self._h, n, _ptr(frames), self.width * 3, fb,
-                                     _ptr(out) if want_out else None, ow * 3, ow * oh * 3,
+                                     _ptr(out) if want_out else None, ow * oc, ow * oh * oc,
                                      _ptr(yuyv) if want_yuyv else None, ow * oh * 2,
                                      _ptr(mask) if want_mask else None, npx)
         if not ok:
@@ -146,7 +159,7 @@ class MaskGen:
         fb, npx = self.height * self.width * 3, self.height * self.width
         ow, opx = self.out_width, self.out_width * self.out_height
         ok = self._lib.bsb_composite(self._h, n, _ptr(frames), self.width * 3, fb,
-                                     _ptr(out) if out is not None else None, ow * 3, opx * 3,
+                                     _ptr(out) if out is not None else None, ow * self.out_channels, opx * self.out_channels,
                                      _ptr(yuyv) if yuyv is not None else None, opx * 2,
                                      _ptr(mask) if mask is not None else None, npx)
         if not ok:
@@ -157,7 +170,7 @@ class MaskGen:
         n = yuyv_frames.shape[0]
         npx, opx = self.height * self.width, self.out_width * self.out_height
         ok = self._lib.bsb_composite_yuyv(self._h, n, _ptr(yuyv_frames), npx * 2,
-                                          _ptr(out) if out is not None else None, opx * 3,
+                                          _ptr(out) if out is not None else None, opx * self.out_channels,
                                           _ptr(yuyv) if yuyv is not None else None, opx * 2,
                                           _ptr(mask) if mask is not None else None, npx)
         if not ok:
@@ -166,7 +179,7 @@ class MaskGen:
     def composite_yuyv(self, yuyv_frames: np.ndarray):
         yuyv_frames = np.ascontiguousarray(yuyv_frames, np.uint8)
         n = yuyv_frames.shape[0]
-        out = np.empty((n, self.out_height, self.out_width, 3), np.uint8)
+        out = np.empty((n, self.out_height, self.out_width, self.out_channels), np.uint8)
         yuyv = np.empty((n, self.out_height, self.out_width, 2), np.uint8)
         mask = np.empty((n, self.height, self.width), np.uint8)
         self.composite_yuyv_into(yuyv_frames, out, yuyv, mask)
@@ -186,25 +199,25 @@ class MaskGen:
         n = len(bufs)
         ptrs = (C.c_void_p * n)(*[b.ctypes.data for b in bufs])
         sizes = (C.c_size_t * n)(*[b.size for b in bufs])
-        out = np.empty((n, self.out_height, self.out_width, 3), np.uint8)
+        out = np.empty((n, self.out_height, self.out_width, self.out_channels), np.uint8)
         yuyv = np.empty((n, self.out_height, self.out_width, 2), np.uint8)
         mask = np.empty((n, self.height, self.width), np.uint8)
         opx = self.out_width * self.out_height
-        if not self._lib.bsb_composite_mjpg(self._h, n, ptrs, sizes, _ptr(out), opx * 3, _ptr(yuyv), opx * 2, _ptr(mask), self.height * self.width):
+        if not self._lib.bsb_composite_mjpg(self._h, n, ptrs, sizes, _ptr(out), opx * self.out_channels, _ptr(yuyv), opx * 2, _ptr(mask), self.height * self.width):
             self._fail("bsb_composite_mjpg")
         return out, yuyv, mask
 
     def composite_device(self, n, d_frames, d_out=0, d_yuyv=0, d_mask=0, sync=False):
         """Fused path on DEVICE pointers (ints, e.g. torch.Tensor.data_ptr()); tightly packed frames."""
         fb, npx, opx = self.height * self.width * 3, self.height * self.width, self.out_width * self.out_height
-        if not self._lib.bsb_composite_device(self._h, n, d_frames, fb, d_out or None, opx * 3, d_yuyv or None, opx * 2,
+        if not self._lib.bsb_composite_device(self._h, n, d_frames, fb, d_out or None, opx * self.out_channels, d_yuyv or None, opx * 2,
                                               d_mask or None, npx, int(sync)):
             self._fail("bsb_composite_device")
 
     def composite_yuyv_device(self, n, d_yuyv_in, d_out=0, d_yuyv=0, d_mask=0, sync=False):
         """Fused path from DEVICE-resident camera YUYV frames (tightly packed)."""
         npx, opx = self.height * self.width, self.out_width * self.out_height
-        if not self._lib.bsb_composite_yuyv_device(self._h, n, d_yuyv_in, d_out or None, opx * 3, d_yuyv or None, opx * 2,
+        if not self._lib.bsb_composite_yuyv_device(self._h, n, d_yuyv_in, d_out or None, opx * self.out_channels, d_yuyv or None, opx * 2,
                                                    d_mask or None, npx, int(sync)):
             self._fail("bsb_composite_yuyv_device")
 
@@ -223,11 +236,12 @@ class MaskGen:
             raise BackscrubError(f"frame shape {frames.shape[1:]} != {(self.height * 3 // 2, self.width)}")
         npx = self.height * self.width
         ow, oh = self.out_width, self.out_height
-        out = np.empty((n, oh, ow, 3), np.uint8) if want_out else None
+        oc = self.out_channels
+        out = np.empty((n, oh, ow, oc), np.uint8) if want_out else None
         nv12 = np.empty((n, oh * 3 // 2, ow), np.uint8) if want_nv12 else None
         mask = np.empty((n, self.height, self.width), np.uint8) if want_mask else None
         ok = self._lib.bsb_composite_nv12(self._h, n, _ptr(frames), npx * 3 // 2,
-                                          _ptr(out) if want_out else None, ow * oh * 3,
+                                          _ptr(out) if want_out else None, ow * oh * oc,
                                           _ptr(nv12) if want_nv12 else None, ow * oh * 3 // 2,
                                           _ptr(mask) if want_mask else None, npx)
         if not ok:
@@ -239,7 +253,7 @@ class MaskGen:
         BGR / tightly packed NV12 / mask on the device; asynchronous unless `sync`."""
         p, uv, st = self._nv12_layout(pitch, uv_offset, in_stride)
         npx, opx = self.height * self.width, self.out_width * self.out_height
-        if not self._lib.bsb_composite_nv12_device(self._h, n, d_nv12, p, uv, st, d_out or None, opx * 3, d_nv12_out or None, opx * 3 // 2,
+        if not self._lib.bsb_composite_nv12_device(self._h, n, d_nv12, p, uv, st, d_out or None, opx * self.out_channels, d_nv12_out or None, opx * 3 // 2,
                                                    d_mask or None, npx, int(sync)):
             self._fail("bsb_composite_nv12_device")
 
@@ -345,11 +359,12 @@ class MaskGen:
         fb, npx = self.height * self.width * 3, self.height * self.width
         sizes = [self._src_out.get(int(s), (self.out_width, self.out_height)) for s in ids]
         opx = max(w * h for w, h in sizes) if sizes else self.out_width * self.out_height
-        out = np.empty(n * opx * 3, np.uint8) if want_out else None
+        oc = self.out_channels
+        out = np.empty(n * opx * oc, np.uint8) if want_out else None
         yuyv = np.empty(n * opx * 2, np.uint8) if want_yuyv else None
         mask = np.empty((n, self.height, self.width), np.uint8) if want_mask else None
         ok = self._lib.bsb_composite_sources(self._h, n, tab, _ptr(frames), self.width * 3, fb,
-                                             _ptr(out) if want_out else None, opx * 3,
+                                             _ptr(out) if want_out else None, opx * oc,
                                              _ptr(yuyv) if want_yuyv else None, opx * 2,
                                              _ptr(mask) if want_mask else None, npx)
         if not ok:
@@ -362,7 +377,7 @@ class MaskGen:
                 ow, oh = sizes[0]
                 return buf.reshape(n, oh, ow, ch)
             return [buf[b * opx * ch: b * opx * ch + w * h * ch].reshape(h, w, ch) for b, (w, h) in enumerate(sizes)]
-        return shape(out, 3), shape(yuyv, 2), mask
+        return shape(out, oc), shape(yuyv, 2), mask
 
     def composite_sources_yuyv_device(self, n, ids, d_yuyv_in, d_out=0, d_yuyv=0, d_mask=0, sync=False, out_stride=None, yuyv_stride=None):
         """DEVICE-resident camera YUYV frames (tightly packed), frame b of source ids[b]; asynchronous unless `sync`.  Frame b's
@@ -371,7 +386,7 @@ class MaskGen:
         if m != n:
             raise BackscrubError(f"{m} source ids for {n} frames")
         npx, opx = self.height * self.width, self._sources_out_px()
-        ost = opx * 3 if out_stride is None else int(out_stride)
+        ost = opx * self.out_channels if out_stride is None else int(out_stride)
         vst = opx * 2 if yuyv_stride is None else int(yuyv_stride)
         if not self._lib.bsb_composite_sources_yuyv_device(self._h, n, tab, d_yuyv_in, d_out or None, ost, d_yuyv or None, vst,
                                                            d_mask or None, npx, int(sync)):
@@ -386,7 +401,7 @@ class MaskGen:
             raise BackscrubError(f"{m} source ids for {n} frames")
         p, uv, st = self._nv12_layout(pitch, uv_offset, in_stride)
         npx, opx = self.height * self.width, self._sources_out_px()
-        ost = opx * 3 if out_stride is None else int(out_stride)
+        ost = opx * self.out_channels if out_stride is None else int(out_stride)
         vst = opx * 3 // 2 if nv12_stride is None else int(nv12_stride)
         if not self._lib.bsb_composite_sources_nv12_device(self._h, n, tab, d_nv12, p, uv, st, d_out or None, ost, d_nv12_out or None,
                                                            vst, d_mask or None, npx, int(sync)):

@@ -147,8 +147,8 @@ cudaError_t copy_out(const bsb::Call& h, size_t out_pitch, const bsb::Call& d, s
   return r;
 }
 
-// a sources call some of whose frames have their own output size (bsb_set_source_output): each frame's composite and
-// video output back at its own size, packed
+// a sources call some of whose frames have their own output size (bsb_set_source_output): each frame's composite (or
+// BGRA frame) and video output back at its own size, packed
 cudaError_t copy_out_sized(const bsb::Call& h, const bsb::Call& d, const Engine* e, bool nv12, cudaStream_t s) {
   const cudaMemcpyKind k = cudaMemcpyDeviceToHost;
   for (int b = 0; b < h.n; ++b) {
@@ -156,7 +156,7 @@ cudaError_t copy_out_sized(const bsb::Call& h, const bsb::Call& d, const Engine*
     e->source_output_size(h.ids[b], &w, &hh);
     const size_t px = (size_t)w * hh;
     cudaError_t r = cudaSuccess;
-    if (h.out) r = cudaMemcpyAsync(h.out + b * h.out_stride, d.out + b * d.out_stride, px * 3, k, s);
+    if (h.out) r = cudaMemcpyAsync(h.out + b * h.out_stride, d.out + b * d.out_stride, px * e->out_bpp(), k, s);
     if (h.video && r == cudaSuccess) r = cudaMemcpyAsync(h.video + b * h.video_stride, d.video + b * d.video_stride, nv12 ? px * 3 / 2 : px * 2, k, s);
     if (h.mask && r == cudaSuccess) r = cudaMemcpyAsync(h.mask + b * h.mask_stride, d.mask + b * d.mask_stride, d.mask_stride, k, s);
     if (r != cudaSuccess) return r;
@@ -181,7 +181,8 @@ int host_call(bsb_ctx* ctx, const bsb::Call& h, const char* what, const size_t* 
   Engine* e = ctx->eng;
   const FeedConsumed consumed{e};
   const bool bgr = h.fmt == bsb::IN_BGR, nv12 = h.fmt == bsb::IN_NV12;
-  const size_t W = e->W(), H = e->H(), orow = (size_t)e->out_w() * 3, cpx = (size_t)e->out_w() * e->out_h();
+  const size_t bpp = (size_t)e->out_bpp();            // bytes per `out` pixel: 3 (BGR), 4 (BGRA)
+  const size_t W = e->W(), H = e->H(), orow = (size_t)e->out_w() * bpp, cpx = (size_t)e->out_w() * e->out_h();
   // sources calls: the staging holds frames of the largest size any source has; `sized`: some frame's size is its own
   bool sized = false;
   size_t opix = cpx;
@@ -208,7 +209,8 @@ int host_call(bsb_ctx* ctx, const bsb::Call& h, const char* what, const size_t* 
   uint8_t* stage = bgr ? e->d_frames() : e->d_yuyv_in();
   bsb::Call d = h;                                   // the same call on the context staging
   d.in = stage; d.pitch = pitch; d.uv = nv12 ? W * H : 0; d.stride = fbytes;
-  d.out = h.out ? e->d_out() : nullptr; d.out_stride = opix * 3;
+  d.out = h.out ? (bpp == 3 ? e->d_out() : e->out_staging(&err)) : nullptr; d.out_stride = opix * bpp;
+  if (h.out && !d.out) { report(cbp, "error: " + err); return 0; }
   d.video = nullptr; d.video_stride = nv12 ? opix * 3 / 2 : opix * 2;
   if (h.video && !(d.video = nv12 ? e->nv12_staging(&err) : e->d_yuyv())) { report(cbp, "error: " + err); return 0; }
   d.mask = h.mask ? e->d_mask() : nullptr; d.mask_stride = W * H;
@@ -385,6 +387,13 @@ int bsb_set_filter(bsb_ctx* ctx, int active) {
   if (!check_ctx(ctx)) return 0;
   if (active != 0 && active != 1) { report(&ctx->cb, "error: filter must be 0 (off) or 1 (on)"); return 0; }
   ctx->eng->set_filter(active != 0);
+  return 1;
+}
+
+int bsb_set_out_format(bsb_ctx* ctx, int format) {
+  if (!check_ctx(ctx)) return 0;
+  if (format != BSB_OUT_BGR && format != BSB_OUT_BGRA) { report(&ctx->cb, "error: output format must be BSB_OUT_BGR (0) or BSB_OUT_BGRA (1)"); return 0; }
+  ctx->eng->set_out_bgra(format == BSB_OUT_BGRA);
   return 1;
 }
 

@@ -1176,7 +1176,6 @@ void Engine::enqueue_decision(int n, bool sources) {
 PostArgs Engine::post_args(const Call& c, const Plan& p) const {
   const size_t fbytes = (size_t)W_ * H_ * 3;
   const bool tail = call_tail(p);
-  const bool want_rgb = c.out || c.video;
   const bool nv12_in = p.native && c.fmt == IN_NV12;
   PostArgs a{};
   a.B = c.n; a.W = W_; a.H = H_;
@@ -1191,7 +1190,7 @@ PostArgs Engine::post_args(const Call& c, const Plan& p) const {
   if (has_bg_) {
     if (bgblur_k_) a.bg = d_bg_eff_;                       // blurred once, when the background / strength was set
     if (bg_count_ > 1) { a.bg_stride = fbytes; a.bg_cursor = d_bg_cursor_; a.bg_count = bg_count_; a.bg_advance = bg_advance_; }
-  } else if (bgblur_k_ && want_rgb && !p.passed) {
+  } else if (bgblur_k_ && blends(c, p) && !p.passed) {
     a.bg = d_bg_frames_; a.bg_stride = fbytes;            // the blurred camera frame itself (filled by enqueue_post)
   }
   if (bg_yuyv_valid_ && !(bgblur_k_ && !has_bg_)) { a.bg_yuyv = d_bg_yuyv_; a.bg_nv12 = bg_nv12_valid_ ? d_bg_nv12_ : nullptr; }
@@ -1213,7 +1212,8 @@ PostArgs Engine::post_args(const Call& c, const Plan& p) const {
   a.tab = tab_up_.tab; a.area2x2 = tab_up_.area2x2;
   a.out_pitch = (size_t)W_ * 3;
   if (!tail) {
-    a.out = c.out; a.out_stride = c.out_stride;
+    a.out = p.bgra ? nullptr : c.out; a.out_stride = c.out_stride;
+    if (p.bgra) { a.bgra = c.out; a.bgra_pitch = (size_t)W_ * 4; a.bgra_stride = c.out_stride; }
     uint8_t* video = p.nv12_staged ? d_yuyv_ : c.video;
     const size_t vstride = p.nv12_staged ? (size_t)W_ * H_ * 2 : c.video_stride;
     if (nv12_in) { a.nv12 = video; a.nv12_stride = vstride; }
@@ -1222,8 +1222,10 @@ PostArgs Engine::post_args(const Call& c, const Plan& p) const {
     // Without flipped frames no table is passed, and the post kernel runs as for a plain call.
     if (p.mode != CALL_PLAIN && p.flipped) a.flip = d_src_tab_ + 3 * (size_t)max_batch_;
   } else {
-    a.out = want_rgb ? d_stage_a_ : nullptr; a.out_stride = fbytes;
+    // the tail reads the staged BGR composites for the video (and a BGR output), the staged BGRA frames for a BGRA output
+    a.out = blends(c, p) ? d_stage_a_ : nullptr; a.out_stride = fbytes;
     a.yuyv = nullptr; a.yuyv_stride = 0;
+    if (p.bgra) { a.bgra = d_stage_a_ + stage_bgra_off(c, p); a.bgra_pitch = (size_t)W_ * 4; a.bgra_stride = (size_t)W_ * H_ * 4; }
   }
   a.mask = c.mask; a.mask_stride = c.mask_stride;
   // frames whose filter is off (app/deepseg.cc:639-664): the post kernel passes their camera frame through.  A call without
@@ -1243,7 +1245,7 @@ bool Engine::enqueue_post(const Call& c, const Plan& p) {
   // app/deepseg.cc:652-658: no background source => the background is the blurred camera frame itself (sources: frame b
   // at its own strength into the bank's camera-blur slot b, with the slot's YUYV / NV12; the camera frame is read in
   // its wire format when the post kernel reads it so)
-  if (p.mode == CALL_SOURCES_CAMBLUR && want_rgb) {
+  if (p.mode == CALL_SOURCES_CAMBLUR && blends(c, p)) {
     // the slots' cached video format is the one the post kernel copies: NV12 when it reads the NV12 frames in place, else
     // YUYV (also for an NV12 call that falls back to BGR frames)
     const bool nv12_in = p.native && c.fmt == IN_NV12;
@@ -1253,7 +1255,7 @@ bool Engine::enqueue_post(const Call& c, const Plan& p) {
     uint8_t* nv = (!p.all_blur && nv12_in) ? d_bank_nv12_ : nullptr;
     launch_gauss_frames(stream_, n, cam, d_src_tab_ + 2 * (size_t)max_batch_, p.gclass, const_cast<uint8_t*>(a.frames), d_gauss_tmp_,
                         d_bank_, yv, nv, W_, H_);
-  } else if (p.mode == CALL_PLAIN && !has_bg_ && bgblur_k_ && want_rgb && !p.passed)
+  } else if (p.mode == CALL_PLAIN && !has_bg_ && bgblur_k_ && blends(c, p) && !p.passed)
     launch_gauss_blur(stream_, n, a.frames, a.frame_pitch, a.frame_stride, d_gauss_tmp_, d_bg_frames_, (size_t)W_ * 3, fbytes, W_, H_, taps_);
   if (!launch_post(stream_, a)) return false;
   if (ring && bg_advance_) launch_advance_cursor(stream_, d_bg_cursor_, (int)(((long)n * bg_advance_) % bg_count_), bg_count_);
@@ -1263,6 +1265,7 @@ bool Engine::enqueue_post(const Call& c, const Plan& p) {
   TailArgs t{};
   t.n = n; t.W = W_; t.H = H_; t.src = d_stage_a_; t.src_stride = fbytes;
   t.out = c.out; t.out_stride = c.out_stride; t.video = c.video; t.video_stride = c.video_stride;
+  if (p.bgra) { t.bgra = 1; t.src4 = d_stage_a_ + stage_bgra_off(c, p); t.src4_stride = (size_t)W_ * H_ * 4; }
   t.nv12 = c.fmt == IN_NV12 && c.video;     // 2x2 blocks only where an NV12 output (even sizes) is written
   long max_px = (long)out_w_ * out_h_;
   if (p.mode == CALL_PLAIN) {
@@ -1283,7 +1286,7 @@ bool Engine::yuyv_native(const Call& c, Plan p) const {
   // a sources call whose every frame blurs its camera frame converts every frame to BGR for the Gaussian anyway, and the
   // post kernel reads BGR frames faster than it converts the wire format.  A plain call with the filter off has no
   // Gaussian.
-  const bool camblur = p.mode == CALL_PLAIN ? (bgblur_k_ && !has_bg_ && !p.passed) : p.all_blur;
+  const bool camblur = p.mode == CALL_PLAIN ? (bgblur_k_ && !has_bg_ && !p.passed && blends(c, p)) : p.all_blur;
   if (c.fmt == IN_BGR || camblur) return false;
   p.native = true; p.nv12_staged = false;
   return post_tma_eligible(post_args(c, p));
@@ -1311,7 +1314,10 @@ bool Engine::plan_launch(const Call& c, Plan* p, std::string* err) {
     p->flip_tail = !in_place;
   }
   // set_output allocates the staging for a context flip / resize; grown once (dropping the graphs) on first other need
-  if (call_tail(*p) && (c.out || c.video) && !ensure((void**)&d_stage_a_, &stage_a_cap_, (size_t)max_batch_ * W_ * H_ * 3, err))
+  // (BGRA calls: the BGRA frames, after the BGR composites when the call stages those too)
+  const size_t stage_px = (size_t)max_batch_ * W_ * H_;
+  const size_t stage_need = p->bgra ? stage_bgra_off(c, *p) + stage_px * 4 : stage_px * 3;
+  if (call_tail(*p) && (c.out || c.video) && !ensure((void**)&d_stage_a_, &stage_a_cap_, stage_need, err))
     return false;
   decide();
   return true;
@@ -1401,6 +1407,9 @@ bool Engine::run(const Call& c, std::string* err) {
   // a call without a composite or video output is the same whatever the filter switches say (the mask is unaffected)
   const bool want_rgb = c.out || c.video;
   p.passed = want_rgb && !c.ids && !filter_;
+  p.bgra = bgra_ && c.out;
+  // a call that blends nothing (BGRA and mask only) adds no Gaussian class for its camera-blur frames
+  const bool blend = blends(c, p);
   std::vector<int> tab;
   if (c.ids) {
     if (has_bg_ && bg_count_ > 1) { *err = "sources calls need a still context background (animate a source with bsb_set_source_background)"; return false; }
@@ -1423,7 +1432,7 @@ bool Engine::run(const Call& c, std::string* err) {
       p.passed = p.passed || off;
       const int from = source_bg(id, &k, &slot);
       if (from == SRC_FROM_CAMBLUR) slot = b;
-      if (from == SRC_FROM_CAMBLUR && !off) { tab[2 * (size_t)max_batch_ + b] = k; p.gclass |= (unsigned)gauss_class(k); ++n_blur; }
+      if (from == SRC_FROM_CAMBLUR && !off && blend) { tab[2 * (size_t)max_batch_ + b] = k; p.gclass |= (unsigned)gauss_class(k); ++n_blur; }
       tab[(size_t)max_batch_ + b] = (int)slot;
       const int fl = src_flip_[id] < 0 ? ctx_flip : src_flip_[id];
       tab[3 * (size_t)max_batch_ + b] = fl;
@@ -1505,6 +1514,12 @@ void Engine::move_cursors(const Call& c) {
     SrcRing& r = src_ring_[c.ids[b]];
     if (r.count > 1) r.cursor = (int)(((long)r.cursor + r.advance) % r.count);
   }
+}
+
+uint8_t* Engine::out_staging(std::string* err) {
+  const long px = std::max({(long)out_w_ * out_h_, (long)W_ * H_, n_sources_ ? sources_out_px_max() : 0L});
+  if (!ensure((void**)&d_out_, &out_cap_, (size_t)max_batch_ * px * out_bpp(), err)) return nullptr;
+  return d_out_;
 }
 
 uint8_t* Engine::nv12_staging(std::string* err) {
@@ -1889,7 +1904,7 @@ bool Engine::check_source_outputs(const Call& c, std::string* err) const {
     const int i = src_size_[id];
     if (i < 0) continue;                                        // at the context size: checked as a plain call's frames
     const size_t w = (size_t)own_sizes_[i].w, h = (size_t)own_sizes_[i].h;
-    if (c.out && w * h * 3 > c.out_stride) { *err = "a source's output frame does not fit in the output stride"; return false; }
+    if (c.out && w * h * (size_t)out_bpp() > c.out_stride) { *err = "a source's output frame does not fit in the output stride"; return false; }
     if (!c.video) continue;
     if (c.fmt == IN_NV12 && ((w & 1) || (h & 1))) { *err = "NV12 output needs an even output width and height"; return false; }
     if ((c.fmt == IN_NV12 ? w * h * 3 / 2 : w * h / 2 * 4) > c.video_stride) {

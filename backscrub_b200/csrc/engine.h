@@ -80,7 +80,8 @@ struct Call {
   const uint8_t* in = nullptr;
   size_t pitch = 0, uv = 0, stride = 0;   // row pitch, NV12's UV plane offset inside a frame (else 0), frame stride
   const int* ids = nullptr;          // HOST array: frame b belongs to source ids[b] (n distinct ids); null: a plain call
-  uint8_t* out = nullptr; size_t out_stride = 0;       // BGR composite, out_w x out_h (sources: the frame's own), rows out_w*3 bytes
+  uint8_t* out = nullptr; size_t out_stride = 0;       // BGR composite, out_w x out_h (sources: the frame's own), rows out_w*3 bytes;
+                                                       // in the BGRA output format the transparent BGRA frames, rows out_w*4 bytes
   uint8_t* video = nullptr; size_t video_stride = 0;   // tightly packed YUYV, or NV12 when the input is NV12
   uint8_t* mask = nullptr; size_t mask_stride = 0;     // W x H
   bool callbacks = false;            // fire the stage callbacks (the call then runs eagerly, synchronised at each stage)
@@ -115,6 +116,14 @@ class Engine {
   // the captured call, so toggling replays once both states have been captured.
   void set_filter(bool active) { filter_ = active; }
   bool filter() const { return filter_; }
+  // Output format of the `out` buffers (include/backscrub_b200.h, bsb_set_out_format): BGR composites, or straight-alpha
+  // BGRA frames (the camera with alpha 255 - mask, flipped and resized like the composite).  Host state only, like
+  // set_filter: the format is part of the captured call.
+  void set_out_bgra(bool bgra) { bgra_ = bgra; }
+  bool out_bgra() const { return bgra_; }
+  int out_bpp() const { return bgra_ ? 4 : 3; }
+  // device staging of max_batch `out` frames in the current format (host-buffer API), grown on demand; nullptr on error
+  uint8_t* out_staging(std::string* err);
   bool sync(std::string* err);
   bool reset_state(std::string* err);
 
@@ -190,7 +199,7 @@ class Engine {
     if (last_call_launches_ > 0) return last_call_launches_;
     int n = 4;
     for (const Step& s : steps_) n += s.launches();
-    if (bgblur_k_ && !has_bg_ && filter_) n += 2;
+    if (bgblur_k_ && !has_bg_ && filter_ && !bgra_) n += 2;   // (a BGRA call without video blurs nothing)
     if (bg_count_ > 1 && bg_advance_) n += 1;
     if (flip_h_ || flip_v_ || out_w_ != W_ || out_h_ != H_) n += 1;   // k_tail
     return n;
@@ -233,7 +242,13 @@ class Engine {
     bool native = false;             // the post stage reads the camera frames (YUYV or NV12) in place, no BGR frame is materialised
     bool nv12_staged = false;        // the NV12 output is converted from a YUYV output staged in d_yuyv_ (k_yuyv_to_nv12): an
                                      // NV12 call whose post kernel reads BGR frames, without a tail
+    bool bgra = false;               // the call's `out` takes BGRA frames (the context's format, and the call has an out buffer)
   };
+  // the call blends a composite: it has a video output, or a BGR composite output.  A call that does not reads no
+  // background and blurs nothing.
+  static bool blends(const Call& c, const Plan& p) { return c.video || (c.out && !p.bgra); }
+  // where the tail's staged BGRA frames begin in d_stage_a_ (after the staged BGR composites when the call stages them)
+  size_t stage_bgra_off(const Call& c, const Plan& p) const { return blends(c, p) ? (size_t)max_batch_ * W_ * H_ * 3 : 0; }
   // flip_tail, native and nv12_staged (and the tail's staging); false with *err when a buffer cannot be grown
   bool plan_launch(const Call& c, Plan* p, std::string* err);
   void enqueue_pre(const Call& c);
@@ -348,8 +363,9 @@ class Engine {
   bool flip_h_ = false, flip_v_ = false;
   int out_w_ = 0, out_h_ = 0;
   bool filter_ = true;
+  bool bgra_ = false;                // set_out_bgra
   int* d_pass_all_ = nullptr;        // [max_batch] ones: the filter table of a plain call with the filter off
-  uint8_t* d_stage_a_ = nullptr;     // [B][H][W][3] unflipped composites that k_tail reads
+  uint8_t* d_stage_a_ = nullptr;     // [B][H][W][3] unflipped composites that k_tail reads, then [B][H][W][4] BGRA frames (BGRA calls)
   int2* d_tile_geo_ = nullptr;       // k_post_tma patch geometry per tile row | per 64-wide tile column | per 128-wide tile column
   int geo_nty_ = 0, geo_ntx64_ = 0;
   uint8_t* d_bg_yuyv_ = nullptr;     // YUYV of the effective background (ring): all-background tiles are copies
@@ -423,19 +439,19 @@ class Engine {
   // an absent output does not matter), and the plan's mode (a plain and a sources graph over the same buffers are
   // different graphs), Gaussian classes (strengths within them replay), all-blur, flipped and passed (which frames flip or
   // are filtered off is table data), resized and the largest output size of the sources, which the tail's grid covers
-  // (which frame has which size is table data too).  The rest of the plan is decided from these.
+  // (which frame has which size is table data too), and the output format.  The rest of the plan is decided from these.
   struct GraphKey {
     int n, fmt; const void* in; size_t pitch, uv, stride;
     const void* out; const void* video; const void* mask; size_t ostride, vstride, mstride;
-    int mode; unsigned gclass; bool all_blur, flipped, resized, passed; long out_px_max;
+    int mode; unsigned gclass; bool all_blur, flipped, resized, passed; long out_px_max; bool bgra;
     GraphKey(const Call& c, const Plan& p, long px_max)
         : n(c.n), fmt(c.fmt), in(c.in), pitch(c.pitch), uv(c.uv), stride(c.stride), out(c.out), video(c.video), mask(c.mask),
           ostride(c.out ? c.out_stride : 0), vstride(c.video ? c.video_stride : 0), mstride(c.mask ? c.mask_stride : 0),
           mode(p.mode), gclass(p.gclass), all_blur(p.all_blur), flipped(p.flipped), resized(p.resized), passed(p.passed),
-          out_px_max(px_max) {}
+          out_px_max(px_max), bgra(p.bgra) {}
     auto tie() const {
       return std::tie(n, fmt, in, pitch, uv, stride, out, video, mask, ostride, vstride, mstride, mode, gclass, all_blur, flipped, resized,
-                      passed, out_px_max);
+                      passed, out_px_max, bgra);
     }
     bool operator<(const GraphKey& r) const { return tie() < r.tie(); }
   };

@@ -257,6 +257,10 @@ struct PostArgs {
   // composite is the camera frame (blend weight 0) and no background is read; its mask is stored as for any frame.  Every
   // post kernel honours it; each compiles it into separate instantiations, so a call without it runs as before.
   const int* pass;
+  // may be null: the transparent output, straight-alpha BGRA (rows `bgra_pitch` bytes apart, W*4 used): the camera pixel
+  // with alpha 255 - mask, or 255 for a frame whose filter is off.  Written mirrored by `flip` like `out`.  Every post
+  // kernel compiles it into separate instantiations; with neither `out` nor a video output the call reads no background.
+  uint8_t* bgra; size_t bgra_pitch, bgra_stride;
 };
 // false (nothing launched) when a.flip is set and k_post_tma cannot take the arguments
 bool launch_post(cudaStream_t s, const PostArgs& a);
@@ -294,7 +298,7 @@ bool launch_gauss_frames(cudaStream_t s, int n, const GaussSrc& cam, const int* 
 void launch_flip_u8c3(cudaStream_t s, int n, const uint8_t* src, size_t sstride, uint8_t* dst, size_t dstride, int W, int H, bool flip_h, bool flip_v);
 // app/deepseg.cc:667-681 in one launch, the tail of a call whose frames are mirrored or resized outside the post kernel:
 // cv::flip, then cv::resize to the frame's virtual-camera geometry, then the YUYV (or NV12) conversion, from the staged
-// W x H BGR composites.  The flip mirrors each tap's source coordinate and keeps the weights; ow == W and oh == H is a
+// W x H BGR composites (and the BGRA output from the staged BGRA frames, 8UC4).  The flip mirrors each tap's source coordinate and keeps the weights; ow == W and oh == H is a
 // mirrored copy.  Bit-exact against the chain k_flip_u8c3 -> k_resize_u8c3 -> k_rgb_to_yuyv (-> k_yuyv_to_nv12).
 struct TailGeo { int ow, oh; ResizeTab tab; int area2x2; };   // tab: INTER_LINEAR tables W x H -> ow x oh
 struct TailArgs {
@@ -306,6 +310,9 @@ struct TailArgs {
   TailGeo geo; int flip;                   // every frame's geometry and flip code (bit 0 horizontal, bit 1 vertical) ...
   const int* slot; const TailGeo* geos;    // ... unless set: frame b's geometry is geos[slot[b]] (DEVICE)
   const int* flips;                        // ... and its flip code flips[b] (DEVICE)
+  // bgra != 0: `out` is BGRA (tightly packed rows ow*4 bytes), flipped and resized channel by channel from the staged
+  // W x H BGRA frames `src4` (rows W*4 bytes); `src` is then read only for the video output
+  const uint8_t* src4; size_t src4_stride; int bgra;
 };
 // max_px: the largest ow * oh a frame of the call can have (the grid covers it; smaller frames' extra CTAs exit)
 void launch_tail(cudaStream_t s, const TailArgs& a, long max_px);

@@ -449,8 +449,8 @@ BSB_D void load48(const uint8_t* p, bool fast, Px16& r) {
   }
 }
 
-// PASS: the launch has a filter table (PostArgs::pass), as k_post_fast
-template <bool PASS>
+// PASS: the launch has a filter table (PostArgs::pass), BGRA a transparent output (PostArgs::bgra), as k_post_fast
+template <bool PASS, bool BGRA = false>
 __global__ void __launch_bounds__(256) k_post(PostArgs a) {
   __shared__ __align__(16) uint8_t Us[PT_UH * PT_US];
   __shared__ __align__(16) unsigned short Vs[PT_H * PT_UW];
@@ -513,7 +513,8 @@ __global__ void __launch_bounds__(256) k_post(PostArgs a) {
   const size_t fo = (size_t)b * a.frame_stride + (size_t)y * a.frame_pitch + (size_t)x0 * 3;
   const bool full = npx == PT_PX;
   Px16 f, g, o;
-  if (pass) {
+  // (a transparent output without a composite or video output blends nothing: no background is read)
+  if (pass || (BGRA && !a.out && !a.yuyv)) {
     // filter off: the camera frame alone, blended at weight 0
     const bool fast_in = full && (reinterpret_cast<uintptr_t>(a.frames + fo) & 15) == 0;
     if (full) load48(a.frames + fo, fast_in, f);
@@ -534,6 +535,13 @@ __global__ void __launch_bounds__(256) k_post(PostArgs a) {
   const uint8_t* fb = reinterpret_cast<const uint8_t*>(&f);
   const uint8_t* gb = reinterpret_cast<const uint8_t*>(&g);
   uint8_t* ob = reinterpret_cast<uint8_t*>(&o);
+  if (BGRA) {
+    uint8_t* bp = a.bgra + (size_t)b * a.bgra_stride + (size_t)y * a.bgra_pitch + (size_t)x0 * 4;
+    for (int i = 0; i < npx; ++i) {
+      bp[4 * i] = fb[3 * i]; bp[4 * i + 1] = fb[3 * i + 1]; bp[4 * i + 2] = fb[3 * i + 2];
+      bp[4 * i + 3] = (uint8_t)(pass ? 255u : 255u - m[i]);
+    }
+  }
 #pragma unroll
   for (int i = 0; i < PT_PX; ++i) {
     const unsigned aw = blend_weight(pass, m[i]), bw = 255u - aw;
@@ -583,8 +591,9 @@ __global__ void __launch_bounds__(256) k_post(PostArgs a) {
 //       16-byte streaming loads / stores.
 // ---------------------------------------------------------------------------
 
-// PASS: the launch has a filter table (PostArgs::pass); without one the kernel is compiled without the pass-through
-template <bool OUT, bool YUYV, bool PASS>
+// PASS: the launch has a filter table (PostArgs::pass); without one the kernel is compiled without the pass-through.
+// BGRA: the launch writes the transparent output (PostArgs::bgra); without OUT and YUYV it reads no background.
+template <bool OUT, bool YUYV, bool PASS, bool BGRA = false>
 __global__ void __launch_bounds__(256, 4) k_post_fast(PostArgs a) {
   __shared__ __align__(16) unsigned short Hs[PF_RMAX * PF_US];
   __shared__ __align__(16) unsigned short Us[PF_UH * PF_US];
@@ -601,7 +610,7 @@ __global__ void __launch_bounds__(256, 4) k_post_fast(PostArgs a) {
   {
     // pull this thread's 48 bytes of camera frame into L2 while the mask tile is being built
     const int px0 = tx0 + (tid & 7) * PF_PX, py = ty0 + (tid >> 3);
-    if ((OUT || YUYV) && py < a.H && px0 < a.W) prefetch_l2(a.frames + (size_t)b * a.frame_stride + (size_t)py * a.frame_pitch + (size_t)px0 * 3);
+    if ((OUT || YUYV || BGRA) && py < a.H && px0 < a.W) prefetch_l2(a.frames + (size_t)b * a.frame_stride + (size_t)py * a.frame_pitch + (size_t)px0 * 3);
   }
 
   if (hits_roi) {
@@ -699,14 +708,14 @@ __global__ void __launch_bounds__(256, 4) k_post_fast(PostArgs a) {
 
   // ---- issue the streaming loads early ----
   unsigned f[12], g[12];
-  if (OUT || YUYV) {
+  if (OUT || YUYV || BGRA) {
     const uint8_t* fp = a.frames + (size_t)b * a.frame_stride + (size_t)y * a.frame_pitch + (size_t)x0 * 3;
     const uint8_t* gp = a.bg + bg_frame_offset(a, b) + (size_t)y * a.bg_pitch + (size_t)x0 * 3;
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
       const uint4 t = a.frame_l1 ? __ldg(reinterpret_cast<const uint4*>(fp + 16 * k)) : ldg_stream(fp + 16 * k);
       f[4 * k] = t.x; f[4 * k + 1] = t.y; f[4 * k + 2] = t.z; f[4 * k + 3] = t.w;
-      const uint4 s = pass ? t : __ldg(reinterpret_cast<const uint4*>(gp + 16 * k));
+      const uint4 s = (pass || !(OUT || YUYV)) ? t : __ldg(reinterpret_cast<const uint4*>(gp + 16 * k));
       g[4 * k] = s.x; g[4 * k + 1] = s.y; g[4 * k + 2] = s.z; g[4 * k + 3] = s.w;
     }
   }
@@ -723,6 +732,14 @@ __global__ void __launch_bounds__(256, 4) k_post_fast(PostArgs a) {
     mv.z = m[8] | (m[9] << 8) | (m[10] << 16) | (m[11] << 24);
     mv.w = m[12] | (m[13] << 8) | (m[14] << 16) | (m[15] << 24);
     stg_stream(a.mask + (size_t)b * a.mask_stride + (size_t)y * a.W + x0, mv);
+  }
+  if (BGRA) {
+    // (m becomes the blend weights here, as below for a filtered-off frame: the mask is stored already)
+#pragma unroll
+    for (int i = 0; i < PF_PX; ++i) m[i] = blend_weight(pass, m[i]);
+    uint8_t* bp = a.bgra + (size_t)b * a.bgra_stride + (size_t)y * a.bgra_pitch + (size_t)x0 * 4;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) stg_stream(bp + 16 * k, bgra4(f + 3 * k, m + 4 * k, false));
   }
   if (!(OUT || YUYV)) return;
   if (pass) {
@@ -752,6 +769,7 @@ static bool post_fast_ok(const PostArgs& a) {
   if (a.out && (!al16(a.out) || a.out_pitch % 16 || a.out_stride % 16)) return false;
   if (a.yuyv && (!al16(a.yuyv) || a.yuyv_stride % 16)) return false;
   if (a.mask && (!al16(a.mask) || a.mask_stride % 16)) return false;
+  if (a.bgra && (!al16(a.bgra) || a.bgra_pitch % 16 || a.bgra_stride % 16)) return false;
   if (a.ow > 32000 || a.oh > 32000 || a.roi_w < 8 || a.roi_h < 8) return false;
   // source rows touched by one 36-row tile must fit the Hs buffer: ceil(36 * scale) + 2
   const double scale_y = (double)a.out_h / (double)a.roi_h;
@@ -763,12 +781,12 @@ static bool post_fast_ok(const PostArgs& a) {
 
 bool launch_post_tma(cudaStream_t s, const PostArgs& a);   // kernels_post.cu
 
-template <bool PASS>
+template <bool PASS, bool BGRA = false>
 static void launch_post_fast(cudaStream_t s, dim3 grid, const PostArgs& a) {
-  if (a.yuyv && a.out) { auto k = k_post_fast<true, true, PASS>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
-  else if (a.yuyv) { auto k = k_post_fast<false, true, PASS>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
-  else if (a.out) { auto k = k_post_fast<true, false, PASS>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
-  else { auto k = k_post_fast<false, false, PASS>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  if (a.yuyv && a.out) { auto k = k_post_fast<true, true, PASS, BGRA>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  else if (a.yuyv) { auto k = k_post_fast<false, true, PASS, BGRA>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  else if (a.out) { auto k = k_post_fast<true, false, PASS, BGRA>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  else { auto k = k_post_fast<false, false, PASS, BGRA>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
 }
 
 bool launch_post(cudaStream_t s, const PostArgs& a_in) {
@@ -779,13 +797,17 @@ bool launch_post(cudaStream_t s, const PostArgs& a_in) {
   a.frame_l1 = tuning().post_l1;                 // measurement switch: frame loads allocate in L1
   if (post_fast_ok(a)) {
     dim3 grid((unsigned)ceil_div(a.W, PF_W), (unsigned)ceil_div(a.H, PF_H), (unsigned)a.B);
-    if (a.pass) launch_post_fast<true>(s, grid, a);
+    if (a.bgra) { if (a.pass) launch_post_fast<true, true>(s, grid, a); else launch_post_fast<false, true>(s, grid, a); }
+    else if (a.pass) launch_post_fast<true>(s, grid, a);
     else launch_post_fast<false>(s, grid, a);
     count_launch();
     return true;
   }
   dim3 grid((unsigned)ceil_div(a.W, PT_W), (unsigned)ceil_div(a.H, PT_H), (unsigned)a.B);
-  if (a.pass) { auto k = k_post<true>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  if (a.bgra) {
+    if (a.pass) { auto k = k_post<true, true>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+    else { auto k = k_post<false, true>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  } else if (a.pass) { auto k = k_post<true>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
   else { auto k = k_post<false>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
   count_launch();
   return true;
@@ -798,6 +820,8 @@ bool launch_post(cudaStream_t s, const PostArgs& a_in) {
 // INTER_AREA mean (a+b+c+d+2)>>2 when area2x2, else INTER_LINEAR through the tables.  flip (bit 0 horizontally, bit 1
 // vertically) mirrors the image before the resize (app/deepseg.cc:667-679): each tap's source coordinate is mirrored and
 // its weight kept, which is not the same as mirroring the resized image (the fixed-point tables need not be symmetric).
+// CN channels (3, or 4 for the BGRA output): OpenCV resizes channel by channel with the same tables.
+template <int CN = 3>
 BSB_D void resize_px(const uint8_t* src, int sw, int sh, size_t spitch, const ResizeTab& t, bool area2x2, int flip, int dx, int dy,
                      uint8_t* d) {
   if (area2x2) {
@@ -807,7 +831,7 @@ BSB_D void resize_px(const uint8_t* src, int sw, int sh, size_t spitch, const Re
     const uint8_t* s0 = src + (size_t)y0 * spitch;
     const uint8_t* s1 = src + (size_t)y1 * spitch;
 #pragma unroll
-    for (int c = 0; c < 3; ++c) d[c] = (uint8_t)((s0[3 * x0 + c] + s0[3 * x1 + c] + s1[3 * x0 + c] + s1[3 * x1 + c] + 2) >> 2);
+    for (int c = 0; c < CN; ++c) d[c] = (uint8_t)((s0[CN * x0 + c] + s0[CN * x1 + c] + s1[CN * x0 + c] + s1[CN * x1 + c] + 2) >> 2);
     return;
   }
   int sx = __ldg(t.xofs + dx), sx1 = min(sx + 1, sw - 1);
@@ -819,7 +843,7 @@ BSB_D void resize_px(const uint8_t* src, int sw, int sh, size_t spitch, const Re
   const uint8_t* r0 = src + (size_t)y0 * spitch;
   const uint8_t* r1 = src + (size_t)y1 * spitch;
 #pragma unroll
-  for (int c = 0; c < 3; ++c) d[c] = lin_v(lin_h(r0, sx, sx1, 3, c, a0, a1), lin_h(r1, sx, sx1, 3, c, a0, a1), b0, b1);
+  for (int c = 0; c < CN; ++c) d[c] = lin_v(lin_h(r0, sx, sx1, CN, c, a0, a1), lin_h(r1, sx, sx1, CN, c, a0, a1), b0, b1);
 }
 
 __global__ void __launch_bounds__(256) k_resize_u8c3(const uint8_t* src, int sw, int sh, size_t spitch,
@@ -984,16 +1008,20 @@ void launch_yuyv_to_nv12(cudaStream_t s, int n, const uint8_t* yuyv, size_t yuyv
 // odd width a pair spans a row end; a last odd pixel has no pair).  NV12: one thread = one 2x2 block, whose two YUYV
 // words give its Y bytes and UV pair directly.
 // ---------------------------------------------------------------------------
-// pixel (x, y) of frame geometry g: the mirrored copy when g is the staged size, else the mirrored resize
+// pixel (x, y) of frame geometry g: the mirrored copy when g is the staged size, else the mirrored resize (CN channels)
+template <int CN = 3>
 BSB_D void tail_px(const uint8_t* src, int W, int H, const TailGeo& g, int flip, int x, int y, uint8_t* d) {
   if (g.ow == W && g.oh == H) {
-    const uint8_t* s = src + ((size_t)((flip & 2) ? H - 1 - y : y) * W + ((flip & 1) ? W - 1 - x : x)) * 3;
-    d[0] = s[0]; d[1] = s[1]; d[2] = s[2];
+    const uint8_t* s = src + ((size_t)((flip & 2) ? H - 1 - y : y) * W + ((flip & 1) ? W - 1 - x : x)) * CN;
+#pragma unroll
+    for (int c = 0; c < CN; ++c) d[c] = s[c];
   } else {
-    resize_px(src, W, H, (size_t)W * 3, g.tab, g.area2x2 != 0, flip, x, y, d);
+    resize_px<CN>(src, W, H, (size_t)W * CN, g.tab, g.area2x2 != 0, flip, x, y, d);
   }
 }
 
+// BGRA: TailArgs::bgra, the output is the transparent BGRA (from src4; the BGR composite is read for the video only)
+template <bool BGRA>
 __global__ void __launch_bounds__(256) k_tail(TailArgs a) {
   const int b = blockIdx.y;
   const TailGeo g = a.slot ? a.geos[__ldg(a.slot + b)] : a.geo;
@@ -1003,15 +1031,24 @@ __global__ void __launch_bounds__(256) k_tail(TailArgs a) {
   const uint8_t* src = a.src + (size_t)b * a.src_stride;
   uint8_t* out = a.out ? a.out + (size_t)b * a.out_stride : nullptr;
   uint8_t* vid = a.video ? a.video + (size_t)b * a.video_stride : nullptr;
+  const uint8_t* src4 = BGRA ? a.src4 + (size_t)b * a.src4_stride : nullptr;
   if (a.nv12) {
     if (i >= npx / 4) return;
     const int hw = g.ow / 2, x = (int)(i % hw) * 2, y = (int)(i / hw) * 2;
     uint8_t px[12];                                   // (x, y) (x+1, y) | (x, y+1) (x+1, y+1)
-    tail_px(src, a.W, a.H, g, fl, x, y, px);
-    tail_px(src, a.W, a.H, g, fl, x + 1, y, px + 3);
-    tail_px(src, a.W, a.H, g, fl, x, y + 1, px + 6);
-    tail_px(src, a.W, a.H, g, fl, x + 1, y + 1, px + 9);
-    if (out) {
+    if (!BGRA || vid) {
+      tail_px(src, a.W, a.H, g, fl, x, y, px);
+      tail_px(src, a.W, a.H, g, fl, x + 1, y, px + 3);
+      tail_px(src, a.W, a.H, g, fl, x, y + 1, px + 6);
+      tail_px(src, a.W, a.H, g, fl, x + 1, y + 1, px + 9);
+    }
+    if (BGRA && out) {
+      uint8_t* o = out + ((size_t)y * g.ow + x) * 4;
+      tail_px<4>(src4, a.W, a.H, g, fl, x, y, o);
+      tail_px<4>(src4, a.W, a.H, g, fl, x + 1, y, o + 4);
+      tail_px<4>(src4, a.W, a.H, g, fl, x, y + 1, o + (size_t)g.ow * 4);
+      tail_px<4>(src4, a.W, a.H, g, fl, x + 1, y + 1, o + (size_t)g.ow * 4 + 4);
+    } else if (out) {
       uint8_t* o = out + ((size_t)y * g.ow + x) * 3;
 #pragma unroll
       for (int k = 0; k < 6; ++k) { o[k] = px[k]; o[(size_t)g.ow * 3 + k] = px[6 + k]; }
@@ -1023,9 +1060,14 @@ __global__ void __launch_bounds__(256) k_tail(TailArgs a) {
   if (p >= npx) return;
   const bool pair = p + 1 < npx;
   uint8_t px[6];
-  tail_px(src, a.W, a.H, g, fl, (int)(p % g.ow), (int)(p / g.ow), px);
-  if (pair) tail_px(src, a.W, a.H, g, fl, (int)((p + 1) % g.ow), (int)((p + 1) / g.ow), px + 3);
-  if (out) {
+  if (!BGRA || vid) {
+    tail_px(src, a.W, a.H, g, fl, (int)(p % g.ow), (int)(p / g.ow), px);
+    if (pair) tail_px(src, a.W, a.H, g, fl, (int)((p + 1) % g.ow), (int)((p + 1) / g.ow), px + 3);
+  }
+  if (BGRA && out) {
+    tail_px<4>(src4, a.W, a.H, g, fl, (int)(p % g.ow), (int)(p / g.ow), out + 4 * p);
+    if (pair) tail_px<4>(src4, a.W, a.H, g, fl, (int)((p + 1) % g.ow), (int)((p + 1) / g.ow), out + 4 * p + 4);
+  } else if (out) {
     uint8_t* o = out + 3 * p;
     o[0] = px[0]; o[1] = px[1]; o[2] = px[2];
     if (pair) { o[3] = px[3]; o[4] = px[4]; o[5] = px[5]; }
@@ -1043,7 +1085,8 @@ __global__ void __launch_bounds__(256) k_tail(TailArgs a) {
 
 void launch_tail(cudaStream_t s, const TailArgs& a, long max_px) {
   const long threads = (max_px + 1) / 2;
-  BSB_LAUNCH(k_tail, dim3((unsigned)((threads + 255) / 256), (unsigned)a.n), dim3(256), 0, s, a);
+  if (a.bgra) { auto k = k_tail<true>; BSB_LAUNCH(k, dim3((unsigned)((threads + 255) / 256), (unsigned)a.n), dim3(256), 0, s, a); }
+  else { auto k = k_tail<false>; BSB_LAUNCH(k, dim3((unsigned)((threads + 255) / 256), (unsigned)a.n), dim3(256), 0, s, a); }
   count_launch();
 }
 

@@ -16,7 +16,11 @@
 //   * a frame with a flip code (PostArgs::flip, sources calls) is written mirrored: each thread puts its 16 pixels,
 //     reversed, into the mirrored slot of the staging tiles, and the stores go to the mirrored box;
 //   * a frame whose filter is off (PostArgs::pass) loads no background: every tile loads the camera tile and takes the
-//     person-tile path, and the mask patch is loaded and classified only when the call stores the mask.
+//     person-tile path, and the mask patch is loaded and classified only when the call stores the mask;
+//   * a launch with the transparent output (PostArgs::bgra) loads the camera tile of every tile, and background tiles
+//     take the mixed-tile path (the blend of mask 255 is the background, bit for bit); each thread writes its 16 BGRA
+//     pixels (camera bytes, alpha 255 - mask) with 16-byte stores straight from registers, mirrored in place for a
+//     flipped frame.  Without a composite or video output it loads no background at all.
 // Arithmetic is shared with k_post_fast through post_math.h, so both kernels produce the oracle's bits.
 #include "kernels.h"
 #include "post_math.h"
@@ -138,8 +142,9 @@ template <int TW> struct PtL {
 
 // FMT: IN_BGR / IN_YUYV frames with YUYV video output, or IN_NV12 frames with NV12 video output.  FLIP: the launch has a
 // flip table (sources calls); without one the kernel is compiled without the mirroring paths.  PASS: the launch has a
-// filter table; without one the kernel is compiled without the pass-through paths.
-template <int FMT, int TW, bool FLIP, bool PASS>
+// filter table; without one the kernel is compiled without the pass-through paths.  BGRA: the launch writes the
+// transparent output; without it the kernel is compiled without those paths.
+template <int FMT, int TW, bool FLIP, bool PASS, bool BGRA>
 __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const __grid_constant__ PostMapsOf<FMT> tm, const PostArgs a, const PostTmaCfg cfg) {
   using L = PtL<TW>;
   constexpr bool IN_YUYV = FMT == InFmt::IN_YUYV, NV12 = FMT == InFmt::IN_NV12;
@@ -164,6 +169,8 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
   int* geo = reinterpret_cast<int*>(smem + L::OFF_GEO);                 // tile geometry, published by thread 0
   // geo[9]: the frame's flip code, and with PASS its filter-off flag in bit 2
   auto flip_code = [&]() -> int { return FLIP ? (PASS ? (geo[9] & 3) : geo[9]) : 0; };
+  // a transparent output alone blends nothing: no background tile is loaded or waited for
+  const bool bgra_only = BGRA && !cfg.has_out && !cfg.has_yuyv;
 
   // ---- thread 0: geometry of the tile and ALL the loads, before anybody else does anything.  The geometry is uniform
   //      over the CTA: computing it once and publishing it through shared memory takes ~25 instructions off every other
@@ -194,7 +201,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
     else if (a.bg_stride) bgi = b;
     if (FLIP) geo[9] = __ldg(a.flip + b);             // the frame's flip code, read by every thread after the first barrier
     if (PASS) geo[9] = (FLIP ? geo[9] : 0) | (pass ? 4 : 0);
-    if (!pass) {                                       // (a filtered-off frame arms no background barrier, nor waits on it)
+    if (!pass && !bgra_only) {                         // (a filtered-off frame arms no background barrier, nor waits on it)
       tma::mbar_expect_tx(barB, (unsigned)L::F_BYTES + (cfg.has_bgy ? (NV12 ? (unsigned)L::N_BYTES : (unsigned)L::Y_BYTES) : 0u));
       tma::load_3d(sB, &tm.bg, blockIdx.x * (TW * 3 / 4), ty0, bgi, barB);
       if constexpr (NV12) {
@@ -208,7 +215,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
     }
     // ... and the camera tile when the tile can contain a person at all (every tile of a filtered-off frame): waiting for
     // the classification first would put a second memory round trip on the critical path of every person / mixed tile
-    if (hit || pass) {
+    if (hit || pass || BGRA) {
       if constexpr (NV12) {
         tma::mbar_expect_tx(barF, (unsigned)L::N_BYTES);
         tma::load_3d(sF, &tm.frame, blockIdx.x * (TW / 4), ty0, b, barF);
@@ -227,6 +234,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
   const int4 g0 = *reinterpret_cast<const int4*>(geo), g1 = *reinterpret_cast<const int4*>(geo + 4);
   const bool hits_roi = g0.x != 0;
   const bool pz = PASS && (geo[9] & 4) != 0;            // the frame's filter is off
+  const bool nobg = pz || bgra_only;                     // no background tile was loaded
   const int gy_lo = g0.y, gx_lo = g0.z, rmin = g0.w, nrows = g1.x, cmin = g1.y, ncols = g1.z, coff = g1.w;
 
   const int lx = (tid % (TW / PF_PX)) * PF_PX, ly = tid / (TW / PF_PX);
@@ -328,11 +336,11 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
   // waits for the background tiles, and for the (speculatively loaded, unused) camera tile after the stores are on their
   // way — shared memory must be quiet when the CTA exits.  A mirrored frame's background tile is reversed by the threads.
   // A filtered-off frame's tiles all take the person-tile path on the camera tile, which every one of them loaded.
-  const bool bg_copy = kind == 0 && !pz && !(cfg.has_yuyv && !cfg.has_bgy);
+  const bool bg_copy = !BGRA && kind == 0 && !pz && !(cfg.has_yuyv && !cfg.has_bgy);
   const bool engine_only = bg_copy && !(FLIP && flip_code());
-  if (!engine_only && !pz) tma::mbar_wait(barB, 0);
-  if ((hits_roi && kind != 0) || pz) tma::mbar_wait(barF, 0);
-  if (kind == 0 && !pz) {
+  if (!engine_only && !nobg) tma::mbar_wait(barB, 0);
+  if ((hits_roi && kind != 0) || pz || BGRA) tma::mbar_wait(barF, 0);
+  if (!BGRA && kind == 0 && !pz) {
     // ---- background tile: out = background tile, YUYV = cached YUYV tile, mask = 255.  No per-pixel arithmetic ----
     if (cfg.has_mask) *mdst = make_uint4(0xffffffffu, 0xffffffffu, 0xffffffffu, 0xffffffffu);
     const int fl = flip_code();
@@ -405,7 +413,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
 #pragma unroll
       for (int i = 0; i < PF_PX; ++i) m[i] = 0u;
     } else if (!pz || cfg.has_mask) {
-      const bool row_in = (!PASS || hits_roi) && y >= a.roi_y && y < a.roi_y + a.roi_h;
+      const bool row_in = (!(PASS || BGRA) || hits_roi) && y >= a.roi_y && y < a.roi_y + a.roi_h;
       post_mask16(a, row_in, tile_const, x0, Vs + ly * US + lx, m);
     }
     unsigned f[12], gg[12];
@@ -429,7 +437,25 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
       f[0] = f0.x; f[1] = f0.y; f[2] = f0.z; f[3] = f0.w; f[4] = f1.x; f[5] = f1.y; f[6] = f1.z; f[7] = f1.w;
       f[8] = f2.x; f[9] = f2.y; f[10] = f2.z; f[11] = f2.w;
     }
-    if (kind == 2 && !pz) {
+    if (BGRA) {
+      // the transparent output, from the camera bytes before the blend overwrites the tile: straight to global memory,
+      // at the mirrored position of a flipped frame (x0 and W are multiples of 16 pixels, so a run is wholly inside).
+      // The mask is staged first, so that m can turn into the blend weights (alpha = 255 - weight).
+      if (!pz || cfg.has_mask)
+        *mdst = make_uint4(m[0] | (m[1] << 8) | (m[2] << 16) | (m[3] << 24), m[4] | (m[5] << 8) | (m[6] << 16) | (m[7] << 24),
+                           m[8] | (m[9] << 8) | (m[10] << 16) | (m[11] << 24), m[12] | (m[13] << 8) | (m[14] << 16) | (m[15] << 24));
+#pragma unroll
+      for (int i = 0; i < PF_PX; ++i) m[i] = blend_weight(pz, m[i]);
+      const int fl = flip_code();
+      if (x0 < a.W && y < a.H) {
+        uint8_t* bp = a.bgra + (size_t)b * a.bgra_stride + (size_t)((fl & 2) ? a.H - 1 - y : y) * a.bgra_pitch +
+                      (size_t)((fl & 1) ? a.W - PF_PX - x0 : x0) * 4;
+        // pixels 4k..4k+3, reversed into the mirrored quarter of the run when the frame is flipped horizontally
+#pragma unroll
+        for (int k = 0; k < 4; ++k) stg_stream(bp + 16 * ((fl & 1) ? 3 - k : k), bgra4(f + 3 * k, m + 4 * k, (fl & 1) != 0));
+      }
+    }
+    if ((kind == 2 || (BGRA && kind == 0)) && !nobg) {
       const uint4* gq = reinterpret_cast<const uint4*>(sB + ly * (TW * 3) + lx * 3);
       const uint4 g0 = gq[0], g1 = gq[1], g2 = gq[2];
       gg[0] = g0.x; gg[1] = g0.y; gg[2] = g0.z; gg[3] = g0.w; gg[4] = g1.x; gg[5] = g1.y; gg[6] = g1.z; gg[7] = g1.w;
@@ -468,7 +494,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
       odst[0] = make_uint4(o[0], o[1], o[2], o[3]); odst[1] = make_uint4(o[4], o[5], o[6], o[7]); odst[2] = make_uint4(o[8], o[9], o[10], o[11]);
       ydst[0] = make_uint4(yy[0], yy[1], yy[2], yy[3]); ydst[1] = make_uint4(yy[4], yy[5], yy[6], yy[7]);
     }
-    if (!pz || cfg.has_mask)
+    if (!BGRA && (!pz || cfg.has_mask))
       *mdst = make_uint4(m[0] | (m[1] << 8) | (m[2] << 16) | (m[3] << 24), m[4] | (m[5] << 8) | (m[6] << 16) | (m[7] << 24),
                          m[8] | (m[9] << 8) | (m[10] << 16) | (m[11] << 24), m[12] | (m[13] << 8) | (m[14] << 16) | (m[15] << 24));
     out_src = sF;
@@ -525,7 +551,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
     }
     if (cfg.has_mask) tma::store_3d(&tm.mask, sM, tx0, ty0, b);
     tma::store_commit();
-    if (hits_roi && kind == 0 && !pz) tma::mbar_wait(barF, 0);
+    if (!BGRA && hits_roi && kind == 0 && !pz) tma::mbar_wait(barF, 0);
     tma::store_wait_read();            // shared memory may be handed to the next CTA only after the engine has read it
   }
 }
@@ -620,7 +646,8 @@ static bool post_tma_shape_ok(const PostArgs& a) {
   if (a.out && (!al16(a.out) || a.out_pitch % 16 || a.out_stride % 16)) return false;
   if (a.yuyv && (!al16(a.yuyv) || a.yuyv_stride % 16)) return false;
   if (a.mask && (!al16(a.mask) || a.mask_stride % 16)) return false;
-  if (!(a.out || a.yuyv || a.nv12 || a.mask) || !al16(a.ofinal) || a.opitch % 16) return false;
+  if (a.bgra && (!al16(a.bgra) || a.bgra_pitch % 16 || a.bgra_stride % 16)) return false;
+  if (!(a.out || a.yuyv || a.nv12 || a.mask || a.bgra) || !al16(a.ofinal) || a.opitch % 16) return false;
   if (a.ow > 32000 || a.oh > 32000 || a.roi_w < 8 || a.roi_h < 8) return false;
   const double scale_y = (double)a.out_h / (double)a.roi_h, scale_x = (double)a.out_w / (double)a.roi_w;
   const int tw = post_tile_width(a);
@@ -633,28 +660,33 @@ bool post_tma_eligible(const PostArgs& a) {
   return post_tma_shape_ok(a) && build_post_maps(a, &tm, post_tile_width(a), &tm);
 }
 
-template <int FMT, int TW, bool FLIP, bool PASS>
+template <int FMT, int TW, bool FLIP, bool PASS, bool BGRA>
 static bool launch_post_tma_f(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
   using L = PtL<TW>;
-  if (!ensure_dyn_smem(reinterpret_cast<const void*>(k_post_tma<FMT, TW, FLIP, PASS>), L::SMEM)) return false;
+  if (!ensure_dyn_smem(reinterpret_cast<const void*>(k_post_tma<FMT, TW, FLIP, PASS, BGRA>), L::SMEM)) return false;
   const dim3 grid((unsigned)ceil_div(a.W, TW), (unsigned)ceil_div(a.H, PF_H), (unsigned)a.B);
-  k_post_tma<FMT, TW, FLIP, PASS><<<grid, L::NT, L::SMEM, s>>>(tm, a, cfg);
+  k_post_tma<FMT, TW, FLIP, PASS, BGRA><<<grid, L::NT, L::SMEM, s>>>(tm, a, cfg);
   return true;
 }
-template <int FMT, int TW, bool PASS>
+template <int FMT, int TW, bool PASS, bool BGRA>
 static bool launch_post_tma_p(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
-  return a.flip ? launch_post_tma_f<FMT, TW, true, PASS>(s, tm, a, cfg) : launch_post_tma_f<FMT, TW, false, PASS>(s, tm, a, cfg);
+  return a.flip ? launch_post_tma_f<FMT, TW, true, PASS, BGRA>(s, tm, a, cfg) : launch_post_tma_f<FMT, TW, false, PASS, BGRA>(s, tm, a, cfg);
+}
+template <int FMT, int TW, bool BGRA>
+static bool launch_post_tma_b(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
+  return a.pass ? launch_post_tma_p<FMT, TW, true, BGRA>(s, tm, a, cfg) : launch_post_tma_p<FMT, TW, false, BGRA>(s, tm, a, cfg);
 }
 template <int FMT, int TW>
 static bool launch_post_tma_t(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
-  return a.pass ? launch_post_tma_p<FMT, TW, true>(s, tm, a, cfg) : launch_post_tma_p<FMT, TW, false>(s, tm, a, cfg);
+  return a.bgra ? launch_post_tma_b<FMT, TW, true>(s, tm, a, cfg) : launch_post_tma_b<FMT, TW, false>(s, tm, a, cfg);
 }
 
 bool launch_post_tma(cudaStream_t s, const PostArgs& a) {
   PostMapsNv12 tm;
   const int tw = post_tile_width(a);
   if (!post_tma_shape_ok(a) || !build_post_maps(a, &tm, tw, &tm)) return false;
-  const PostTmaCfg cfg{a.out ? 1 : 0, (a.yuyv || a.nv12) ? 1 : 0, a.mask ? 1 : 0, (a.bg_yuyv || a.bg_nv12) ? 1 : 0};
+  // (a launch with the transparent output blends its background tiles per thread: it copies no cached video tile)
+  const PostTmaCfg cfg{a.out ? 1 : 0, (a.yuyv || a.nv12) ? 1 : 0, a.mask ? 1 : 0, ((a.bg_yuyv || a.bg_nv12) && !a.bgra) ? 1 : 0};
   const PostMaps& pm = tm;
   bool ok;
   if (a.nv12_in) ok = tw == 128 ? launch_post_tma_t<IN_NV12, 128>(s, tm, a, cfg) : launch_post_tma_t<IN_NV12, 64>(s, tm, a, cfg);

@@ -164,6 +164,18 @@ BSB_D void post_mask16(const PostArgs& a, bool row_in, int tile_const, int x0, c
 // is m either way.
 BSB_D unsigned blend_weight(bool pass, unsigned m) { return pass ? 0u : m; }
 
+// the transparent output (PostArgs::bgra) of 4 pixels from their blend weights w (blend_weight): the camera bytes f (3 words
+// of BGR) with alpha 255 - w, i.e. 255 - mask (the person matte), or 255 when the frame's filter is off -> 4 BGRA words.
+// rev: in reversed pixel order (a mirrored frame).
+BSB_D uint4 bgra4(const unsigned* f, const unsigned* w, bool rev) {
+  const unsigned A = f[0], B = f[1], C = f[2];                          // b0 g0 r0 b1 | g1 r1 b2 g2 | r2 b3 g3 r3
+  const unsigned p0 = __byte_perm(A, 255u - w[0], 0x4210);
+  const unsigned p1 = __byte_perm(__byte_perm(A, B, 0x0543), 255u - w[1], 0x4210);
+  const unsigned p2 = __byte_perm(__byte_perm(B, C, 0x0432), 255u - w[2], 0x4210);
+  const unsigned p3 = __byte_perm(C >> 8, 255u - w[3], 0x4210);
+  return rev ? make_uint4(p3, p2, p1, p0) : make_uint4(p0, p1, p2, p3);
+}
+
 // 16 pixels: f / g = frame / background bytes (12 words each), m = masks; o = blended BGR (12 words), yy = YUYV (8 words)
 template <bool OUT, bool YUYV>
 BSB_D void post_blend16(const unsigned* f, const unsigned* g, const unsigned* m, unsigned* o, unsigned* yy) {

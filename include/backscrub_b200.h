@@ -109,7 +109,8 @@ BSB_API int bsb_set_background_cursor(bsb_ctx* ctx, int index);
 BSB_API int bsb_set_bgblur(bsb_ctx* ctx, int ksize);
 /* `-H`/`-V` cv::flip of the composited frame (:667-673) and cv::resize to the virtual-camera geometry when it
  * differs from the capture geometry (:677-679); both before the YUYV conversion.  out_w/out_h <= 0 = frame size.
- * After this call `out` buffers are out_w x out_h x 3 and `out_yuyv` out_w x out_h x 2; the mask stays W x H.
+ * After this call `out` buffers are out_w x out_h x 3 (x 4 in the BGRA output format, bsb_set_out_format) and `out_yuyv`
+ * out_w x out_h x 2; the mask stays W x H.
  * The flips and the size are the default of every source of a sources call (bsb_set_source_flip, bsb_set_source_output). */
 BSB_API int bsb_set_output(bsb_ctx* ctx, int flip_h, int flip_v, int out_w, int out_h);
 BSB_API int bsb_output_size(bsb_ctx* ctx, int* out_w, int* out_h);
@@ -123,6 +124,24 @@ BSB_API int bsb_output_size(bsb_ctx* ctx, int* out_w, int* out_h);
  * Host state only: the switch is part of the captured call, so once both states of a call have run, toggling replays.
  * active outside 0..1 returns 0 with a bsb_last_error() message and leaves the context as it was. */
 BSB_API int bsb_set_filter(bsb_ctx* ctx, int active);
+/* Output format of the `out` buffers of every composite entry point (bsb_composite, _device, _yuyv, _yuyv_device, _mjpg,
+ * _nv12, _nv12_device and the three bsb_composite_sources*).  BSB_OUT_BGR (the default): the BGR composite.  BSB_OUT_BGRA:
+ * the person on a transparent background, straight (not premultiplied) alpha, for compositors that take BGRA.  Frame b,
+ * with C its camera frame as the fused path reads it (BGR as given, YUYV / NV12 converted exactly as for the composite) and
+ * M the W x H mask the same call writes (255 = background, outside the ROI included):
+ *   A0[y][x] = (C.B, C.G, C.R, 255 - M[y][x])   (its filter off, bsb_set_filter / bsb_set_source_filter: alpha 255)
+ *   out_b    = cv::resize(cv::flip(A0), INTER_LINEAR) with the flip and output size the frame's composite gets (the
+ *              context's, or its source's own), in the reference's order; OpenCV resizes 8UC4 channel by channel with
+ *              the tables of the 3-channel composite, so the colour bytes are those of a filter-off composite.
+ * Rows are out_w*4 bytes: packed on the device entry points and in the sources strides (a frame of its own size must fit
+ * its out stride at 4 bytes per pixel), out_pitch >= out_w*4 for bsb_composite.  The video output (YUYV / NV12) and the
+ * mask are byte for byte those of a BGR-format call; the smoother, rings and cursors behave as in one.  A call without a
+ * video output blends nothing: it reads and blurs no background (camera blur included) while ring cursors still move.
+ * Host state only, like bsb_set_filter: once both formats of a call have run, toggling replays; the host-buffer staging
+ * grows to 4 bytes per pixel on the first BGRA call that needs it.  A format outside 0..1 returns 0 with a
+ * bsb_last_error() message and changes nothing. */
+enum { BSB_OUT_BGR = 0, BSB_OUT_BGRA = 1 };
+BSB_API int bsb_set_out_format(bsb_ctx* ctx, int format);
 
 /* ---- fused per-frame path: one CUDA-graph launch per call ---------------------------
  * mask generation (bs_maskgen_process) + alpha_blend(bg, frame, mask)
