@@ -125,6 +125,43 @@ class MaskGen:
             self._fail("bsb_set_out_format")
         self.out_channels = 3 + code
 
+    @staticmethod
+    def _live_args(frames, fmt, size, pitch, uv_offset):
+        """(pointer, format code, w, h, pitch, uv_offset) of a live background: an int device pointer or a CUDA tensor"""
+        code = {"bgr": 0, "nv12": 1}.get(fmt, -1) if isinstance(fmt, str) else -1
+        if code < 0:
+            raise BackscrubError(f"unknown live background format {fmt!r} (\"bgr\" or \"nv12\")")
+        if frames is None:
+            return None, code, 0, 0, 0, 0
+        ptr = frames.data_ptr() if hasattr(frames, "data_ptr") else int(frames)
+        w, h = size
+        p = (w * 3 if code == 0 else w) if pitch is None else pitch
+        uv = (p * h if code == 1 else 0) if uv_offset is None else uv_offset
+        return ptr, code, int(w), int(h), int(p), int(uv)
+
+    def set_live_background(self, frames, fmt="bgr", size=None, pitch=None, uv_offset=None, frame_stride=0):
+        """Live background of plain calls: a device image (int pointer, or a CUDA torch.Tensor's data_ptr()) that every later
+        plain call resizes to W x H, blurs at the context's strength and blends, inside the call.  fmt "bgr" (rows `pitch`
+        bytes apart, default w*3) or "nv12" (pitch default w, UV plane at `uv_offset`, default pitch*h); size = (w, h).
+        Frame b of a call blends frames + b*frame_stride (0: one image for every frame).  None clears.  The memory must stay
+        valid and unchanged until the calls that read it have completed on bsb_stream; a tensor is kept referenced here
+        until it is replaced."""
+        ptr, code, w, h, p, uv = self._live_args(frames, fmt, size, pitch, uv_offset)
+        if not self._lib.bsb_set_live_background(self._h, ptr, code, w, h, p, uv, int(frame_stride)):
+            self._fail("bsb_set_live_background")
+        self._live_refs = getattr(self, "_live_refs", {})
+        self._live_refs[None] = frames
+
+    def set_source_live_background(self, source: int, frame, fmt="bgr", size=None, pitch=None, uv_offset=None):
+        """Live background of one source of a sources context (set_live_background's image rules): every later sources call
+        carrying a frame of `source` blends it, at the source's strength, where the source's background is "default".
+        None clears."""
+        ptr, code, w, h, p, uv = self._live_args(frame, fmt, size, pitch, uv_offset)
+        if not self._lib.bsb_set_source_live_background(self._h, int(source), ptr, code, w, h, p, uv):
+            self._fail("bsb_set_source_live_background")
+        self._live_refs = getattr(self, "_live_refs", {})
+        self._live_refs[int(source)] = frame
+
     def background(self) -> np.ndarray:
         out = np.empty((self.height, self.width, 3), np.uint8)
         if not self._lib.bsb_get_background(self._h, _ptr(out), self.width * 3):

@@ -133,6 +133,7 @@ cudaError_t copy_frames(uint8_t* dst, size_t dpitch, size_t dstride, const uint8
 bsb::Call frames_of(bsb::Call c, int b0, int n) {
   auto at = [b0](auto* p, size_t stride) { return p ? p + (size_t)b0 * stride : p; };
   c.n = n; c.in = at(c.in, c.stride); c.out = at(c.out, c.out_stride); c.video = at(c.video, c.video_stride); c.mask = at(c.mask, c.mask_stride);
+  c.frame0 += b0;
   return c;
 }
 
@@ -394,6 +395,22 @@ int bsb_set_out_format(bsb_ctx* ctx, int format) {
   if (!check_ctx(ctx)) return 0;
   if (format != BSB_OUT_BGR && format != BSB_OUT_BGRA) { report(&ctx->cb, "error: output format must be BSB_OUT_BGR (0) or BSB_OUT_BGRA (1)"); return 0; }
   ctx->eng->set_out_bgra(format == BSB_OUT_BGRA);
+  return 1;
+}
+
+int bsb_set_live_background(bsb_ctx* ctx, const uint8_t* d_frames, int fmt, int bg_w, int bg_h, size_t pitch, size_t uv_offset,
+                            size_t frame_stride) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_live_background(d_frames, fmt, bg_w, bg_h, pitch, uv_offset, frame_stride, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
+int bsb_set_source_live_background(bsb_ctx* ctx, int source, const uint8_t* d_frame, int fmt, int bg_w, int bg_h, size_t pitch,
+                                   size_t uv_offset) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_source_live_background(source, d_frame, fmt, bg_w, bg_h, pitch, uv_offset, &err)) { report(&ctx->cb, "error: " + err); return 0; }
   return 1;
 }
 

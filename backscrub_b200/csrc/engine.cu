@@ -897,6 +897,7 @@ bool Engine::upload(std::string* err) {
     const std::vector<int> ones(B, 1);
     CUDA_OK(cudaMalloc((void**)&d_pass_all_, B * sizeof(int)));
     CUDA_OK(cudaMemcpy(d_pass_all_, ones.data(), B * sizeof(int), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMalloc((void**)&d_live_tab_, B * sizeof(LiveDesc)));
   }
   out_w_ = W_; out_h_ = H_;
   out_cap_ = B * fpx * 3; yuyv_cap_ = B * fpx * 2;
@@ -943,7 +944,8 @@ Engine::~Engine() {
     if (p) cudaFree(p);
   for (ChainPlan& cp : chains_) if (cp.d_ops) cudaFree(cp.d_ops);
   free_sources();
-  for (void* p : {(void*)d_src_tab_, (void*)d_src_raw_, tab_src_.blob, (void*)d_pass_all_}) if (p) cudaFree(p);
+  for (void* p : {(void*)d_src_tab_, (void*)d_src_raw_, tab_src_.blob, (void*)d_pass_all_, (void*)d_live_tab_, (void*)d_live_stage_}) if (p) cudaFree(p);
+  for (LiveSize& l : live_sizes_) if (l.tab.blob) cudaFree(l.tab.blob);
   if (h_mask_) cudaFreeHost(h_mask_);
   if (stream_) cudaStreamDestroy(stream_);
 }
@@ -1187,13 +1189,16 @@ PostArgs Engine::post_args(const Call& c, const Plan& p) const {
     a.yuyv_in = p.native ? c.in : nullptr; a.yuyv_in_stride = (size_t)W_ * H_ * 2;
   }
   a.bg = d_bg_; a.bg_pitch = (size_t)W_ * 3; a.bg_stride = 0;
-  if (has_bg_) {
+  if (p.mode == CALL_PLAIN && p.live) {
+    // the resized (and blurred) live images, written by enqueue_post into the per-frame background frames; no YUYV cache
+    a.bg = d_bg_frames_; a.bg_stride = p.live == 2 ? fbytes : 0;
+  } else if (has_bg_) {
     if (bgblur_k_) a.bg = d_bg_eff_;                       // blurred once, when the background / strength was set
     if (bg_count_ > 1) { a.bg_stride = fbytes; a.bg_cursor = d_bg_cursor_; a.bg_count = bg_count_; a.bg_advance = bg_advance_; }
   } else if (bgblur_k_ && blends(c, p) && !p.passed) {
     a.bg = d_bg_frames_; a.bg_stride = fbytes;            // the blurred camera frame itself (filled by enqueue_post)
   }
-  if (bg_yuyv_valid_ && !(bgblur_k_ && !has_bg_)) { a.bg_yuyv = d_bg_yuyv_; a.bg_nv12 = bg_nv12_valid_ ? d_bg_nv12_ : nullptr; }
+  if (bg_yuyv_valid_ && !(bgblur_k_ && !has_bg_) && !p.live) { a.bg_yuyv = d_bg_yuyv_; a.bg_nv12 = bg_nv12_valid_ ? d_bg_nv12_ : nullptr; }
   if (p.mode != CALL_PLAIN) {
     // sources: frame b blends bank slot bg_index[b]; the camera-blur slots' YUYV / NV12 are written by the call's
     // Gaussian, so every slot's cached copy is valid.  A call whose every frame is camera blur runs without them, as a
@@ -1255,8 +1260,9 @@ bool Engine::enqueue_post(const Call& c, const Plan& p) {
     uint8_t* nv = (!p.all_blur && nv12_in) ? d_bank_nv12_ : nullptr;
     launch_gauss_frames(stream_, n, cam, d_src_tab_ + 2 * (size_t)max_batch_, p.gclass, const_cast<uint8_t*>(a.frames), d_gauss_tmp_,
                         d_bank_, yv, nv, W_, H_);
-  } else if (p.mode == CALL_PLAIN && !has_bg_ && bgblur_k_ && blends(c, p) && !p.passed)
+  } else if (p.mode == CALL_PLAIN && !has_bg_ && bgblur_k_ && blends(c, p) && !p.passed && !p.live)
     launch_gauss_blur(stream_, n, a.frames, a.frame_pitch, a.frame_stride, d_gauss_tmp_, d_bg_frames_, (size_t)W_ * 3, fbytes, W_, H_, taps_);
+  if (p.live) enqueue_live(c, p);
   if (!launch_post(stream_, a)) return false;
   if (ring && bg_advance_) launch_advance_cursor(stream_, d_bg_cursor_, (int)(((long)n * bg_advance_) % bg_count_), bg_count_);
   if (!tail || !want_rgb) return true;
@@ -1286,7 +1292,7 @@ bool Engine::yuyv_native(const Call& c, Plan p) const {
   // a sources call whose every frame blurs its camera frame converts every frame to BGR for the Gaussian anyway, and the
   // post kernel reads BGR frames faster than it converts the wire format.  A plain call with the filter off has no
   // Gaussian.
-  const bool camblur = p.mode == CALL_PLAIN ? (bgblur_k_ && !has_bg_ && !p.passed && blends(c, p)) : p.all_blur;
+  const bool camblur = p.mode == CALL_PLAIN ? (bgblur_k_ && !has_bg_ && !p.passed && blends(c, p) && !p.live) : p.all_blur;
   if (c.fmt == IN_BGR || camblur) return false;
   p.native = true; p.nv12_staged = false;
   return post_tma_eligible(post_args(c, p));
@@ -1411,12 +1417,22 @@ bool Engine::run(const Call& c, std::string* err) {
   // a call that blends nothing (BGRA and mask only) adds no Gaussian class for its camera-blur frames
   const bool blend = blends(c, p);
   std::vector<int> tab;
+  // live backgrounds: a plain call's when it blends; a sources call's frames from their sources' (below)
+  std::vector<LiveDesc> ltab;
+  if (!c.ids && live_.p && blend && !p.passed) {
+    p.live = live_.stride ? 2 : 1;
+    p.live_gclass = (unsigned)gauss_class(bgblur_k_);
+    ltab.resize(p.live == 2 ? (size_t)n : 1);
+    for (size_t b = 0; b < ltab.size(); ++b) ltab[b] = live_desc(live_, live_.p + ((size_t)c.frame0 + b) * live_.stride, bgblur_k_ != 0);
+  }
   if (c.ids) {
     if (has_bg_ && bg_count_ > 1) { *err = "sources calls need a still context background (animate a source with bsb_set_source_background)"; return false; }
     // frame b: state of source ids[b]; background (source_bg) = the context slot, the source's slot, or its camera frame
     // blurred at the source's strength into camera-blur slot b; flip, geometry and filter switch = the source's own, else
     // the context's.  A frame whose filter is off blends nothing: it adds no Gaussian class and is no camera-blur frame.
-    tab.assign(6 * (size_t)max_batch_, 0);
+    // A frame that blends its source's live background takes camera-blur slot b for it, blurred at the source's strength.
+    tab.assign(7 * (size_t)max_batch_, 0);
+    ltab.assign((size_t)n, LiveDesc{});
     int n_blur = 0;
     const int ctx_flip = (flip_h_ ? 1 : 0) | (flip_v_ ? 2 : 0);
     for (int b = 0; b < n; ++b) {
@@ -1431,8 +1447,17 @@ bool Engine::run(const Call& c, std::string* err) {
       tab[5 * (size_t)max_batch_ + b] = off ? 1 : 0;
       p.passed = p.passed || off;
       const int from = source_bg(id, &k, &slot);
-      if (from == SRC_FROM_CAMBLUR) slot = b;
-      if (from == SRC_FROM_CAMBLUR && !off && blend) { tab[2 * (size_t)max_batch_ + b] = k; p.gclass |= (unsigned)gauss_class(k); ++n_blur; }
+      const Live& lv = src_live_[id];
+      if (lv.p && src_fx_[id].bg == SRC_BG_DEFAULT && !off && blend) {
+        slot = b;
+        tab[6 * (size_t)max_batch_ + b] = k;
+        p.live_gclass |= (unsigned)gauss_class(k);
+        p.live = 2;
+        ltab[b] = live_desc(lv, lv.p, k != 0);
+      } else {
+        if (from == SRC_FROM_CAMBLUR) slot = b;
+        if (from == SRC_FROM_CAMBLUR && !off && blend) { tab[2 * (size_t)max_batch_ + b] = k; p.gclass |= (unsigned)gauss_class(k); ++n_blur; }
+      }
       tab[(size_t)max_batch_ + b] = (int)slot;
       const int fl = src_flip_[id] < 0 ? ctx_flip : src_flip_[id];
       tab[3 * (size_t)max_batch_ + b] = fl;
@@ -1449,9 +1474,16 @@ bool Engine::run(const Call& c, std::string* err) {
   if (c.fmt != IN_BGR && (W_ & 1)) { *err = "YUYV ingest needs an even width"; return false; }
   CUDA_OK(cudaSetDevice(device_));
   if (c.ids) {
-    if ((p.gclass & GAUSS_SEPARABLE) && !ensure_gauss_tmp(err)) return false;
+    if (((p.gclass | p.live_gclass) & GAUSS_SEPARABLE) && !ensure_gauss_tmp(err)) return false;
     // outside the graph, before its launch: stream order keeps the previous launch's reads ahead of this write
     CUDA_OK(cudaMemcpyAsync(d_src_tab_, tab.data(), tab.size() * sizeof(int), cudaMemcpyHostToDevice, stream_));
+  }
+  if (p.live) {
+    // grown once (dropping the graphs): a plain call's per-frame background frames, the Gaussian's staging
+    const size_t fb = (size_t)max_batch_ * W_ * H_ * 3;
+    if (!c.ids && !ensure((void**)&d_bg_frames_, &bg_frames_cap_, fb, err)) return false;
+    if (p.live_gclass && !ensure((void**)&d_live_stage_, &live_stage_cap_, fb, err)) return false;
+    CUDA_OK(cudaMemcpyAsync(d_live_tab_, ltab.data(), ltab.size() * sizeof(LiveDesc), cudaMemcpyHostToDevice, stream_));
   }
   const bool cbs = c.callbacks && (cb_.onprep || cb_.oninfer || cb_.onmask);
   bool eager = cbs || (flags_ & 2u) || fed_;
@@ -1503,6 +1535,100 @@ bool Engine::run(const Call& c, std::string* err) {
   CUDA_OK(cudaGraphLaunch(it->second.exec, stream_));
   move_cursors(c);
 #endif
+  return true;
+}
+
+// The live frames of a call (app/deepseg.cc:648-661 on a live `-b` source): resized into their background slots, or into
+// the staging for the Gaussian that then writes the slots.  Plain calls: the per-frame background frames at the context's
+// strength (one frame at frame_stride 0), without a YUYV cache; sources calls: camera-blur slot b of the bank at the
+// source's strength, with the slot's YUYV / NV12 in the format the post kernel copies.
+void Engine::enqueue_live(const Call& c, const Plan& p) {
+  const size_t fbytes = (size_t)W_ * H_ * 3;
+  if (p.mode == CALL_PLAIN) {
+    const int n = p.live == 2 ? c.n : 1;
+    launch_live_bg(stream_, n, d_live_tab_, d_bg_frames_, d_live_stage_, nullptr, nullptr, W_, H_);
+    if (bgblur_k_)
+      launch_gauss_blur(stream_, n, d_live_stage_, (size_t)W_ * 3, fbytes, d_gauss_tmp_, d_bg_frames_, (size_t)W_ * 3, fbytes, W_, H_, taps_);
+    return;
+  }
+  const bool nv12_in = p.native && c.fmt == IN_NV12;
+  uint8_t* yv = (!nv12_in && !(W_ & 1)) ? d_bank_yuyv_ : nullptr;
+  uint8_t* nv = nv12_in ? d_bank_nv12_ : nullptr;
+  launch_live_bg(stream_, c.n, d_live_tab_, d_bank_, d_live_stage_, yv, nv, W_, H_);
+  if (p.live_gclass)
+    launch_gauss_frames(stream_, c.n, GaussSrc{}, d_src_tab_ + 6 * (size_t)max_batch_, p.live_gclass, d_live_stage_, d_gauss_tmp_, d_bank_, yv, nv,
+                        W_, H_);
+}
+
+LiveDesc Engine::live_desc(const Live& l, const uint8_t* p, bool blur) const {
+  const DevResizeTab& t = live_sizes_[l.size].tab;
+  LiveDesc d{};
+  d.p = p; d.pitch = l.pitch; d.uv = l.uv; d.fmt = l.fmt; d.w = l.w; d.h = l.h;
+  d.blur = blur ? 1 : 0; d.area2x2 = t.area2x2 ? 1 : 0; d.tab = t.tab;
+  return d;
+}
+
+bool Engine::check_live(int fmt, int w, int h, size_t pitch, size_t uv, std::string* err) const {
+  if (fmt != LIVE_BGR && fmt != LIVE_NV12) { *err = "live background format must be BSB_LIVE_BGR (0) or BSB_LIVE_NV12 (1)"; return false; }
+  if (w < 1 || h < 1 || w > 16384 || h > 16384) { *err = "live background size out of range (1..16384)"; return false; }
+  if (fmt == LIVE_BGR && pitch < (size_t)w * 3) { *err = "live background row pitch is smaller than bg_w*3"; return false; }
+  if (fmt == LIVE_NV12) {
+    if ((w & 1) || (h & 1)) { *err = "NV12 live background needs an even width and height"; return false; }
+    if (pitch < (size_t)w) { *err = "NV12 live background row pitch is smaller than bg_w"; return false; }
+    if (uv < pitch * (size_t)h) { *err = "NV12 live background UV plane offset lies inside the Y plane"; return false; }
+  }
+  return true;
+}
+
+// The resize tables of live size w x h: an entry of that size (its tables are kept while unused), else a free entry (a
+// queued call may still read its old tables, so wait for the stream), else a new one
+bool Engine::live_size_acquire(int w, int h, int* idx, std::string* err) {
+  int i = -1;
+  for (size_t j = 0; j < live_sizes_.size() && i < 0; ++j)
+    if (live_sizes_[j].w == w && live_sizes_[j].h == h) i = (int)j;
+  if (i < 0) {
+    for (size_t j = 0; j < live_sizes_.size() && i < 0; ++j)
+      if (!live_sizes_[j].refs) i = (int)j;
+    CUDA_OK(cudaSetDevice(device_));
+    if (i >= 0) CUDA_OK(cudaStreamSynchronize(stream_));
+    else { i = (int)live_sizes_.size(); live_sizes_.emplace_back(); }
+    LiveSize& l = live_sizes_[i];
+    l.w = l.h = 0;                                   // until the new tables are in place
+    if (!upload_resize_tab(build_resize_tab(w, h, W_, H_), &l.tab, err)) return false;
+    l.w = w; l.h = h;
+  }
+  ++live_sizes_[i].refs;
+  *idx = i;
+  return true;
+}
+
+bool Engine::set_live_background(const uint8_t* p, int fmt, int w, int h, size_t pitch, size_t uv, size_t stride, std::string* err) {
+  if (p) {
+    if (!check_live(fmt, w, h, pitch, uv, err)) return false;
+    const size_t frame = fmt == LIVE_BGR ? pitch * (size_t)(h - 1) + (size_t)w * 3 : uv + pitch * (size_t)(h / 2 - 1) + (size_t)w;
+    if (stride && stride < frame) { *err = "live background frame stride is smaller than one frame"; return false; }
+  }
+  Live l{};
+  if (p) {
+    l = Live{p, fmt, w, h, pitch, fmt == LIVE_NV12 ? uv : 0, stride, -1};
+    if (!live_size_acquire(w, h, &l.size, err)) return false;
+  }
+  live_size_release(live_.size);
+  live_ = l;
+  return true;
+}
+
+bool Engine::set_source_live_background(int source, const uint8_t* p, int fmt, int w, int h, size_t pitch, size_t uv, std::string* err) {
+  if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
+  if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
+  if (p && !check_live(fmt, w, h, pitch, uv, err)) return false;
+  Live l{};
+  if (p) {
+    l = Live{p, fmt, w, h, pitch, fmt == LIVE_NV12 ? uv : 0, 0, -1};
+    if (!live_size_acquire(w, h, &l.size, err)) return false;
+  }
+  live_size_release(src_live_[source].size);
+  src_live_[source] = l;
   return true;
 }
 
@@ -1697,6 +1823,8 @@ void Engine::free_sources() {
   src_flip_.clear();
   src_filter_.clear();
   src_size_.clear();
+  for (const Live& l : src_live_) live_size_release(l.size);
+  src_live_.clear();
   for (OwnSize& o : own_sizes_) if (o.tab.blob) cudaFree(o.tab.blob);
   own_sizes_.clear();
   if (d_geo_) cudaFree(d_geo_);
@@ -1712,8 +1840,8 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   const size_t fbytes = (size_t)W_ * H_ * 3, npix = (size_t)W_ * H_, opx = (size_t)oh_ * ow_;
   const size_t slots = (size_t)max_batch_ + 1 + (size_t)n_sources;
   if (!d_src_tab_) {
-    CUDA_OK(cudaMalloc((void**)&d_src_tab_, 6 * (size_t)max_batch_ * sizeof(int)));
-    CUDA_OK(cudaMemset(d_src_tab_, 0, 6 * (size_t)max_batch_ * sizeof(int)));
+    CUDA_OK(cudaMalloc((void**)&d_src_tab_, 7 * (size_t)max_batch_ * sizeof(int)));
+    CUDA_OK(cudaMemset(d_src_tab_, 0, 7 * (size_t)max_batch_ * sizeof(int)));
   }
   CUDA_OK(cudaMalloc((void**)&src_state_, (size_t)n_sources * opx));
   CUDA_OK(cudaMemset(src_state_, 0, (size_t)n_sources * opx));
@@ -1740,6 +1868,7 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   src_flip_.assign((size_t)n_sources, -1);
   src_filter_.assign((size_t)n_sources, -1);
   src_size_.assign((size_t)n_sources, -1);
+  src_live_.assign((size_t)n_sources, Live{});
   CUDA_OK(cudaMalloc((void**)&d_geo_, (1 + (size_t)n_sources) * sizeof(TailGeo)));
   if (!upload_geo(0, ctx_geo(), err)) return false;
   if (!refresh_bank_ctx(err)) return false;

@@ -85,6 +85,7 @@ struct Call {
   uint8_t* video = nullptr; size_t video_stride = 0;   // tightly packed YUYV, or NV12 when the input is NV12
   uint8_t* mask = nullptr; size_t mask_stride = 0;     // W x H
   bool callbacks = false;            // fire the stage callbacks (the call then runs eagerly, synchronised at each stage)
+  int frame0 = 0;                    // frame 0's index in the caller's call (a chunk of a split call): plain live backgrounds
 };
 
 class Engine {
@@ -122,6 +123,12 @@ class Engine {
   void set_out_bgra(bool bgra) { bgra_ = bgra; }
   bool out_bgra() const { return bgra_; }
   int out_bpp() const { return bgra_ ? 4 : 3; }
+  // Live backgrounds (include/backscrub_b200.h): a caller-owned device image (LiveFmt, any size) that later calls resize
+  // (and blur) inside the call.  Host bookkeeping only, except that a size not seen before has its resize tables built
+  // once.  Plain calls: frame b blends p + b*stride (stride 0: one image for every frame); p null clears.
+  bool set_live_background(const uint8_t* p, int fmt, int w, int h, size_t pitch, size_t uv, size_t stride, std::string* err);
+  // sources calls: every frame of `source` blends this image (where the source's background is BSB_SOURCE_BG_DEFAULT)
+  bool set_source_live_background(int source, const uint8_t* p, int fmt, int w, int h, size_t pitch, size_t uv, std::string* err);
   // device staging of max_batch `out` frames in the current format (host-buffer API), grown on demand; nullptr on error
   uint8_t* out_staging(std::string* err);
   bool sync(std::string* err);
@@ -243,6 +250,9 @@ class Engine {
     bool nv12_staged = false;        // the NV12 output is converted from a YUYV output staged in d_yuyv_ (k_yuyv_to_nv12): an
                                      // NV12 call whose post kernel reads BGR frames, without a tail
     bool bgra = false;               // the call's `out` takes BGRA frames (the context's format, and the call has an out buffer)
+    int live = 0;                    // frames that blend a live background: 0 none, 1 one image for every frame (a plain call
+                                     // at frame_stride 0), 2 one per frame (the live table's descriptors say which)
+    unsigned live_gclass = 0;        // the Gaussian launch classes of the blurred live frames
   };
   // the call blends a composite: it has a video output, or a BGR composite output.  A call that does not reads no
   // background and blurs nothing.
@@ -271,6 +281,7 @@ class Engine {
   void enqueue_cnn(int n, bool from_u8);
   void enqueue_decision(int n, bool sources);
   bool enqueue_post(const Call& c, const Plan& p);
+  void enqueue_live(const Call& c, const Plan& p);
   // base of tensor t for the frames [frame_off_, ...) of the batch (frame_off_ != 0 only inside a sub-batched segment)
   float* tptr(int t) const {
     const TensorInfo& I = tinfo_[t];
@@ -383,10 +394,27 @@ class Engine {
   // ---- independent sources (calls with ids) ----
   int n_sources_ = 0;
   uint8_t* src_state_ = nullptr;     // [n_sources][oh*ow] smoother state per source
-  // [6][max_batch]: source id of frame b | background-bank slot of frame b | camera-blur strength of frame b (0 = none) |
+  // [7][max_batch]: source id of frame b | background-bank slot of frame b | camera-blur strength of frame b (0 = none) |
   // flip code of frame b (bit 0 horizontal, bit 1 vertical; the source's own, or the context's) | geometry slot of frame b
-  // (d_geo_ index) | 1 when frame b's filter is off (the source's own switch, or the context's), written before each launch
+  // (d_geo_ index) | 1 when frame b's filter is off (the source's own switch, or the context's) | live-background strength
+  // of frame b (0 = not blurred, or no live background), written before each launch
   int* d_src_tab_ = nullptr;
+  // ---- live backgrounds ----
+  struct Live { const uint8_t* p = nullptr; int fmt = 0, w = 0, h = 0; size_t pitch = 0, uv = 0, stride = 0; int size = -1; };
+  Live live_;                        // plain calls
+  std::vector<Live> src_live_;       // per source
+  // resize tables per distinct live size, shared by the plain and the source live backgrounds; an entry no live background
+  // uses any more keeps its tables until a new size needs the entry
+  struct LiveSize { int w = 0, h = 0, refs = 0; DevResizeTab tab; };
+  std::vector<LiveSize> live_sizes_;
+  bool check_live(int fmt, int w, int h, size_t pitch, size_t uv, std::string* err) const;
+  bool live_size_acquire(int w, int h, int* idx, std::string* err);
+  void live_size_release(int idx) { if (idx >= 0) --live_sizes_[idx].refs; }
+  // the descriptor of live image l at p, blurred by a Gaussian that follows or not
+  LiveDesc live_desc(const Live& l, const uint8_t* p, bool blur) const;
+  LiveDesc* d_live_tab_ = nullptr;   // [max_batch] descriptors of a call's frames, written before each launch with live frames
+  uint8_t* d_live_stage_ = nullptr;  // [max_batch][H][W][3] resized live images the Gaussian reads
+  size_t live_stage_cap_ = 0;
   // Output geometries k_tail reads, [1 + n_sources]: slot 0 the context's (set_output), slot 1 + i own size i.  Each own
   // size is kept once, however many sources use it; a slot no source uses any more is reused by the next new size.
   TailGeo* d_geo_ = nullptr;
@@ -439,19 +467,21 @@ class Engine {
   // an absent output does not matter), and the plan's mode (a plain and a sources graph over the same buffers are
   // different graphs), Gaussian classes (strengths within them replay), all-blur, flipped and passed (which frames flip or
   // are filtered off is table data), resized and the largest output size of the sources, which the tail's grid covers
-  // (which frame has which size is table data too), and the output format.  The rest of the plan is decided from these.
+  // (which frame has which size is table data too), the output format, and whether frames blend live backgrounds, with
+  // the Gaussian classes they add (their images, sizes and strengths within the classes are the live table's data).  The
+  // rest of the plan is decided from these.
   struct GraphKey {
     int n, fmt; const void* in; size_t pitch, uv, stride;
     const void* out; const void* video; const void* mask; size_t ostride, vstride, mstride;
-    int mode; unsigned gclass; bool all_blur, flipped, resized, passed; long out_px_max; bool bgra;
+    int mode; unsigned gclass; bool all_blur, flipped, resized, passed; long out_px_max; bool bgra; int live; unsigned live_gclass;
     GraphKey(const Call& c, const Plan& p, long px_max)
         : n(c.n), fmt(c.fmt), in(c.in), pitch(c.pitch), uv(c.uv), stride(c.stride), out(c.out), video(c.video), mask(c.mask),
           ostride(c.out ? c.out_stride : 0), vstride(c.video ? c.video_stride : 0), mstride(c.mask ? c.mask_stride : 0),
           mode(p.mode), gclass(p.gclass), all_blur(p.all_blur), flipped(p.flipped), resized(p.resized), passed(p.passed),
-          out_px_max(px_max), bgra(p.bgra) {}
+          out_px_max(px_max), bgra(p.bgra), live(p.live), live_gclass(p.live_gclass) {}
     auto tie() const {
       return std::tie(n, fmt, in, pitch, uv, stride, out, video, mask, ostride, vstride, mstride, mode, gclass, all_blur, flipped, resized,
-                      passed, out_px_max, bgra);
+                      passed, out_px_max, bgra, live, live_gclass);
     }
     bool operator<(const GraphKey& r) const { return tie() < r.tie(); }
   };

@@ -273,6 +273,24 @@ void launch_resize_u8c3(cudaStream_t s, const uint8_t* src, int sw, int sh, size
                         uint8_t* dst, int dw, int dh, size_t dpitch, ResizeTab tab, bool area2x2,
                         int n = 1, size_t sstride = 0, size_t dstride = 0);
 
+// Live backgrounds (include/backscrub_b200.h, bsb_set_live_background / bsb_set_source_live_background): frame b of a call
+// blends a caller-owned device image, BGR or NV12 of any size, resized to W x H inside the call (app/background.cc:178-194
+// on the newest frame of the `-b` source, app/deepseg.cc:648-650).
+enum LiveFmt : int { LIVE_BGR = 0, LIVE_NV12 = 1 };
+struct LiveDesc {
+  const uint8_t* p;          // null: the frame has no live background (its CTAs exit at once)
+  size_t pitch, uv;          // row pitch; NV12: the UV plane's byte offset
+  int fmt, w, h;             // LiveFmt and size
+  int blur;                  // non-zero: a Gaussian follows, so the frame goes to the staging, else to its slot
+  int area2x2;               // exact 2x down (OpenCV's INTER_AREA case), else INTER_LINEAR through tab
+  ResizeTab tab;             // w x h -> W x H (the tables of the live size, kept per distinct size)
+};
+// descs: DEVICE [n].  Frame b: cv::resize(INTER_LINEAR) of its live image to W x H (NV12 taps converted per source pixel as
+// cv::cvtColor(COLOR_YUV2BGR_NV12) would) into slot + b*W*H*3 and, where given, the slot's YUYV (yuyv + b*W*H*2, W even)
+// or NV12 (nv12 + b*W*H*3/2, W and H even); a frame with `blur` set goes to stage + b*W*H*3 instead (tightly packed BGR
+// the Gaussian reads), without YUYV / NV12.
+void launch_live_bg(cudaStream_t s, int n, const LiveDesc* descs, uint8_t* slot, uint8_t* stage, uint8_t* yuyv, uint8_t* nv12, int W, int H);
+
 // app/deepseg.cc:657-658: cv::GaussianBlur(bg, bg, Size(k,k), 0), 8UC3 — OpenCV's 8.8 fixed-point taps (sum 256)
 struct GaussTaps { int k; uint16_t q[255]; };
 bool gauss_taps(int k, GaussTaps* out);           // false unless k is odd, 1..255

@@ -866,6 +866,73 @@ void launch_resize_u8c3(cudaStream_t s, const uint8_t* src, int sw, int sh, size
 }
 
 // ---------------------------------------------------------------------------
+// Live backgrounds: the caller's device image of each frame resized to W x H (app/background.cc:178-194) inside the call.
+// One thread = one 2x2 output block of one frame (frames along blockIdx.y), so the block's two YUYV words and its NV12
+// come from registers.  NV12 images are never converted as a whole: each tap is converted where resize_px reads it
+// (cv::cvtColor(COLOR_YUV2BGR_NV12) then cv::resize, as the pre-processing reads NV12 camera frames).
+// ---------------------------------------------------------------------------
+// output pixel (dx, dy) of live image d
+BSB_D void live_px(const LiveDesc& d, int dx, int dy, uint8_t* o) {
+  if (d.fmt == LIVE_BGR) { resize_px(d.p, d.w, d.h, d.pitch, d.tab, d.area2x2 != 0, 0, dx, dy, o); return; }
+  int p00[3], p01[3], p10[3], p11[3];
+  if (d.area2x2) {
+    const int x0 = 2 * dx, y0 = 2 * dy;
+    nv12_px_to_bgr(d.p, d.pitch, d.uv, x0, y0, p00); nv12_px_to_bgr(d.p, d.pitch, d.uv, x0 + 1, y0, p01);
+    nv12_px_to_bgr(d.p, d.pitch, d.uv, x0, y0 + 1, p10); nv12_px_to_bgr(d.p, d.pitch, d.uv, x0 + 1, y0 + 1, p11);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) o[c] = (uint8_t)((p00[c] + p01[c] + p10[c] + p11[c] + 2) >> 2);
+    return;
+  }
+  const int sx = __ldg(d.tab.xofs + dx), sx1 = min(sx + 1, d.w - 1);
+  const int y0 = __ldg(d.tab.yofs0 + dy), y1 = __ldg(d.tab.yofs1 + dy);
+  const int a0 = __ldg(d.tab.xw + 2 * dx), a1 = __ldg(d.tab.xw + 2 * dx + 1);
+  const int b0 = __ldg(d.tab.yw + 2 * dy), b1 = __ldg(d.tab.yw + 2 * dy + 1);
+  nv12_px_to_bgr(d.p, d.pitch, d.uv, sx, y0, p00); nv12_px_to_bgr(d.p, d.pitch, d.uv, sx1, y0, p01);
+  nv12_px_to_bgr(d.p, d.pitch, d.uv, sx, y1, p10); nv12_px_to_bgr(d.p, d.pitch, d.uv, sx1, y1, p11);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) o[c] = lin_v(p00[c] * a0 + p01[c] * a1, p10[c] * a0 + p11[c] * a1, b0, b1);
+}
+
+__global__ void __launch_bounds__(256) k_live_bg(const LiveDesc* descs, uint8_t* slot, uint8_t* stage, uint8_t* yuyv, uint8_t* nv12,
+                                                 int W, int H) {
+  const int b = blockIdx.y;
+  const LiveDesc d = descs[b];
+  if (!d.p) return;
+  const int hw = (W + 1) / 2;
+  const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long)hw * ((H + 1) / 2)) return;
+  const int x = (int)(i % hw) * 2, y = (int)(i / hw) * 2;
+  const bool xr = x + 1 < W, yr = y + 1 < H;             // the block's right column / lower row exist
+  uint8_t px[12];                                         // (x, y) (x+1, y) | (x, y+1) (x+1, y+1)
+  live_px(d, x, y, px);
+  if (xr) live_px(d, x + 1, y, px + 3);
+  if (yr) {
+    live_px(d, x, y + 1, px + 6);
+    if (xr) live_px(d, x + 1, y + 1, px + 9);
+  }
+  const size_t npix = (size_t)W * H;
+  uint8_t* o = (d.blur ? stage : slot) + (size_t)b * npix * 3 + ((size_t)y * W + x) * 3;
+  const int nb = xr ? 6 : 3;
+  for (int k = 0; k < nb; ++k) o[k] = px[k];
+  if (yr) for (int k = 0; k < nb; ++k) o[(size_t)W * 3 + k] = px[6 + k];
+  if (d.blur) return;
+  if (nv12) {                                             // W and H even
+    uint8_t* f = nv12 + (size_t)b * (npix * 3 / 2);
+    nv12_block(yuyv_pair_word(px), yuyv_pair_word(px + 6), f + (size_t)y * W + x, W, f + npix + (size_t)(y / 2) * W + x);
+  } else if (yuyv) {                                      // W even: the pixel pairs of convert_rgb_to_yuyv are row pairs
+    unsigned* f = reinterpret_cast<unsigned*>(yuyv + (size_t)b * npix * 2);
+    f[((size_t)y * W + x) / 2] = yuyv_pair_word(px);
+    if (yr) f[((size_t)(y + 1) * W + x) / 2] = yuyv_pair_word(px + 6);
+  }
+}
+
+void launch_live_bg(cudaStream_t s, int n, const LiveDesc* descs, uint8_t* slot, uint8_t* stage, uint8_t* yuyv, uint8_t* nv12, int W, int H) {
+  const long blocks = ((long)((W + 1) / 2) * ((H + 1) / 2) + 255) / 256;
+  BSB_LAUNCH(k_live_bg, dim3((unsigned)blocks, (unsigned)n), dim3(256), 0, s, descs, slot, stage, yuyv, nv12, W, H);
+  count_launch();
+}
+
+// ---------------------------------------------------------------------------
 // YUYV -> BGR ingest (cv::cvtColor COLOR_YUV2BGR_YUYV, BT.601 limited range, 20-bit fixed point).
 // One thread = 8 pixels: one 16-byte load, 24 bytes out.
 // ---------------------------------------------------------------------------

@@ -142,6 +142,42 @@ BSB_API int bsb_set_filter(bsb_ctx* ctx, int active);
  * bsb_last_error() message and changes nothing. */
 enum { BSB_OUT_BGR = 0, BSB_OUT_BGRA = 1 };
 BSB_API int bsb_set_out_format(bsb_ctx* ctx, int format);
+/* Live backgrounds (the reference's `-b` takes any OpenCV source and blends its newest frame every loop iteration,
+ * app/deepseg.cc:522-524,648-661): device images the caller already holds (decoded video surfaces, screen captures, a
+ * second camera) are resized, blurred and blended inside the call, with no host copy and no launch outside it.
+ * BSB_LIVE_BGR: bg_w x bg_h x 3 rows `pitch` bytes apart.  BSB_LIVE_NV12: a Y plane of bg_h rows `pitch` bytes apart and the
+ * interleaved UV plane at byte `uv_offset` (the pitched surfaces of a hardware decoder need no copy); uv_offset is ignored
+ * for BGR.
+ *   Exactness: frame b of a call with live background L gives exactly the composite, video output (YUYV / NV12), mask and
+ *   BGRA output of a plain batch-1 context set up the same way (bgblur, output, filter and format settings) plus
+ *   bsb_set_background(L), fed the same stream one frame per call; for an NV12 L, bsb_set_background of
+ *   bsb_convert_nv12_to_bgr(L).  That is cv::resize INTER_LINEAR of L to W x H (the exact 2x down-scale takes OpenCV's
+ *   INTER_AREA mean), then the Gaussian at the frame's strength, then alpha_blend.
+ *   Precedence: in plain calls a live background wins over the context image or ring, and a camera-blur context blurs the
+ *   live frame instead of the camera frame.  In sources calls, for a source at BSB_SOURCE_BG_DEFAULT: its live background,
+ *   else its own image or ring, else the context background; at BSB_SOURCE_BG_NONE the live background is ignored, as its
+ *   own image is.  The strength is the source's effective one; bsb_set_live_background applies to plain calls only.
+ *   A ring cursor keeps moving while a live background hides the ring.  A frame that blends nothing (its filter off, or a
+ *   BGRA call without a video output) reads no live background.
+ *   Host bookkeeping only: no device work and no synchronisation, so the pointers may change every call; they reach the
+ *   device with the call's tables, and a captured call replays for new pointers, sizes already seen and strengths within
+ *   the Gaussian classes it was captured with.  A size not seen before has its resize tables built once (kept per distinct
+ *   size; reusing the tables of a size no live background uses any more waits for the context's stream).
+ *   Caller contract: device memory of the context's device, in place when the call's work runs on the context stream
+ *   (bsb_stream) and unchanged until that work completes; read by every later call until replaced or cleared, the
+ *   host-buffer entry points included.
+ * A violated rule returns 0 with a bsb_last_error() message and leaves the context as it was: fmt outside 0..1, bg_w or bg_h
+ * outside 1..16384, BGR pitch < bg_w*3, NV12 with an odd bg_w or bg_h, pitch < bg_w or uv_offset < pitch*bg_h. */
+enum { BSB_LIVE_BGR = 0, BSB_LIVE_NV12 = 1 };
+/* plain calls: frame b of every later plain composite call blends live frame b (d_frames + b*frame_stride; frame_stride 0 =
+ * one image for every frame of the call; a nonzero frame_stride smaller than one frame is refused).  d_frames NULL clears. */
+BSB_API int bsb_set_live_background(bsb_ctx* ctx, const uint8_t* d_frames, int fmt, int bg_w, int bg_h,
+                                    size_t pitch, size_t uv_offset, size_t frame_stride);
+/* sources calls: the frame of `source` in every later sources call blends this image.  d_frame NULL clears.  No
+ * bsb_set_sources yet or a source id out of range is refused.  bsb_set_sources clears every source's live background;
+ * bsb_reset_source keeps it. */
+BSB_API int bsb_set_source_live_background(bsb_ctx* ctx, int source, const uint8_t* d_frame, int fmt, int bg_w, int bg_h,
+                                           size_t pitch, size_t uv_offset);
 
 /* ---- fused per-frame path: one CUDA-graph launch per call ---------------------------
  * mask generation (bs_maskgen_process) + alpha_blend(bg, frame, mask)
