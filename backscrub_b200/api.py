@@ -114,6 +114,12 @@ class MaskGen:
         if not self._lib.bsb_set_filter(self._h, int(bool(active))):
             self._fail("bsb_set_filter")
 
+    def set_mask_interval(self, k: int):
+        """segment every k-th frame (1..256, default 1); the frames between are composited with their camera's latest mask
+        (include/backscrub_b200.h, bsb_set_mask_interval)"""
+        if not self._lib.bsb_set_mask_interval(self._h, int(k)):
+            self._fail("bsb_set_mask_interval")
+
     def set_out_format(self, fmt: str):
         """format of the `out` frames of every composite call: "bgr" (the composite, the default) or "bgra" (the camera with
         alpha 255 - mask, straight alpha, flipped and resized like the composite; the video output and the mask are
@@ -360,6 +366,11 @@ class MaskGen:
         v = -1 if active is None else int(bool(active))
         if not self._lib.bsb_set_source_filter(self._h, int(source), v):
             self._fail("bsb_set_source_filter")
+
+    def set_source_mask_interval(self, source: int, k=None):
+        """mask interval of one source: None = follow set_mask_interval, including later changes; otherwise 1..256"""
+        if not self._lib.bsb_set_source_mask_interval(self._h, int(source), -1 if k is None else int(k)):
+            self._fail("bsb_set_source_mask_interval")
 
     def set_source_output(self, source: int, out_size=None):
         """virtual-camera size of one source (cv::resize after the flip, app/deepseg.cc:677-679): out_size = (w, h), or

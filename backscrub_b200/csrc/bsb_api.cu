@@ -391,6 +391,20 @@ int bsb_set_filter(bsb_ctx* ctx, int active) {
   return 1;
 }
 
+int bsb_set_mask_interval(bsb_ctx* ctx, int interval) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_mask_interval(interval, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
+int bsb_set_source_mask_interval(bsb_ctx* ctx, int source, int interval) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_source_mask_interval(source, interval, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
 int bsb_set_out_format(bsb_ctx* ctx, int format) {
   if (!check_ctx(ctx)) return 0;
   if (format != BSB_OUT_BGR && format != BSB_OUT_BGRA) { report(&ctx->cb, "error: output format must be BSB_OUT_BGR (0) or BSB_OUT_BGRA (1)"); return 0; }

@@ -944,7 +944,8 @@ Engine::~Engine() {
     if (p) cudaFree(p);
   for (ChainPlan& cp : chains_) if (cp.d_ops) cudaFree(cp.d_ops);
   free_sources();
-  for (void* p : {(void*)d_src_tab_, (void*)d_src_raw_, tab_src_.blob, (void*)d_pass_all_, (void*)d_live_tab_, (void*)d_live_stage_}) if (p) cudaFree(p);
+  for (void* p : {(void*)d_src_tab_, (void*)d_src_raw_, tab_src_.blob, (void*)d_pass_all_, (void*)d_live_tab_, (void*)d_live_stage_, (void*)d_seg_tab_})
+    if (p) cudaFree(p);
   for (LiveSize& l : live_sizes_) if (l.tab.blob) cudaFree(l.tab.blob);
   if (h_mask_) cudaFreeHost(h_mask_);
   if (stream_) cudaStreamDestroy(stream_);
@@ -953,13 +954,13 @@ Engine::~Engine() {
 // ---------------------------------------------------------------------------
 // enqueue: the per-call kernel sequence (captured into a CUDA graph by run())
 // ---------------------------------------------------------------------------
-void Engine::enqueue_pre(const Call& c) {
+void Engine::enqueue_pre(const Call& c, int m, const int* gather) {
   // camera YUYV / NV12 frames are read in place (each bilinear tap converted like cv::COLOR_YUV2BGR_YUYV / _NV12 would have)
-  launch_resize_roi_swap(stream_, c.n, c.in, c.stride, c.pitch, roidim_[0], roidim_[1], roidim_[2], roidim_[3], tab_in_.tab,
-                         in_u8_, mw_, mh_, in_roidim_[0], in_roidim_[1], in_roidim_[2], in_roidim_[3], tab_in_.area2x2, c.fmt, c.uv);
+  launch_resize_roi_swap(stream_, m, c.in, c.stride, c.pitch, roidim_[0], roidim_[1], roidim_[2], roidim_[3], tab_in_.tab,
+                         in_u8_, mw_, mh_, in_roidim_[0], in_roidim_[1], in_roidim_[2], in_roidim_[3], tab_in_.area2x2, c.fmt, c.uv, gather);
   // with the fused stem the fp32 input tensor is only materialised for introspection (KEEP_TENSORS)
   float* f32 = (stem_u8_ok_ && !(flags_ & 1u)) ? nullptr : tptr(g_.input);
-  launch_bilateral_norm(stream_, c.n, in_u8_, mw_, mh_, lut_, lut_ + 768, scaling_, offset_, f32, filt_u8_);
+  launch_bilateral_norm(stream_, m, in_u8_, mw_, mh_, lut_, lut_ + 768, scaling_, offset_, f32, filt_u8_);
 }
 
 // Frames per pass of a sub-batched segment: the segment's largest tensor, in and out, should stay L2-resident
@@ -1157,20 +1158,71 @@ void Engine::run_step(size_t si, int n, bool from_u8, bool* first_p, bool* skip_
   }
 }
 
-// sources: per-source states, looked up through the id table
-void Engine::enqueue_decision(int n, bool sources) {
+// sources: per-source states, looked up through the id table.  n call frames, m of them segmented (the CNN batch; m == n
+// with null rows when none is held).  Sources calls launch over the n frames, plain calls over the m decisions.
+void Engine::enqueue_decision(int n, bool sources, int m, const SegRows& seg) {
   if (dec_up_step_ >= 0) {
     const Step& st = steps_[dec_up_step_];
     const TensorInfo& I = tinfo_[st.in];
     if (sources)
       launch_decision_up_sources(stream_, n, tptr(st.in), I.h, I.w, I.ld, st.align_corners, st.half_pixel, oh_, ow_, src_state_, d_src_tab_,
-                                 ofinal_, opitch_);
+                                 ofinal_, opitch_, seg.cidx);
     else
-      launch_decision_up_iir(stream_, n, tptr(st.in), I.h, I.w, I.ld, st.align_corners, st.half_pixel, oh_, ow_, state_, ofinal_, opitch_);
+      launch_decision_up_iir(stream_, m, tptr(st.in), I.h, I.w, I.ld, st.align_corners, st.half_pixel, oh_, ow_, state_, ofinal_, opitch_, seg);
     return;
   }
-  if (sources) launch_decision_sources(stream_, model_type_, n, tptr(g_.output), oh_, ow_, oc_, src_state_, d_src_tab_, ofinal_, opitch_);
-  else launch_decision_iir(stream_, model_type_, n, tptr(g_.output), oh_, ow_, oc_, state_, ofinal_, opitch_);
+  if (sources) launch_decision_sources(stream_, model_type_, n, tptr(g_.output), oh_, ow_, oc_, src_state_, d_src_tab_, ofinal_, opitch_, seg.cidx);
+  else launch_decision_iir(stream_, model_type_, m, tptr(g_.output), oh_, ow_, oc_, state_, ofinal_, opitch_, seg);
+}
+
+// Mask interval: plain frame c (counted over the context's plain calls) is segmented iff c % k == 0; frame f of source s
+// iff f == 0 || (f + s) % k_s == 0 (the id as the phase staggers sources with consecutive ids, and a new or reset camera
+// always starts with a mask of its own).
+int Engine::segment(const Call& c, std::vector<int>* rows) const {
+  const int n = c.n;
+  if (fed_ || (!c.ids && mask_interval_ == 1)) return n;
+  rows->assign(3 * (size_t)max_batch_, -1);
+  int m = 0;
+  for (int b = 0; b < n; ++b) {
+    bool seg;
+    if (c.ids) {
+      const int s = c.ids[b];
+      seg = src_frames_[s] == 0 || (src_frames_[s] + s) % src_interval(s) == 0;
+    } else {
+      seg = (plain_frames_ + b) % mask_interval_ == 0;
+    }
+    if (seg) { (*rows)[m] = b; (*rows)[(size_t)max_batch_ + b] = m; ++m; }
+    (*rows)[2 * (size_t)max_batch_ + b] = m - 1;
+  }
+  return m;
+}
+
+SegRows Engine::seg_rows(const Call& c, const Plan& p) const {
+  if (p.m == c.n) return SegRows{};
+  const size_t mb = (size_t)max_batch_;
+  if (p.mode == CALL_PLAIN) return SegRows{c.n, d_seg_tab_, d_seg_tab_ + mb, d_seg_tab_ + 2 * mb};
+  const int* t = d_src_tab_ + SRC_TAB_SEG * mb;
+  return SegRows{c.n, t, t + mb, nullptr};
+}
+
+void Engine::count_frames(const Call& c) {
+  if (fed_) return;
+  if (!c.ids) { plain_frames_ += c.n; return; }
+  for (int b = 0; b < c.n; ++b) ++src_frames_[c.ids[b]];
+}
+
+bool Engine::set_mask_interval(int k, std::string* err) {
+  if (k < 1 || k > MASK_INTERVAL_MAX) { *err = "mask interval out of range (1..256)"; return false; }
+  mask_interval_ = k;
+  return true;
+}
+
+bool Engine::set_source_mask_interval(int source, int k, std::string* err) {
+  if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
+  if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
+  if (k != -1 && (k < 1 || k > MASK_INTERVAL_MAX)) { *err = "source mask interval out of range (-1, or 1..256)"; return false; }
+  src_interval_[source] = k;
+  return true;
 }
 
 // PostArgs of one call.  p.native: the post kernel reads the camera frames in place — YUYV, or NV12, which then also
@@ -1336,13 +1388,15 @@ bool Engine::enqueue_all(const Call& c, const Plan& p) {
   if (c.fmt == IN_YUYV && !p.native) launch_yuyv_to_bgr(stream_, c.in, d_frames_, (size_t)n * W_ * H_);
   if (fed_) {
     enqueue_feed(*fed_);
-    if (fed_->stage == FEED_LOGITS) enqueue_decision(n, p.mode != CALL_PLAIN);
+    if (fed_->stage == FEED_LOGITS) enqueue_decision(n, p.mode != CALL_PLAIN, n, SegRows{});
   } else {
-    enqueue_pre(c);
+    // a call with held frames pre-processes and segments its m segmented frames only (none: no launch before the decision)
+    const SegRows seg = seg_rows(c, p);
+    if (p.m) enqueue_pre(c, p.m, seg.gather);
     if (c.callbacks && cb_.onprep) { cudaStreamSynchronize(stream_); cb_.onprep(cb_.caller_ctx); }
-    enqueue_cnn(n, true);
+    if (p.m) enqueue_cnn(p.m, true);
     if (c.callbacks && cb_.oninfer) { cudaStreamSynchronize(stream_); cb_.oninfer(cb_.caller_ctx); }
-    enqueue_decision(n, p.mode != CALL_PLAIN);
+    enqueue_decision(n, p.mode != CALL_PLAIN, p.m, seg);
     if (c.callbacks && cb_.onmask) { cudaStreamSynchronize(stream_); cb_.onmask(cb_.caller_ctx); }
   }
   if (!enqueue_post(c, p)) return false;
@@ -1431,7 +1485,7 @@ bool Engine::run(const Call& c, std::string* err) {
     // blurred at the source's strength into camera-blur slot b; flip, geometry and filter switch = the source's own, else
     // the context's.  A frame whose filter is off blends nothing: it adds no Gaussian class and is no camera-blur frame.
     // A frame that blends its source's live background takes camera-blur slot b for it, blurred at the source's strength.
-    tab.assign(7 * (size_t)max_batch_, 0);
+    tab.assign(SRC_TAB_ROWS * (size_t)max_batch_, 0);
     ltab.assign((size_t)n, LiveDesc{});
     int n_blur = 0;
     const int ctx_flip = (flip_h_ ? 1 : 0) | (flip_v_ ? 2 : 0);
@@ -1472,7 +1526,15 @@ bool Engine::run(const Call& c, std::string* err) {
     p.all_blur = n_blur == n;
   }
   if (c.fmt != IN_BGR && (W_ & 1)) { *err = "YUYV ingest needs an even width"; return false; }
+  std::vector<int> seg;
+  p.m = segment(c, &seg);
+  if (c.ids && p.m < n) std::copy(seg.begin(), seg.begin() + 2 * (size_t)max_batch_, tab.begin() + SRC_TAB_SEG * (size_t)max_batch_);
   CUDA_OK(cudaSetDevice(device_));
+  if (!c.ids && p.m < n) {
+    // outside the graph, before its launch, like the source table
+    if (!d_seg_tab_) CUDA_OK(cudaMalloc((void**)&d_seg_tab_, seg.size() * sizeof(int)));
+    CUDA_OK(cudaMemcpyAsync(d_seg_tab_, seg.data(), seg.size() * sizeof(int), cudaMemcpyHostToDevice, stream_));
+  }
   if (c.ids) {
     if (((p.gclass | p.live_gclass) & GAUSS_SEPARABLE) && !ensure_gauss_tmp(err)) return false;
     // outside the graph, before its launch: stream order keeps the previous launch's reads ahead of this write
@@ -1497,6 +1559,7 @@ bool Engine::run(const Call& c, std::string* err) {
     if (!enqueue_all(c, p)) { *err = kNoMirror; return false; }
     CUDA_OK(cudaGetLastError());
     move_cursors(c);
+    count_frames(c);
     return true;
   }
 #ifndef BSB_EMU
@@ -1534,6 +1597,7 @@ bool Engine::run(const Call& c, std::string* err) {
   last_native_ = it->second.native;
   CUDA_OK(cudaGraphLaunch(it->second.exec, stream_));
   move_cursors(c);
+  count_frames(c);
 #endif
   return true;
 }
@@ -1806,6 +1870,7 @@ bool Engine::reset_state(std::string* err) {
   CUDA_OK(cudaSetDevice(device_));
   CUDA_OK(cudaMemsetAsync(state_, 0, (size_t)oh_ * ow_, stream_));
   CUDA_OK(cudaStreamSynchronize(stream_));
+  plain_frames_ = 0;
   return true;
 }
 
@@ -1823,6 +1888,8 @@ void Engine::free_sources() {
   src_flip_.clear();
   src_filter_.clear();
   src_size_.clear();
+  src_interval_.clear();
+  src_frames_.clear();
   for (const Live& l : src_live_) live_size_release(l.size);
   src_live_.clear();
   for (OwnSize& o : own_sizes_) if (o.tab.blob) cudaFree(o.tab.blob);
@@ -1840,8 +1907,8 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   const size_t fbytes = (size_t)W_ * H_ * 3, npix = (size_t)W_ * H_, opx = (size_t)oh_ * ow_;
   const size_t slots = (size_t)max_batch_ + 1 + (size_t)n_sources;
   if (!d_src_tab_) {
-    CUDA_OK(cudaMalloc((void**)&d_src_tab_, 7 * (size_t)max_batch_ * sizeof(int)));
-    CUDA_OK(cudaMemset(d_src_tab_, 0, 7 * (size_t)max_batch_ * sizeof(int)));
+    CUDA_OK(cudaMalloc((void**)&d_src_tab_, SRC_TAB_ROWS * (size_t)max_batch_ * sizeof(int)));
+    CUDA_OK(cudaMemset(d_src_tab_, 0, SRC_TAB_ROWS * (size_t)max_batch_ * sizeof(int)));
   }
   CUDA_OK(cudaMalloc((void**)&src_state_, (size_t)n_sources * opx));
   CUDA_OK(cudaMemset(src_state_, 0, (size_t)n_sources * opx));
@@ -1869,6 +1936,8 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   src_filter_.assign((size_t)n_sources, -1);
   src_size_.assign((size_t)n_sources, -1);
   src_live_.assign((size_t)n_sources, Live{});
+  src_interval_.assign((size_t)n_sources, -1);
+  src_frames_.assign((size_t)n_sources, 0);
   CUDA_OK(cudaMalloc((void**)&d_geo_, (1 + (size_t)n_sources) * sizeof(TailGeo)));
   if (!upload_geo(0, ctx_geo(), err)) return false;
   if (!refresh_bank_ctx(err)) return false;
@@ -1883,6 +1952,7 @@ bool Engine::reset_source(int source, std::string* err) {
   const size_t opx = (size_t)oh_ * ow_;
   CUDA_OK(cudaMemsetAsync(src_state_ + (size_t)source * opx, 0, opx, stream_));
   CUDA_OK(cudaStreamSynchronize(stream_));
+  src_frames_[source] = 0;
   return true;
 }
 
@@ -2210,9 +2280,9 @@ double Engine::time_stage(int stage, int n, int iters, std::string* err) {
   Plan p;
   p.native = yuyv;
   auto once = [&]() {
-    if (stage == 0 || stage == 4) enqueue_pre(c);
+    if (stage == 0 || stage == 4) enqueue_pre(c, n, nullptr);
     if (stage == 1 || stage == 4) enqueue_cnn(n, true);
-    if (stage == 2 || stage == 4) enqueue_decision(n, false);
+    if (stage == 2 || stage == 4) enqueue_decision(n, false, n, SegRows{});
     if (stage == 3 || stage == 4) (void)enqueue_post(c, p);
   };
   once();                                   // warm-up (instruction cache, tables)

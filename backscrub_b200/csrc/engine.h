@@ -131,6 +131,12 @@ class Engine {
   bool set_source_live_background(int source, const uint8_t* p, int fmt, int w, int h, size_t pitch, size_t uv, std::string* err);
   // device staging of max_batch `out` frames in the current format (host-buffer API), grown on demand; nullptr on error
   uint8_t* out_staging(std::string* err);
+  // Mask interval (include/backscrub_b200.h, bsb_set_mask_interval): segment every k-th frame of a camera, composite the
+  // frames between with its latest mask.  Host state only: which frames are segmented reaches the device as table data.
+  enum { MASK_INTERVAL_MAX = 256 };
+  bool set_mask_interval(int k, std::string* err);
+  // one source's interval: -1 follows set_mask_interval, else 1..MASK_INTERVAL_MAX
+  bool set_source_mask_interval(int source, int k, std::string* err);
   bool sync(std::string* err);
   bool reset_state(std::string* err);
 
@@ -253,6 +259,7 @@ class Engine {
     int live = 0;                    // frames that blend a live background: 0 none, 1 one image for every frame (a plain call
                                      // at frame_stride 0), 2 one per frame (the live table's descriptors say which)
     unsigned live_gclass = 0;        // the Gaussian launch classes of the blurred live frames
+    int m = 0;                       // frames segmented (the CNN batch); m == n: every frame, the parent path with no table
   };
   // the call blends a composite: it has a video output, or a BGR composite output.  A call that does not reads no
   // background and blurs nothing.
@@ -261,7 +268,8 @@ class Engine {
   size_t stage_bgra_off(const Call& c, const Plan& p) const { return blends(c, p) ? (size_t)max_batch_ * W_ * H_ * 3 : 0; }
   // flip_tail, native and nv12_staged (and the tail's staging); false with *err when a buffer cannot be grown
   bool plan_launch(const Call& c, Plan* p, std::string* err);
-  void enqueue_pre(const Call& c);
+  // pre-processing of the m segmented frames of c (gather: the device row of their call frames; null: all n, m == n)
+  void enqueue_pre(const Call& c, int m, const int* gather);
   PostArgs post_args(const Call& c, const Plan& p) const;
   bool yuyv_native(const Call& c, Plan p) const;
   // the call ends with k_tail (post -> stage -> flip, resize, YUYV / NV12): plain calls with a context flip or resize;
@@ -279,7 +287,14 @@ class Engine {
   void enqueue_feed(const Feed& f);
   bool refresh_bg_yuyv(std::string* err);
   void enqueue_cnn(int n, bool from_u8);
-  void enqueue_decision(int n, bool sources);
+  void enqueue_decision(int n, bool sources, int m, const SegRows& seg);
+  // the segmented frames of call c (the cadence of set_mask_interval) into rows [gather | cidx | lat] of max_batch_ ints
+  // each (SegRows); returns m.  A fed call segments every frame.
+  int segment(const Call& c, std::vector<int>* rows) const;
+  // the device segment rows of a call with held frames (p.m < c.n); null rows when every frame is segmented
+  SegRows seg_rows(const Call& c, const Plan& p) const;
+  // after a call is enqueued: the frame counters of the cadence move on (not for a fed call)
+  void count_frames(const Call& c);
   bool enqueue_post(const Call& c, const Plan& p);
   void enqueue_live(const Call& c, const Plan& p);
   // base of tensor t for the frames [frame_off_, ...) of the batch (frame_off_ != 0 only inside a sub-batched segment)
@@ -394,11 +409,20 @@ class Engine {
   // ---- independent sources (calls with ids) ----
   int n_sources_ = 0;
   uint8_t* src_state_ = nullptr;     // [n_sources][oh*ow] smoother state per source
-  // [7][max_batch]: source id of frame b | background-bank slot of frame b | camera-blur strength of frame b (0 = none) |
+  // [9][max_batch]: source id of frame b | background-bank slot of frame b | camera-blur strength of frame b (0 = none) |
   // flip code of frame b (bit 0 horizontal, bit 1 vertical; the source's own, or the context's) | geometry slot of frame b
   // (d_geo_ index) | 1 when frame b's filter is off (the source's own switch, or the context's) | live-background strength
-  // of frame b (0 = not blurred, or no live background), written before each launch
+  // of frame b (0 = not blurred, or no live background) | the segment rows gather and cidx (calls with held frames, else
+  // unused), written before each launch
   int* d_src_tab_ = nullptr;
+  enum { SRC_TAB_ROWS = 9, SRC_TAB_SEG = 7 };
+  // ---- mask interval ----
+  int mask_interval_ = 1;
+  long long plain_frames_ = 0;       // frames of plain calls since creation / reset_state: frame c is segmented iff c % k == 0
+  std::vector<int> src_interval_;    // per source: -1 = mask_interval_, else its own
+  std::vector<long long> src_frames_;   // per source: frames delivered since set_sources / reset_source
+  int src_interval(int s) const { return src_interval_[s] < 0 ? mask_interval_ : src_interval_[s]; }
+  int* d_seg_tab_ = nullptr;         // [3][max_batch] the segment rows of a plain call with held frames, written before its launch
   // ---- live backgrounds ----
   struct Live { const uint8_t* p = nullptr; int fmt = 0, w = 0, h = 0; size_t pitch = 0, uv = 0, stride = 0; int size = -1; };
   Live live_;                        // plain calls
@@ -467,9 +491,10 @@ class Engine {
   // an absent output does not matter), and the plan's mode (a plain and a sources graph over the same buffers are
   // different graphs), Gaussian classes (strengths within them replay), all-blur, flipped and passed (which frames flip or
   // are filtered off is table data), resized and the largest output size of the sources, which the tail's grid covers
-  // (which frame has which size is table data too), the output format, and whether frames blend live backgrounds, with
-  // the Gaussian classes they add (their images, sizes and strengths within the classes are the live table's data).  The
-  // rest of the plan is decided from these.
+  // (which frame has which size is table data too), the output format, whether frames blend live backgrounds, with
+  // the Gaussian classes they add (their images, sizes and strengths within the classes are the live table's data), and the
+  // CNN batch of a call with held frames (which frames are segmented is the segment rows' data).  The rest of the plan is
+  // decided from these.
   struct GraphKey {
     int n, fmt; const void* in; size_t pitch, uv, stride;
     const void* out; const void* video; const void* mask; size_t ostride, vstride, mstride;
@@ -478,10 +503,11 @@ class Engine {
         : n(c.n), fmt(c.fmt), in(c.in), pitch(c.pitch), uv(c.uv), stride(c.stride), out(c.out), video(c.video), mask(c.mask),
           ostride(c.out ? c.out_stride : 0), vstride(c.video ? c.video_stride : 0), mstride(c.mask ? c.mask_stride : 0),
           mode(p.mode), gclass(p.gclass), all_blur(p.all_blur), flipped(p.flipped), resized(p.resized), passed(p.passed),
-          out_px_max(px_max), bgra(p.bgra), live(p.live), live_gclass(p.live_gclass) {}
+          out_px_max(px_max), bgra(p.bgra), live(p.live), live_gclass(p.live_gclass), seg(p.m) {}
+    int seg;                         // the CNN batch m (n: every frame segmented, the parent's launches)
     auto tie() const {
       return std::tie(n, fmt, in, pitch, uv, stride, out, video, mask, ostride, vstride, mstride, mode, gclass, all_blur, flipped, resized,
-                      passed, out_px_max, bgra, live, live_gclass);
+                      passed, out_px_max, bgra, live, live_gclass, seg);
     }
     bool operator<(const GraphKey& r) const { return tie() < r.tie(); }
   };

@@ -185,30 +185,38 @@ void launch_resize_roi_swap(cudaStream_t s, int B, const uint8_t* frames, size_t
                             int roi_x, int roi_y, int roi_w, int roi_h, ResizeTab tab,
                             uint8_t* in_u8, int mw, int mh, int in_x, int in_y, int in_w, int in_h, bool area2x2,
                             int in_fmt = IN_BGR,     // IN_YUYV: camera YUYV frames (pitch W*2); IN_NV12: camera NV12 frames
-                            size_t uv_off = 0);      // (Y rows `frame_pitch` apart, UV plane at byte uv_off); converted per tap
+                            size_t uv_off = 0,       // (Y rows `frame_pitch` apart, UV plane at byte uv_off); converted per tap
+                            const int* gather = nullptr);   // DEVICE [B]: output frame b is input frame gather[b] (null: b)
 
 // lib/libbackscrub.cc:295-302: bilateralFilter(5,100,100) + convertTo(CV_32F, scale, offset)
 void launch_bilateral_norm(cudaStream_t s, int B, const uint8_t* in_u8, int mw, int mh,
                            const float* color_w, const float* space_w, float scale, float offset,
                            float* out_f32, uint8_t* out_u8_dbg);
 
+// Calls with held frames (bsb_set_mask_interval): DEVICE rows over the call's n frames, of which the B the CNN ran on are
+// segmented.  gather[i]: the call frame of segmented frame i; cidx[b]: call frame b's index among the segmented frames, -1
+// when it is held; lat[b] (plain calls): the index of the latest segmented frame at or before b, -1 when none.  A held
+// frame's ofinal is its smoother's state after the latest segmented frame.  Null rows: every frame is segmented (n == B).
+struct SegRows { int n = 0; const int* gather = nullptr; const int* cidx = nullptr; const int* lat = nullptr; };
+
 // lib/libbackscrub.cc:314-361: decision + 3-tap bit-shift IIR over B consecutive frames.
 // state: [oh*ow] persistent; ofinal: [B][oh][opitch] state after each frame (opitch >= ow: rows are padded to a
 // multiple of 16 bytes so the post kernel can fetch patches of it with TMA).
 void launch_decision_iir(cudaStream_t s, int model_type, int B, const float* model_out, int oh, int ow, int oc,
-                         uint8_t* state, uint8_t* ofinal, int opitch);
+                         uint8_t* state, uint8_t* ofinal, int opitch, const SegRows& seg = SegRows{});
 // DeepLab: the graph ends with RESIZE_BILINEAR 33x33x21 -> 257x257x21 and the decision is an argmax over the 21 classes of
 // every output pixel.  This variant interpolates the 21 values of a pixel on the fly (the exact expression of the resize
 // kernel) instead of writing and re-reading the 5.5 MB-per-frame tensor.
 void launch_decision_up_iir(cudaStream_t s, int B, const float* low, int ih, int iw, int ld, bool align_corners, bool half_pixel,
-                            int oh, int ow, uint8_t* state, uint8_t* ofinal, int opitch);
+                            int oh, int ow, uint8_t* state, uint8_t* ofinal, int opitch, const SegRows& seg = SegRows{});
 // Independent sources: frame b of the batch belongs to source src[b] (DEVICE table [B], ids distinct within the call) and
 // advances that source's state, states: [n_sources][oh*ow].  One step of the IIR per frame, every frame in parallel.
+// cidx (SegRows::cidx, B = the call's frames): frame b reads segmented frame cidx[b] of model_out, or holds its state.
 void launch_decision_sources(cudaStream_t s, int model_type, int B, const float* model_out, int oh, int ow, int oc,
-                             uint8_t* states, const int* src, uint8_t* ofinal, int opitch);
+                             uint8_t* states, const int* src, uint8_t* ofinal, int opitch, const int* cidx = nullptr);
 // DeepLab form with the final 33 -> 257 resize folded in (as launch_decision_up_iir)
 void launch_decision_up_sources(cudaStream_t s, int B, const float* low, int ih, int iw, int ld, bool align_corners, bool half_pixel,
-                                int oh, int ow, uint8_t* states, const int* src, uint8_t* ofinal, int opitch);
+                                int oh, int ow, uint8_t* states, const int* src, uint8_t* ofinal, int opitch, const int* cidx = nullptr);
 // source coordinate / neighbours of RESIZE_BILINEAR (TF/lite/kernels/internal/reference/resize_bilinear.h:29-57)
 BSB_D void bsb_resize_interp(float value, float scale, bool half_pixel, int in_size, float* scaled, int* lo, int* hi) {
   *scaled = half_pixel ? (value + 0.5f) * scale - 0.5f : value * scale;

@@ -39,18 +39,20 @@ BSB_D size_t bg_frame_offset(const PostArgs& a, int b) {
 // bytes apart, the UV plane at byte `uv_off` of the frame).  Every tap of a camera frame is first converted the way
 // cv::cvtColor(COLOR_YUV2BGR_YUYV / _NV12) would have (cv::VideoCapture's conversion, app/deepseg.cc:553), so the result
 // equals converting the whole frame first — without materialising the BGR frame.
-template <int FMT>
+// GATHER (calls with held frames, bsb_set_mask_interval): output frame b is camera frame gather[b] of the call.
+template <int FMT, bool GATHER>
 __global__ void __launch_bounds__(256) k_resize_roi_swap(int B, const uint8_t* frames, size_t frame_stride, size_t pitch,
                                                          int roi_x, int roi_y, int roi_w, int roi_h, ResizeTab t,
                                                          uint8_t* in_u8, int mw, int mh, int in_x, int in_y, int in_w, int in_h,
-                                                         bool area2x2, size_t uv_off) {
+                                                         bool area2x2, size_t uv_off, const int* gather) {
   const long total = (long)B * in_w * in_h;
   const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= total) return;
   const int dx = (int)(idx % in_w), dy = (int)((idx / in_w) % in_h), b = (int)(idx / ((long)in_w * in_h));
+  const int fb = GATHER ? __ldg(gather + b) : b;
   uint8_t px[3];
   if (FMT == IN_NV12) {
-    const uint8_t* img = frames + (size_t)b * frame_stride;
+    const uint8_t* img = frames + (size_t)fb * frame_stride;
     int p00[3], p01[3], p10[3], p11[3];
     if (area2x2) {
       const int y0 = roi_y + 2 * dy, x0 = roi_x + 2 * dx;
@@ -69,7 +71,7 @@ __global__ void __launch_bounds__(256) k_resize_roi_swap(int B, const uint8_t* f
       for (int c = 0; c < 3; ++c) px[c] = lin_v(p00[c] * a0 + p01[c] * a1, p10[c] * a0 + p11[c] * a1, b0, b1);
     }
   } else if (FMT == IN_YUYV) {
-    const uint8_t* img = frames + (size_t)b * frame_stride;
+    const uint8_t* img = frames + (size_t)fb * frame_stride;
     if (area2x2) {
       int p00[3], p01[3], p10[3], p11[3];
       const uint8_t* s0 = img + (size_t)(roi_y + 2 * dy) * pitch;
@@ -91,7 +93,7 @@ __global__ void __launch_bounds__(256) k_resize_roi_swap(int B, const uint8_t* f
       for (int c = 0; c < 3; ++c) px[c] = lin_v(p00[c] * a0 + p01[c] * a1, p10[c] * a0 + p11[c] * a1, b0, b1);
     }
   } else {
-    const uint8_t* roi = frames + (size_t)b * frame_stride + (size_t)roi_y * pitch + (size_t)roi_x * 3;
+    const uint8_t* roi = frames + (size_t)fb * frame_stride + (size_t)roi_y * pitch + (size_t)roi_x * 3;
     if (area2x2) {
       const uint8_t* s0 = roi + (size_t)(2 * dy) * pitch + (size_t)(2 * dx) * 3;
       const uint8_t* s1 = s0 + pitch;
@@ -114,15 +116,15 @@ __global__ void __launch_bounds__(256) k_resize_roi_swap(int B, const uint8_t* f
 void launch_resize_roi_swap(cudaStream_t s, int B, const uint8_t* frames, size_t frame_stride, size_t frame_pitch,
                             int roi_x, int roi_y, int roi_w, int roi_h, ResizeTab tab,
                             uint8_t* in_u8, int mw, int mh, int in_x, int in_y, int in_w, int in_h, bool area2x2, int in_fmt,
-                            size_t uv_off) {
+                            size_t uv_off, const int* gather) {
   const long total = (long)B * in_w * in_h;
   const dim3 grid((unsigned)((total + 255) / 256));
-  if (in_fmt == IN_NV12) BSB_LAUNCH(k_resize_roi_swap<IN_NV12>, grid, dim3(256), 0, s, B, frames, frame_stride, frame_pitch,
-                                    roi_x, roi_y, roi_w, roi_h, tab, in_u8, mw, mh, in_x, in_y, in_w, in_h, area2x2, uv_off);
-  else if (in_fmt == IN_YUYV) BSB_LAUNCH(k_resize_roi_swap<IN_YUYV>, grid, dim3(256), 0, s, B, frames, frame_stride, frame_pitch,
-                                         roi_x, roi_y, roi_w, roi_h, tab, in_u8, mw, mh, in_x, in_y, in_w, in_h, area2x2, uv_off);
-  else BSB_LAUNCH(k_resize_roi_swap<IN_BGR>, grid, dim3(256), 0, s, B, frames, frame_stride, frame_pitch,
-                  roi_x, roi_y, roi_w, roi_h, tab, in_u8, mw, mh, in_x, in_y, in_w, in_h, area2x2, uv_off);
+  auto k = k_resize_roi_swap<IN_BGR, false>;
+  if (in_fmt == IN_NV12) k = gather ? k_resize_roi_swap<IN_NV12, true> : k_resize_roi_swap<IN_NV12, false>;
+  else if (in_fmt == IN_YUYV) k = gather ? k_resize_roi_swap<IN_YUYV, true> : k_resize_roi_swap<IN_YUYV, false>;
+  else if (gather) k = k_resize_roi_swap<IN_BGR, true>;
+  BSB_LAUNCH(k, grid, dim3(256), 0, s, B, frames, frame_stride, frame_pitch, roi_x, roi_y, roi_w, roi_h, tab, in_u8, mw, mh, in_x, in_y,
+             in_w, in_h, area2x2, uv_off, gather);
   count_launch();
 }
 
@@ -220,24 +222,36 @@ BSB_D unsigned decide(int model_type, const float* t) {
 
 // The per-frame decisions of a pixel are independent (computed 8 at a time so their loads
 // overlap); only the 3-tap state update is sequential, and it is pure ALU on a bit mask.
+// GATHER (calls with held frames, bsb_set_mask_interval): out_f holds the B segmented frames of the call's nf frames;
+// call frame b advances the state on segmented frame cidx[b], or holds it (cidx[b] < 0), and stores it either way.
+template <bool GATHER>
 __global__ void __launch_bounds__(128) k_decision_iir(int model_type, int B, const float* out_f, int npix, int oc,
-                                                      uint8_t* state, uint8_t* ofinal, int ow, int opitch, int oframe) {
+                                                      uint8_t* state, uint8_t* ofinal, int ow, int opitch, int oframe, int nf,
+                                                      const int* cidx) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= npix) return;
   const int opos = (n / ow) * opitch + (n % ow);      // row-padded position inside one frame of ofinal
   unsigned st = state[n];
-  for (int b0 = 0; b0 < B; b0 += 8) {
-    unsigned bits = 0;
+  if (GATHER) {
+    for (int b = 0; b < nf; ++b) {
+      const int j = __ldg(cidx + b);
+      if (j >= 0) st = (decide(model_type, out_f + ((size_t)j * npix + n) * oc) ? 0xE0u : 0u) | (st >> 3);
+      ofinal[(size_t)b * oframe + opos] = (uint8_t)st;
+    }
+  } else {
+    for (int b0 = 0; b0 < B; b0 += 8) {
+      unsigned bits = 0;
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
-      if (b0 + j < B) bits |= decide(model_type, out_f + ((size_t)(b0 + j) * npix + n) * oc) << j;
+      for (int j = 0; j < 8; ++j)
+        if (b0 + j < B) bits |= decide(model_type, out_f + ((size_t)(b0 + j) * npix + n) * oc) << j;
 #pragma unroll
-    for (int j = 0; j < 8; ++j)
-      if (b0 + j < B) {
-        const unsigned val = ((bits >> j) & 1u) ? 255u : 0u;
-        st = (val & 0xE0u) | (st >> 3);
-        ofinal[(size_t)(b0 + j) * oframe + opos] = (uint8_t)st;
-      }
+      for (int j = 0; j < 8; ++j)
+        if (b0 + j < B) {
+          const unsigned val = ((bits >> j) & 1u) ? 255u : 0u;
+          st = (val & 0xE0u) | (st >> 3);
+          ofinal[(size_t)(b0 + j) * oframe + opos] = (uint8_t)st;
+        }
+    }
   }
   state[n] = (uint8_t)st;
 }
@@ -253,44 +267,72 @@ __global__ void __launch_bounds__(128) k_decision_iir(int model_type, int B, con
 // the barrier, written (by the owner of frame B-1) after it.
 constexpr int DEC_PX = 32, DEC_WARPS = 8;
 
+// the state after decision j of d ([B][32], this thread's column tx), entered with state s_in
+BSB_D unsigned decision_window(const uint8_t* d, int tx, int j, unsigned s_in) {
+  unsigned st = d[j * DEC_PX + tx] ? 0xE0u : 0u;
+  if (j >= 1) st |= d[(j - 1) * DEC_PX + tx] ? 0x1Cu : 0u; else st |= s_in >> 3;
+  if (j >= 2) st |= d[(j - 2) * DEC_PX + tx] ? 0x03u : 0u; else if (j == 1) st |= s_in >> 6;
+  return st;
+}
+
 BSB_D void decision_window_store(const uint8_t* d, int tx, int ty, int B, unsigned s_in, uint8_t* state_px, uint8_t* ofinal_px, int oframe) {
   for (int b = ty; b < B; b += DEC_WARPS) {
-    unsigned st = d[b * DEC_PX + tx] ? 0xE0u : 0u;
-    if (b >= 1) st |= d[(b - 1) * DEC_PX + tx] ? 0x1Cu : 0u; else st |= s_in >> 3;
-    if (b >= 2) st |= d[(b - 2) * DEC_PX + tx] ? 0x03u : 0u; else if (b == 1) st |= s_in >> 6;
+    const unsigned st = decision_window(d, tx, b, s_in);
     ofinal_px[(size_t)b * oframe] = (uint8_t)st;
     if (b == B - 1) *state_px = (uint8_t)st;
   }
 }
 
+// Calls with held frames: d holds the decisions of the call's segmented frames only, and call frame b of nf stores the
+// state after its latest segmented frame lat[b] (s_in when none precedes it).  The last call frame's latest segmented
+// frame is the last one, so its state is the new state byte (s_in again when no frame is segmented).
+BSB_D void decision_window_store_held(const uint8_t* d, int tx, int ty, int nf, const int* lat, unsigned s_in, uint8_t* state_px,
+                                      uint8_t* ofinal_px, int oframe) {
+  for (int b = ty; b < nf; b += DEC_WARPS) {
+    const int j = __ldg(lat + b);
+    const unsigned st = j < 0 ? s_in : decision_window(d, tx, j, s_in);
+    ofinal_px[(size_t)b * oframe] = (uint8_t)st;
+    if (b == nf - 1) *state_px = (uint8_t)st;
+  }
+}
+
+template <bool GATHER>
 __global__ void __launch_bounds__(DEC_PX * DEC_WARPS) k_decision_par(int model_type, int B, const float* out_f, int npix, int oc,
-                                                                     uint8_t* state, uint8_t* ofinal, int ow, int opitch, int oframe) {
+                                                                     uint8_t* state, uint8_t* ofinal, int ow, int opitch, int oframe,
+                                                                     int nf, const int* lat) {
   BSB_DYN_SMEM(smem_raw);
   uint8_t* d = reinterpret_cast<uint8_t*>(smem_raw);               // [B][32] decisions
   const int tx = threadIdx.x % DEC_PX, ty = threadIdx.x / DEC_PX;
   const int n = blockIdx.x * DEC_PX + tx;
   const bool valid = n < npix;
-  const unsigned s_in = valid ? state[n] : 0u;
+  // held-frame calls park the entry state behind the decisions (row B), so it is not live across the decision loop
+  const unsigned s_in = (!GATHER && valid) ? state[n] : 0u;
   if (valid) {
+    if (GATHER && ty == 0) d[B * DEC_PX + tx] = state[n];
 #pragma unroll 4
     for (int b = ty; b < B; b += DEC_WARPS) d[b * DEC_PX + tx] = (uint8_t)decide(model_type, out_f + ((size_t)b * npix + n) * oc);
   }
   __syncthreads();
   if (!valid) return;
-  decision_window_store(d, tx, ty, B, s_in, state + n, ofinal + (n / ow) * opitch + (n % ow), oframe);
+  if (GATHER) decision_window_store_held(d, tx, ty, nf, lat, d[B * DEC_PX + tx], state + n, ofinal + (n / ow) * opitch + (n % ow), oframe);
+  else decision_window_store(d, tx, ty, B, s_in, state + n, ofinal + (n / ow) * opitch + (n % ow), oframe);
 }
 
 void launch_decision_iir(cudaStream_t s, int model_type, int B, const float* model_out, int oh, int ow, int oc,
-                         uint8_t* state, uint8_t* ofinal, int opitch) {
+                         uint8_t* state, uint8_t* ofinal, int opitch, const SegRows& seg) {
   const int npix = oh * ow;
-  if (tuning().dec_par && (size_t)B * DEC_PX <= 48 * 1024) {
-    BSB_LAUNCH(k_decision_par, dim3((unsigned)ceil_div(npix, DEC_PX)), dim3(DEC_PX * DEC_WARPS), (size_t)B * DEC_PX, s, model_type, B, model_out,
-               npix, oc, state, ofinal, ow, opitch, oh * opitch);
+  const bool held = seg.cidx != nullptr;
+  const size_t smem = (size_t)(B + (held ? 1 : 0)) * DEC_PX;
+  if (tuning().dec_par && smem <= 48 * 1024) {
+    auto k = held ? k_decision_par<true> : k_decision_par<false>;
+    BSB_LAUNCH(k, dim3((unsigned)ceil_div(npix, DEC_PX)), dim3(DEC_PX * DEC_WARPS), smem, s, model_type, B, model_out,
+               npix, oc, state, ofinal, ow, opitch, oh * opitch, seg.n, seg.lat);
     count_launch();
     return;
   }
-  BSB_LAUNCH(k_decision_iir, dim3((unsigned)ceil_div(npix, 128)), dim3(128), 0, s, model_type, B, model_out, npix, oc, state, ofinal,
-             ow, opitch, oh * opitch);
+  auto k = held ? k_decision_iir<true> : k_decision_iir<false>;
+  BSB_LAUNCH(k, dim3((unsigned)ceil_div(npix, 128)), dim3(128), 0, s, model_type, B, model_out, npix, oc, state, ofinal,
+             ow, opitch, oh * opitch, seg.n, seg.cidx);
   count_launch();
 }
 
@@ -325,54 +367,72 @@ BSB_D unsigned up_decide(const float* f, const UpTap& t) {
   return (maxpos == 15) ? 0u : 1u;
 }
 
+template <bool GATHER>
 __global__ void __launch_bounds__(128) k_decision_up_iir(int B, const float* low, int ih, int iw, int ld, float hs, float ws, bool half_pixel,
-                                                         int oh, int ow, uint8_t* state, uint8_t* ofinal, int opitch, int oframe) {
+                                                         int oh, int ow, uint8_t* state, uint8_t* ofinal, int opitch, int oframe, int nf,
+                                                         const int* cidx) {
   const int n = blockIdx.x * blockDim.x + threadIdx.x;
   if (n >= oh * ow) return;
   const int y = n / ow, x = n - y * ow;
   const UpTap t = up_tap(y, x, ih, iw, ld, hs, ws, half_pixel);
   const int opos = y * opitch + x;
   unsigned st = state[n];
-  for (int b = 0; b < B; ++b) {
-    const unsigned val = up_decide(low + (size_t)b * ih * iw * ld, t) ? 255u : 0u;
-    st = (val & 0xE0u) | (st >> 3);
-    ofinal[(size_t)b * oframe + opos] = (uint8_t)st;
+  if (GATHER) {                                       // as k_decision_iir<true>
+    for (int b = 0; b < nf; ++b) {
+      const int j = __ldg(cidx + b);
+      if (j >= 0) st = (up_decide(low + (size_t)j * ih * iw * ld, t) ? 0xE0u : 0u) | (st >> 3);
+      ofinal[(size_t)b * oframe + opos] = (uint8_t)st;
+    }
+  } else {
+    for (int b = 0; b < B; ++b) {
+      const unsigned val = up_decide(low + (size_t)b * ih * iw * ld, t) ? 255u : 0u;
+      st = (val & 0xE0u) | (st >> 3);
+      ofinal[(size_t)b * oframe + opos] = (uint8_t)st;
+    }
   }
   state[n] = (uint8_t)st;
 }
 
 // frame-parallel form (see k_decision_par): a block = 32 output pixels x all B frames
+template <bool GATHER>
 __global__ void __launch_bounds__(DEC_PX * DEC_WARPS) k_decision_up_par(int B, const float* low, int ih, int iw, int ld, float hs, float ws, bool half_pixel,
-                                                                        int oh, int ow, uint8_t* state, uint8_t* ofinal, int opitch, int oframe) {
+                                                                        int oh, int ow, uint8_t* state, uint8_t* ofinal, int opitch, int oframe,
+                                                                        int nf, const int* lat) {
   BSB_DYN_SMEM(smem_raw);
   uint8_t* d = reinterpret_cast<uint8_t*>(smem_raw);
   const int tx = threadIdx.x % DEC_PX, ty = threadIdx.x / DEC_PX;
   const int n = blockIdx.x * DEC_PX + tx;
   const bool valid = n < oh * ow;
-  const unsigned s_in = valid ? state[n] : 0u;
+  const unsigned s_in = (!GATHER && valid) ? state[n] : 0u;       // held-frame calls: row B, as in k_decision_par
   const int y = valid ? n / ow : 0, x = valid ? n - y * ow : 0;
   if (valid) {
+    if (GATHER && ty == 0) d[B * DEC_PX + tx] = state[n];
     const UpTap t = up_tap(y, x, ih, iw, ld, hs, ws, half_pixel);
     for (int b = ty; b < B; b += DEC_WARPS) d[b * DEC_PX + tx] = (uint8_t)up_decide(low + (size_t)b * ih * iw * ld, t);
   }
   __syncthreads();
   if (!valid) return;
-  decision_window_store(d, tx, ty, B, s_in, state + n, ofinal + y * opitch + x, oframe);
+  if (GATHER) decision_window_store_held(d, tx, ty, nf, lat, d[B * DEC_PX + tx], state + n, ofinal + y * opitch + x, oframe);
+  else decision_window_store(d, tx, ty, B, s_in, state + n, ofinal + y * opitch + x, oframe);
 }
 
 void launch_decision_up_iir(cudaStream_t s, int B, const float* low, int ih, int iw, int ld, bool align_corners, bool half_pixel,
-                            int oh, int ow, uint8_t* state, uint8_t* ofinal, int opitch) {
+                            int oh, int ow, uint8_t* state, uint8_t* ofinal, int opitch, const SegRows& seg) {
   float hs = (float)ih / (float)oh, ws = (float)iw / (float)ow;
   if (align_corners && oh > 1) hs = (float)(ih - 1) / (float)(oh - 1);
   if (align_corners && ow > 1) ws = (float)(iw - 1) / (float)(ow - 1);
-  if (tuning().dec_par && (size_t)B * DEC_PX <= 48 * 1024) {
-    BSB_LAUNCH(k_decision_up_par, dim3((unsigned)ceil_div(oh * ow, DEC_PX)), dim3(DEC_PX * DEC_WARPS), (size_t)B * DEC_PX, s, B, low, ih, iw, ld, hs, ws,
-               half_pixel, oh, ow, state, ofinal, opitch, oh * opitch);
+  const bool held = seg.cidx != nullptr;
+  const size_t smem = (size_t)(B + (held ? 1 : 0)) * DEC_PX;
+  if (tuning().dec_par && smem <= 48 * 1024) {
+    auto k = held ? k_decision_up_par<true> : k_decision_up_par<false>;
+    BSB_LAUNCH(k, dim3((unsigned)ceil_div(oh * ow, DEC_PX)), dim3(DEC_PX * DEC_WARPS), smem, s, B, low, ih, iw, ld, hs, ws,
+               half_pixel, oh, ow, state, ofinal, opitch, oh * opitch, seg.n, seg.lat);
     count_launch();
     return;
   }
-  BSB_LAUNCH(k_decision_up_iir, dim3((unsigned)ceil_div(oh * ow, 128)), dim3(128), 0, s, B, low, ih, iw, ld, hs, ws, half_pixel, oh, ow, state,
-             ofinal, opitch, oh * opitch);
+  auto k = held ? k_decision_up_iir<true> : k_decision_up_iir<false>;
+  BSB_LAUNCH(k, dim3((unsigned)ceil_div(oh * ow, 128)), dim3(128), 0, s, B, low, ih, iw, ld, hs, ws, half_pixel, oh, ow, state,
+             ofinal, opitch, oh * opitch, seg.n, seg.cidx);
   count_launch();
 }
 
@@ -384,44 +444,56 @@ void launch_decision_up_iir(cudaStream_t s, int B, const float* low, int ih, int
 // ---------------------------------------------------------------------------
 constexpr int DEC_SRC_T = 128;
 
+// GATHER (calls with held frames): the grid still covers the call's frames; frame b is segmented frame cidx[b] of out_f,
+// or, at cidx[b] < 0, held: its ofinal is its source's state as it stands (no frame of the launch writes that state, the
+// ids being distinct).
+template <bool GATHER>
 __global__ void __launch_bounds__(DEC_SRC_T) k_decision_sources(int model_type, const float* out_f, int npix, int oc, uint8_t* states,
-                                                                const int* src, uint8_t* ofinal, int ow, int opitch, int oframe) {
+                                                                const int* src, uint8_t* ofinal, int ow, int opitch, int oframe,
+                                                                const int* cidx) {
   const int n = blockIdx.x * DEC_SRC_T + threadIdx.x, b = blockIdx.y;
   if (n >= npix) return;
   uint8_t* sp = states + (size_t)__ldg(src + b) * npix + n;
-  const unsigned st = (decide(model_type, out_f + ((size_t)b * npix + n) * oc) ? 0xE0u : 0u) | ((unsigned)*sp >> 3);
+  const int j = GATHER ? __ldg(cidx + b) : b;
+  if (GATHER && j < 0) { ofinal[(size_t)b * oframe + (n / ow) * opitch + (n % ow)] = *sp; return; }
+  const unsigned st = (decide(model_type, out_f + ((size_t)j * npix + n) * oc) ? 0xE0u : 0u) | ((unsigned)*sp >> 3);
   ofinal[(size_t)b * oframe + (n / ow) * opitch + (n % ow)] = (uint8_t)st;
   *sp = (uint8_t)st;
 }
 
+template <bool GATHER>
 __global__ void __launch_bounds__(DEC_SRC_T) k_decision_up_sources(const float* low, int ih, int iw, int ld, float hs, float ws, bool half_pixel,
                                                                    int oh, int ow, uint8_t* states, const int* src, uint8_t* ofinal, int opitch,
-                                                                   int oframe) {
+                                                                   int oframe, const int* cidx) {
   const int n = blockIdx.x * DEC_SRC_T + threadIdx.x, b = blockIdx.y;
   if (n >= oh * ow) return;
   const int y = n / ow, x = n - y * ow;
   uint8_t* sp = states + (size_t)__ldg(src + b) * oh * ow + n;
-  const unsigned d = up_decide(low + (size_t)b * ih * iw * ld, up_tap(y, x, ih, iw, ld, hs, ws, half_pixel));
+  const int j = GATHER ? __ldg(cidx + b) : b;
+  if (GATHER && j < 0) { ofinal[(size_t)b * oframe + y * opitch + x] = *sp; return; }
+  const unsigned d = up_decide(low + (size_t)j * ih * iw * ld, up_tap(y, x, ih, iw, ld, hs, ws, half_pixel));
   const unsigned st = (d ? 0xE0u : 0u) | ((unsigned)*sp >> 3);
   ofinal[(size_t)b * oframe + y * opitch + x] = (uint8_t)st;
   *sp = (uint8_t)st;
 }
 
 void launch_decision_sources(cudaStream_t s, int model_type, int B, const float* model_out, int oh, int ow, int oc,
-                             uint8_t* states, const int* src, uint8_t* ofinal, int opitch) {
+                             uint8_t* states, const int* src, uint8_t* ofinal, int opitch, const int* cidx) {
   const int npix = oh * ow;
-  BSB_LAUNCH(k_decision_sources, dim3((unsigned)ceil_div(npix, DEC_SRC_T), (unsigned)B), dim3(DEC_SRC_T), 0, s, model_type, model_out, npix, oc,
-             states, src, ofinal, ow, opitch, oh * opitch);
+  auto k = cidx ? k_decision_sources<true> : k_decision_sources<false>;
+  BSB_LAUNCH(k, dim3((unsigned)ceil_div(npix, DEC_SRC_T), (unsigned)B), dim3(DEC_SRC_T), 0, s, model_type, model_out, npix, oc,
+             states, src, ofinal, ow, opitch, oh * opitch, cidx);
   count_launch();
 }
 
 void launch_decision_up_sources(cudaStream_t s, int B, const float* low, int ih, int iw, int ld, bool align_corners, bool half_pixel,
-                                int oh, int ow, uint8_t* states, const int* src, uint8_t* ofinal, int opitch) {
+                                int oh, int ow, uint8_t* states, const int* src, uint8_t* ofinal, int opitch, const int* cidx) {
   float hs = (float)ih / (float)oh, ws = (float)iw / (float)ow;
   if (align_corners && oh > 1) hs = (float)(ih - 1) / (float)(oh - 1);
   if (align_corners && ow > 1) ws = (float)(iw - 1) / (float)(ow - 1);
-  BSB_LAUNCH(k_decision_up_sources, dim3((unsigned)ceil_div(oh * ow, DEC_SRC_T), (unsigned)B), dim3(DEC_SRC_T), 0, s, low, ih, iw, ld, hs, ws,
-             half_pixel, oh, ow, states, src, ofinal, opitch, oh * opitch);
+  auto k = cidx ? k_decision_up_sources<true> : k_decision_up_sources<false>;
+  BSB_LAUNCH(k, dim3((unsigned)ceil_div(oh * ow, DEC_SRC_T), (unsigned)B), dim3(DEC_SRC_T), 0, s, low, ih, iw, ld, hs, ws,
+             half_pixel, oh, ow, states, src, ofinal, opitch, oh * opitch, cidx);
   count_launch();
 }
 

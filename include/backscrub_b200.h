@@ -142,6 +142,37 @@ BSB_API int bsb_set_filter(bsb_ctx* ctx, int active);
  * bsb_last_error() message and changes nothing. */
 enum { BSB_OUT_BGR = 0, BSB_OUT_BGRA = 1 };
 BSB_API int bsb_set_out_format(bsb_ctx* ctx, int format);
+/* Mask interval.  The reference composites every camera frame with whatever mask its AI thread made last
+ * (app/deepseg.cc:627-661, `ai.get_output_mask(mask)`), so a 60 fps camera is routinely composited with masks made at a
+ * lower rate.  These setters make that trade explicit: fewer frames pay for pre-processing and the CNN, and no output
+ * frame is dropped.
+ *   Segmented frame: pre-processing, the CNN, the decision and one smoother step, exactly as at interval 1.
+ *   Held frame: none of those.  Its small mask (ofinal) is the smoother state its camera holds now, i.e. the state after
+ *     the camera's latest segmented frame; upsampling, blur, blend, flip, resize, BGRA, YUYV / NV12 and the mask output
+ *     then proceed as usual.  So its W x H mask is byte for byte that of the latest segmented frame, and its composite is
+ *     that mask applied to the new camera frame.
+ *   Plain calls: the context counts the frames of its plain calls from 0 (at creation and after bsb_reset_state); frame c
+ *     is segmented iff c % k == 0.  The cadence runs across calls and across the chunks of a split host-buffer call; held
+ *     frames before a call's first segmented frame hold the state the previous call left.
+ *   Sources calls: source s counts the frames it delivers from 0 (at bsb_set_sources and bsb_reset_source(s)); its frame f
+ *     is segmented iff f == 0 || (f + s) % k_s == 0, k_s its effective interval.  The id as the phase staggers sources with
+ *     consecutive ids (64 sources at k = 2 segment 32 frames per call), and a new or reset camera never composites with an
+ *     empty mask.
+ *   A new interval applies from the next frame; no counter is reset.  Frames with their filter off follow the cadence
+ *   like any other (segmentation still runs).  Backgrounds, flips, sizes and formats are per call frame as before, and
+ *   ring cursors move as before.  Fed calls (bsb_test_feed) ignore the interval and leave the counters unchanged.  A call
+ *   with stage callbacks fires each once, also when no frame of it is segmented.  The library's own mask-only users
+ *   (bs_maskgen_process, the bsb_calcmask_* front end) never set an interval and so segment every frame.
+ *   Introspection: bsb_get_tensor_frame and stages 0 / 1 of bsb_get_stage_u8 index the call's i-th segmented frame;
+ *   stage 2 (ofinal) and the mask index the call frame.
+ *   Host state only: which frames are segmented reaches the device as table data with the call, so a periodic cadence
+ *   replays at most k captured graphs per buffer set (one per CNN batch size it produces).
+ * interval: 1..256, default 1 (every frame).  Out of range returns 0 with a bsb_last_error() message and changes nothing. */
+BSB_API int bsb_set_mask_interval(bsb_ctx* ctx, int interval);
+/* One source's interval: -1 follows bsb_set_mask_interval (including later changes), else 1..256.  bsb_set_sources resets
+ * every source to -1; bsb_reset_source keeps it.  No bsb_set_sources yet, a source id out of range or an interval out of
+ * range returns 0 with a bsb_last_error() message and changes nothing. */
+BSB_API int bsb_set_source_mask_interval(bsb_ctx* ctx, int source, int interval);
 /* Live backgrounds (the reference's `-b` takes any OpenCV source and blends its newest frame every loop iteration,
  * app/deepseg.cc:522-524,648-661): device images the caller already holds (decoded video surfaces, screen captures, a
  * second camera) are resized, blurred and blended inside the call, with no host copy and no launch outside it.
@@ -454,14 +485,15 @@ BSB_API int bsb_infer(bsb_ctx* ctx, int n_frames, const float* input, float* out
 /* copy an intermediate activation (frame 0) to host; needs BSB_FLAG_KEEP_TENSORS.
  * Returns the element count, 0 if the tensor was folded away, -1 on error. */
 BSB_API long bsb_get_tensor(bsb_ctx* ctx, int tensor_index, float* out, long capacity);
-/* the same for frame `frame` of the last batch */
+/* the same for frame `frame` of the last batch (with a mask interval: its frame-th segmented frame) */
 BSB_API long bsb_get_tensor_frame(bsb_ctx* ctx, int tensor_index, int frame, float* out, long capacity);
 /* the 1x1 convolutions planned for the tensor cores, 9 ints per step into rows (at most `capacity` steps): TFLite op
  * index, input, output and residual tensor (-1: none), K, N, act1, act2, act3 of the step's epilogue
  * out = act3(act2(act1(in * W^T + bias)) + residual).  Returns the number of such steps, -1 on error. */
 BSB_API int bsb_tc_steps(bsb_ctx* ctx, int* rows, int capacity);
 /* stage buffers of the last call, frame `frame`: which = 0 model-sized RGB u8 (after resize +
- * BGR2RGB), 1 bilateral-filtered u8, 2 ofinal (IIR state after that frame) */
+ * BGR2RGB), 1 bilateral-filtered u8, 2 ofinal (IIR state after that frame).  With a mask interval (bsb_set_mask_interval)
+ * stages 0 and 1 index the call's segmented frames (the frame-th of them), stage 2 the call frame. */
 BSB_API long bsb_get_stage_u8(bsb_ctx* ctx, int which, int frame, uint8_t* out, long capacity);
 /* Test entry point: feed chosen values to the decision or the post stage of the next composite call, so that their
  * kernels can be checked on constructed inputs (ties, overflows, thresholds, single-pixel masks) rather than on what the
