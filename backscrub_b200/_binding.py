@@ -39,6 +39,7 @@ SYMBOLS = [
     "bsb_set_filter", "bsb_set_source_filter", "bsb_set_out_format",
     "bsb_set_live_background", "bsb_set_source_live_background",
     "bsb_set_mask_interval", "bsb_set_source_mask_interval",
+    "bsb_set_framing", "bsb_set_framing_auto", "bsb_set_source_framing", "bsb_get_framing",
     "bsb_test_feed_shape", "bsb_test_feed",
 ]
 
@@ -148,6 +149,10 @@ def bind(path: str) -> C.CDLL:
     L.bsb_set_source_filter.argtypes = [C.c_void_p, C.c_int, C.c_int]
     L.bsb_set_mask_interval.argtypes = [C.c_void_p, C.c_int]
     L.bsb_set_source_mask_interval.argtypes = [C.c_void_p, C.c_int, C.c_int]
+    L.bsb_set_framing.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
+    L.bsb_set_framing_auto.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
+    L.bsb_set_source_framing.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
+    L.bsb_get_framing.argtypes = [C.c_void_p, C.c_int, i32p]
     L.bsb_set_source_output.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
     L.bsb_source_output_size.argtypes = [C.c_void_p, C.c_int, i32p, i32p]
     L.bsb_composite_sources.argtypes = [C.c_void_p, C.c_int, i32p, C.c_void_p, C.c_size_t, C.c_size_t, C.c_void_p, C.c_size_t,

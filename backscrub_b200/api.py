@@ -120,6 +120,39 @@ class MaskGen:
         if not self._lib.bsb_set_mask_interval(self._h, int(k)):
             self._fail("bsb_set_mask_interval")
 
+    _FRAMING = {"off": 0, "rect": 1, "auto": 2}
+
+    def _framing_args(self, what, mode, rect):
+        if mode not in self._FRAMING:
+            raise BackscrubError(f"{what}: unknown framing mode {mode!r} (\"off\", \"rect\" or \"auto\")")
+        x, y, w, h = rect if rect is not None else (0, 0, 0, 0)
+        return self._FRAMING[mode], int(x), int(y), int(w), int(h)
+
+    def set_framing(self, mode: str = "off", rect=None):
+        """framing of every frame's output (include/backscrub_b200.h, bsb_set_framing): "off" (the whole frame), "rect"
+        (the crop rect = (x, y, w, h) of the camera frame) or "auto" (a crop that follows the person the mask finds)"""
+        if not self._lib.bsb_set_framing(self._h, *self._framing_args("bsb_set_framing", mode, rect)):
+            self._fail("bsb_set_framing")
+
+    def set_framing_auto(self, max_zoom_pct: int = 300, margin_pct: int = 10, speed: int = 32):
+        """auto-framing parameters: zoom limit 100..1000 %, headroom and side margin 0..100 % of the person's height,
+        speed 1..256 (1/256 of the remaining distance per frame; 256 jumps)"""
+        if not self._lib.bsb_set_framing_auto(self._h, int(max_zoom_pct), int(margin_pct), int(speed)):
+            self._fail("bsb_set_framing_auto")
+
+    def set_source_framing(self, source: int, mode=None, rect=None):
+        """framing of one source: None = follow set_framing, including later changes; otherwise as set_framing"""
+        args = (-1, 0, 0, 0, 0) if mode is None else self._framing_args("bsb_set_source_framing", mode, rect)
+        if not self._lib.bsb_set_source_framing(self._h, int(source), *args):
+            self._fail("bsb_set_source_framing")
+
+    def framing(self, frame: int = 0):
+        """the crop (x, y, w, h) frame `frame` of the last call showed; the whole frame when that call was not framed"""
+        r = (C.c_int * 4)()
+        if not self._lib.bsb_get_framing(self._h, int(frame), r):
+            self._fail("bsb_get_framing")
+        return tuple(r)
+
     def set_out_format(self, fmt: str):
         """format of the `out` frames of every composite call: "bgr" (the composite, the default) or "bgra" (the camera with
         alpha 255 - mask, straight alpha, flipped and resized like the composite; the video output and the mask are

@@ -405,6 +405,35 @@ int bsb_set_source_mask_interval(bsb_ctx* ctx, int source, int interval) {
   return 1;
 }
 
+int bsb_set_framing(bsb_ctx* ctx, int mode, int x, int y, int w, int h) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_framing(mode, x, y, w, h, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
+int bsb_set_framing_auto(bsb_ctx* ctx, int max_zoom_pct, int margin_pct, int speed) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_framing_auto(max_zoom_pct, margin_pct, speed, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
+int bsb_set_source_framing(bsb_ctx* ctx, int source, int mode, int x, int y, int w, int h) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_source_framing(source, mode, x, y, w, h, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
+int bsb_get_framing(bsb_ctx* ctx, int frame, int rect[4]) {
+  if (!check_ctx(ctx)) return 0;
+  if (!rect) { report(&ctx->cb, "error: rect is null"); return 0; }
+  std::string err;
+  if (!ctx->eng->get_framing(frame, rect, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
 int bsb_set_out_format(bsb_ctx* ctx, int format) {
   if (!check_ctx(ctx)) return 0;
   if (format != BSB_OUT_BGR && format != BSB_OUT_BGRA) { report(&ctx->cb, "error: output format must be BSB_OUT_BGR (0) or BSB_OUT_BGRA (1)"); return 0; }

@@ -1,5 +1,6 @@
 // backscrub_b200/csrc/engine.cu — planner + per-stream engine (see engine.h).
 #include "engine.h"
+#include "resize_taps.h"
 
 #include <algorithm>
 #include <cmath>
@@ -24,27 +25,18 @@ HostResizeTab build_resize_tab(int sw, int sh, int dw, int dh) {
   HostResizeTab t;
   t.sw = sw;
   t.area2x2 = (sw == dw * 2 && sh == dh * 2);
-  const double scale_x = 1.0 / ((double)dw / sw), scale_y = 1.0 / ((double)dh / sh);
+  const double scale_x = resize_scale(sw, dw), scale_y = resize_scale(sh, dh);
   t.xofs.resize(dw); t.xw.resize(2 * (size_t)dw);
   for (int dx = 0; dx < dw; ++dx) {
-    float fx = (float)((dx + 0.5) * scale_x - 0.5);
-    int sx = (int)std::floor(fx);
-    fx -= (float)sx;
-    if (sx < 0) { fx = 0; sx = 0; }
-    if (sx >= sw - 1) { fx = 0; sx = sw - 1; }
-    t.xofs[dx] = sx;
-    t.xw[2 * dx] = (short)std::lrintf((1.f - fx) * 2048.f);
-    t.xw[2 * dx + 1] = (short)std::lrintf(fx * 2048.f);
+    int w0, w1;
+    resize_tap_x(dx, scale_x, sw, &t.xofs[dx], &w0, &w1);
+    t.xw[2 * dx] = (short)w0; t.xw[2 * dx + 1] = (short)w1;
   }
   t.yofs0.resize(dh); t.yofs1.resize(dh); t.yw.resize(2 * (size_t)dh);
   for (int dy = 0; dy < dh; ++dy) {
-    float fy = (float)((dy + 0.5) * scale_y - 0.5);
-    int sy = (int)std::floor(fy);
-    fy -= (float)sy;
-    t.yofs0[dy] = std::min(std::max(sy, 0), sh - 1);
-    t.yofs1[dy] = std::min(std::max(sy + 1, 0), sh - 1);
-    t.yw[2 * dy] = (short)std::lrintf((1.f - fy) * 2048.f);
-    t.yw[2 * dy + 1] = (short)std::lrintf(fy * 2048.f);
+    int w0, w1;
+    resize_tap_y(dy, scale_y, sh, &t.yofs0[dy], &t.yofs1[dy], &w0, &w1);
+    t.yw[2 * dy] = (short)w0; t.yw[2 * dy + 1] = (short)w1;
   }
   return t;
 }
@@ -944,7 +936,8 @@ Engine::~Engine() {
     if (p) cudaFree(p);
   for (ChainPlan& cp : chains_) if (cp.d_ops) cudaFree(cp.d_ops);
   free_sources();
-  for (void* p : {(void*)d_src_tab_, (void*)d_src_raw_, tab_src_.blob, (void*)d_pass_all_, (void*)d_live_tab_, (void*)d_live_stage_, (void*)d_seg_tab_})
+  for (void* p : {(void*)d_src_tab_, (void*)d_src_raw_, tab_src_.blob, (void*)d_pass_all_, (void*)d_live_tab_, (void*)d_live_stage_, (void*)d_seg_tab_,
+                  (void*)d_frame_tab_, (void*)d_crop_, (void*)d_frame_box_, (void*)d_frame_counter_, (void*)d_frame_state_})
     if (p) cudaFree(p);
   for (LiveSize& l : live_sizes_) if (l.tab.blob) cudaFree(l.tab.blob);
   if (h_mask_) cudaFreeHost(h_mask_);
@@ -1225,6 +1218,97 @@ bool Engine::set_source_mask_interval(int source, int k, std::string* err) {
   return true;
 }
 
+bool Engine::framing_rows(const Call& c, std::vector<int>* rows) const {
+  bool any = false;
+  for (int b = 0; b < c.n && !any; ++b) any = frame_framing(c.ids ? c.ids[b] : -1).mode != FRAMING_OFF;
+  if (!any) return false;
+  const size_t mb = (size_t)max_batch_;
+  rows->assign(FRAMING_ROWS * mb, 0);
+  int* r = rows->data();
+  const int full[4] = {0, 0, W_, H_};
+  for (int b = 0; b < c.n; ++b) {
+    const int id = c.ids ? c.ids[b] : -1;
+    const Framing& f = frame_framing(id);
+    int ow = out_w_, oh = out_h_;
+    if (c.ids) source_output_size(id, &ow, &oh);
+    r[b] = f.mode;
+    r[mb + b] = c.ids ? src_jump_[id] : (b == 0 && plain_jump_);    // a plain call's later frames follow its first
+    r[2 * mb + b] = c.ids ? id : 0;
+    r[3 * mb + b] = ow; r[4 * mb + b] = oh;
+    for (int k = 0; k < 4; ++k) r[(5 + k) * mb + b] = f.mode == FRAMING_RECT ? f.rect[k] : full[k];
+    r[9 * mb + b] = c.ids ? b : c.frame0 + b;                        // a split host-buffer call's crops by caller frame
+  }
+  return true;
+}
+
+void Engine::count_framing(const Call& c, const Plan& p) {
+  last_framed_ = p.framed;
+  last_frames_ = c.ids ? c.n : c.frame0 + c.n;
+  if (!c.ids) { plain_jump_ = framing_.mode != FRAMING_AUTO; return; }
+  for (int b = 0; b < c.n; ++b) src_jump_[c.ids[b]] = frame_framing(c.ids[b]).mode != FRAMING_AUTO;
+}
+
+void Engine::enqueue_framing(const Call& c) {
+  FramingArgs a{};
+  a.n = c.n; a.ofinal = ofinal_; a.oh = oh_; a.opitch = opitch_; a.ox = out_roidim_[0]; a.oy = out_roidim_[1];
+  a.g = FramingGeo{W_, H_, roidim_[0], roidim_[1], roidim_[2], roidim_[3], out_roidim_[2], out_roidim_[3]};
+  a.p = framing_auto_;
+  a.tab = d_frame_tab_; a.mb = max_batch_;
+  a.state = c.ids ? d_src_frame_state_ : d_frame_state_;
+  a.crop = d_crop_; a.targets = d_frame_box_; a.counter = d_frame_counter_; a.plain = c.ids ? 0 : 1;
+  launch_framing(stream_, a);
+}
+
+namespace {
+bool check_framing(int mode, int x, int y, int w, int h, int W, int H, bool follow, std::string* err) {
+  if (mode < (follow ? -1 : FRAMING_OFF) || mode > FRAMING_AUTO) {
+    *err = follow ? "source framing mode must be -1 (follow the context), BSB_FRAMING_OFF, BSB_FRAMING_RECT or BSB_FRAMING_AUTO"
+                  : "framing mode must be BSB_FRAMING_OFF, BSB_FRAMING_RECT or BSB_FRAMING_AUTO";
+    return false;
+  }
+  if (mode == FRAMING_RECT && (x < 0 || y < 0 || w < 1 || h < 1 || (long)x + w > W || (long)y + h > H)) {
+    *err = "framing rectangle must lie inside the frame, with w and h >= 1";
+    return false;
+  }
+  return true;
+}
+}  // namespace
+
+bool Engine::set_framing(int mode, int x, int y, int w, int h, std::string* err) {
+  if (!check_framing(mode, x, y, w, h, W_, H_, false, err)) return false;
+  framing_ = Framing{mode, {x, y, w, h}};
+  return true;
+}
+
+bool Engine::set_framing_auto(int max_zoom, int margin, int speed, std::string* err) {
+  if (max_zoom < 100 || max_zoom > 1000) { *err = "framing max_zoom_pct out of range (100..1000)"; return false; }
+  if (margin < 0 || margin > 100) { *err = "framing margin_pct out of range (0..100)"; return false; }
+  if (speed < 1 || speed > 256) { *err = "framing speed out of range (1..256)"; return false; }
+  // the parameters are kernel arguments of the captured calls
+  CUDA_OK(cudaSetDevice(device_));
+  CUDA_OK(cudaStreamSynchronize(stream_));
+  drop_graphs();
+  framing_auto_ = FramingParams{max_zoom, margin, speed};
+  return true;
+}
+
+bool Engine::set_source_framing(int source, int mode, int x, int y, int w, int h, std::string* err) {
+  if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
+  if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
+  if (!check_framing(mode, x, y, w, h, W_, H_, true, err)) return false;
+  src_framing_[source] = Framing{mode, {x, y, w, h}};
+  return true;
+}
+
+bool Engine::get_framing(int frame, int* rect, std::string* err) {
+  if (frame < 0 || frame >= last_frames_) { *err = "frame out of range (0 .. the last call's n_frames - 1)"; return false; }
+  if (!last_framed_) { rect[0] = 0; rect[1] = 0; rect[2] = W_; rect[3] = H_; return true; }
+  CUDA_OK(cudaSetDevice(device_));
+  CUDA_OK(cudaStreamSynchronize(stream_));
+  CUDA_OK(cudaMemcpy(rect, d_crop_ + frame, 4 * sizeof(int), cudaMemcpyDeviceToHost));
+  return true;
+}
+
 // PostArgs of one call.  p.native: the post kernel reads the camera frames in place — YUYV, or NV12, which then also
 // writes its video output as NV12; p.nv12_staged: the video output goes to d_yuyv_ as YUYV.
 PostArgs Engine::post_args(const Call& c, const Plan& p) const {
@@ -1332,6 +1416,7 @@ bool Engine::enqueue_post(const Call& c, const Plan& p) {
     t.slot = d_src_tab_ + 4 * (size_t)max_batch_; t.geos = d_geo_; t.flips = d_src_tab_ + 3 * (size_t)max_batch_;
     max_px = sources_out_px_max();
   }
+  if (p.framed) { t.crop = d_crop_; t.crop_idx = d_frame_tab_ + 9 * (size_t)max_batch_; }
   launch_tail(stream_, t, max_px);
   return true;
 }
@@ -1364,7 +1449,7 @@ bool Engine::plan_launch(const Call& c, Plan* p, std::string* err) {
   // where k_post_tma takes the call, it writes them mirrored in place; otherwise the tail flips them.
   p->flip_tail = false;
   if (p->mode != CALL_PLAIN && p->flipped) {
-    bool in_place = !p->resized && tuning().post_tma;
+    bool in_place = !p->resized && !p->framed && tuning().post_tma;
     if (in_place) {
       decide();
       in_place = post_tma_eligible(post_args(c, *p));
@@ -1399,6 +1484,7 @@ bool Engine::enqueue_all(const Call& c, const Plan& p) {
     enqueue_decision(n, p.mode != CALL_PLAIN, p.m, seg);
     if (c.callbacks && cb_.onmask) { cudaStreamSynchronize(stream_); cb_.onmask(cb_.caller_ctx); }
   }
+  if (p.framed) enqueue_framing(c);
   if (!enqueue_post(c, p)) return false;
   if (p.nv12_staged) launch_yuyv_to_nv12(stream_, n, d_yuyv_, (size_t)W_ * H_ * 2, c.video, c.video_stride, W_, H_);
   last_call_launches_ = (int)(thread_launch_count() - l0);
@@ -1526,10 +1612,25 @@ bool Engine::run(const Call& c, std::string* err) {
     p.all_blur = n_blur == n;
   }
   if (c.fmt != IN_BGR && (W_ & 1)) { *err = "YUYV ingest needs an even width"; return false; }
+  std::vector<int> ftab;
+  p.framed = framing_rows(c, &ftab);
   std::vector<int> seg;
   p.m = segment(c, &seg);
   if (c.ids && p.m < n) std::copy(seg.begin(), seg.begin() + 2 * (size_t)max_batch_, tab.begin() + SRC_TAB_SEG * (size_t)max_batch_);
   CUDA_OK(cudaSetDevice(device_));
+  if (p.framed) {
+    const size_t mb = (size_t)max_batch_;
+    if (!d_frame_tab_) {
+      CUDA_OK(cudaMalloc((void**)&d_frame_tab_, FRAMING_ROWS * mb * sizeof(int)));
+      CUDA_OK(cudaMalloc((void**)&d_crop_, mb * sizeof(FrameCrop)));
+      CUDA_OK(cudaMalloc((void**)&d_frame_box_, 4 * mb * sizeof(int)));
+      CUDA_OK(cudaMalloc((void**)&d_frame_counter_, sizeof(unsigned)));
+      CUDA_OK(cudaMemsetAsync(d_frame_counter_, 0, sizeof(unsigned), stream_));
+      CUDA_OK(cudaMalloc((void**)&d_frame_state_, 4 * sizeof(int)));
+    }
+    // outside the graph, before its launch, like the source table
+    CUDA_OK(cudaMemcpyAsync(d_frame_tab_, ftab.data(), ftab.size() * sizeof(int), cudaMemcpyHostToDevice, stream_));
+  }
   if (!c.ids && p.m < n) {
     // outside the graph, before its launch, like the source table
     if (!d_seg_tab_) CUDA_OK(cudaMalloc((void**)&d_seg_tab_, seg.size() * sizeof(int)));
@@ -1560,6 +1661,7 @@ bool Engine::run(const Call& c, std::string* err) {
     CUDA_OK(cudaGetLastError());
     move_cursors(c);
     count_frames(c);
+    count_framing(c, p);
     return true;
   }
 #ifndef BSB_EMU
@@ -1598,6 +1700,7 @@ bool Engine::run(const Call& c, std::string* err) {
   CUDA_OK(cudaGraphLaunch(it->second.exec, stream_));
   move_cursors(c);
   count_frames(c);
+  count_framing(c, p);
 #endif
   return true;
 }
@@ -1871,6 +1974,7 @@ bool Engine::reset_state(std::string* err) {
   CUDA_OK(cudaMemsetAsync(state_, 0, (size_t)oh_ * ow_, stream_));
   CUDA_OK(cudaStreamSynchronize(stream_));
   plain_frames_ = 0;
+  plain_jump_ = true;
   return true;
 }
 
@@ -1890,6 +1994,10 @@ void Engine::free_sources() {
   src_size_.clear();
   src_interval_.clear();
   src_frames_.clear();
+  src_framing_.clear();
+  src_jump_.clear();
+  if (d_src_frame_state_) cudaFree(d_src_frame_state_);
+  d_src_frame_state_ = nullptr;
   for (const Live& l : src_live_) live_size_release(l.size);
   src_live_.clear();
   for (OwnSize& o : own_sizes_) if (o.tab.blob) cudaFree(o.tab.blob);
@@ -1938,6 +2046,9 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   src_live_.assign((size_t)n_sources, Live{});
   src_interval_.assign((size_t)n_sources, -1);
   src_frames_.assign((size_t)n_sources, 0);
+  src_framing_.assign((size_t)n_sources, Framing{});
+  src_jump_.assign((size_t)n_sources, 1);
+  CUDA_OK(cudaMalloc((void**)&d_src_frame_state_, (size_t)n_sources * 4 * sizeof(int)));
   CUDA_OK(cudaMalloc((void**)&d_geo_, (1 + (size_t)n_sources) * sizeof(TailGeo)));
   if (!upload_geo(0, ctx_geo(), err)) return false;
   if (!refresh_bank_ctx(err)) return false;
@@ -1953,6 +2064,7 @@ bool Engine::reset_source(int source, std::string* err) {
   CUDA_OK(cudaMemsetAsync(src_state_ + (size_t)source * opx, 0, opx, stream_));
   CUDA_OK(cudaStreamSynchronize(stream_));
   src_frames_[source] = 0;
+  src_jump_[source] = 1;
   return true;
 }
 

@@ -139,6 +139,15 @@ class Engine {
   bool set_source_mask_interval(int source, int k, std::string* err);
   bool sync(std::string* err);
   bool reset_state(std::string* err);
+  // Framing (include/backscrub_b200.h, bsb_set_framing): the output shows a crop of the camera frame, a fixed rectangle
+  // (RECT) or one that follows the person the mask finds (AUTO, framing.h).  Host state only: the modes and rectangles
+  // reach the device as table data with the call.
+  bool set_framing(int mode, int x, int y, int w, int h, std::string* err);
+  bool set_framing_auto(int max_zoom, int margin, int speed, std::string* err);
+  // one source's framing: mode -1 follows set_framing (rectangle included), else its own
+  bool set_source_framing(int source, int mode, int x, int y, int w, int h, std::string* err);
+  // the crop (x, y, w, h) frame `frame` of the last call showed (synchronises)
+  bool get_framing(int frame, int* rect, std::string* err);
 
   // Independent sources (camera streams) batched one frame each into a call.  set_sources allocates n zeroed smoother
   // states and the per-source background bank (again: everything reallocated and zeroed, graphs dropped).
@@ -260,6 +269,8 @@ class Engine {
                                      // at frame_stride 0), 2 one per frame (the live table's descriptors say which)
     unsigned live_gclass = 0;        // the Gaussian launch classes of the blurred live frames
     int m = 0;                       // frames segmented (the CNN batch); m == n: every frame, the parent path with no table
+    bool framed = false;             // some frame is framed (RECT or AUTO): k_framing runs and every frame goes through the
+                                     // cropping tail from unflipped staging
   };
   // the call blends a composite: it has a video output, or a BGR composite output.  A call that does not reads no
   // background and blurs nothing.
@@ -275,7 +286,7 @@ class Engine {
   // the call ends with k_tail (post -> stage -> flip, resize, YUYV / NV12): plain calls with a context flip or resize;
   // sources calls with a frame not at W x H, or with mirrored frames the post kernel cannot mirror in place
   bool call_tail(const Plan& p) const {
-    return p.mode == CALL_PLAIN ? (flip_h_ || flip_v_ || out_w_ != W_ || out_h_ != H_) : (p.resized || p.flip_tail);
+    return p.framed || (p.mode == CALL_PLAIN ? (flip_h_ || flip_v_ || out_w_ != W_ || out_h_ != H_) : (p.resized || p.flip_tail));
   }
   // false (nothing more enqueued) only when the post kernel cannot write a call's mirrored frames
   bool enqueue_all(const Call& c, const Plan& p);
@@ -295,6 +306,11 @@ class Engine {
   SegRows seg_rows(const Call& c, const Plan& p) const;
   // after a call is enqueued: the frame counters of the cadence move on (not for a fed call)
   void count_frames(const Call& c);
+  // the framing rows of call c (FRAMING_ROWS x max_batch_, kernels.h) into *rows; true when some frame is framed
+  bool framing_rows(const Call& c, std::vector<int>* rows) const;
+  // after a call is enqueued (fed calls included): which cameras now hold a framing state
+  void count_framing(const Call& c, const Plan& p);
+  void enqueue_framing(const Call& c);
   bool enqueue_post(const Call& c, const Plan& p);
   void enqueue_live(const Call& c, const Plan& p);
   // base of tensor t for the frames [frame_off_, ...) of the batch (frame_off_ != 0 only inside a sub-batched segment)
@@ -423,6 +439,23 @@ class Engine {
   std::vector<long long> src_frames_;   // per source: frames delivered since set_sources / reset_source
   int src_interval(int s) const { return src_interval_[s] < 0 ? mask_interval_ : src_interval_[s]; }
   int* d_seg_tab_ = nullptr;         // [3][max_batch] the segment rows of a plain call with held frames, written before its launch
+  // ---- framing ----
+  struct Framing { int mode = -1; int rect[4] = {0, 0, 0, 0}; };
+  Framing framing_{0, {0, 0, 0, 0}};   // the context's (plain calls, and sources that follow it)
+  FramingParams framing_auto_{300, 10, 32};
+  std::vector<Framing> src_framing_;   // per source: mode -1 follows framing_
+  const Framing& frame_framing(int id) const { return id < 0 || src_framing_[id].mode < 0 ? framing_ : src_framing_[id]; }
+  // the camera has no framing state yet (new, reset, or its last frame was not AUTO): its next AUTO frame jumps
+  bool plain_jump_ = true;
+  std::vector<char> src_jump_;
+  int* d_frame_tab_ = nullptr;       // [FRAMING_ROWS][max_batch] the framing rows of a framed call, written before its launch
+  FrameCrop* d_crop_ = nullptr;      // [max_batch] the crop of each frame of the last framed call (the tail reads it)
+  int* d_frame_box_ = nullptr;       // [max_batch][4] targets of a plain call (k_framing scratch)
+  unsigned* d_frame_counter_ = nullptr;
+  int* d_frame_state_ = nullptr;     // [4] the plain stream's state, 1/16 pixel
+  int* d_src_frame_state_ = nullptr; // [n_sources][4] the sources' states
+  bool last_framed_ = false;         // the last call was framed; last_frames_: its frame count (chunks included)
+  int last_frames_ = 0;
   // ---- live backgrounds ----
   struct Live { const uint8_t* p = nullptr; int fmt = 0, w = 0, h = 0; size_t pitch = 0, uv = 0, stride = 0; int size = -1; };
   Live live_;                        // plain calls
@@ -493,21 +526,23 @@ class Engine {
   // are filtered off is table data), resized and the largest output size of the sources, which the tail's grid covers
   // (which frame has which size is table data too), the output format, whether frames blend live backgrounds, with
   // the Gaussian classes they add (their images, sizes and strengths within the classes are the live table's data), and the
-  // CNN batch of a call with held frames (which frames are segmented is the segment rows' data).  The rest of the plan is
+  // CNN batch of a call with held frames (which frames are segmented is the segment rows' data), and whether the call is
+  // framed (modes, rectangles and crops are table data).  The rest of the plan is
   // decided from these.
   struct GraphKey {
     int n, fmt; const void* in; size_t pitch, uv, stride;
     const void* out; const void* video; const void* mask; size_t ostride, vstride, mstride;
     int mode; unsigned gclass; bool all_blur, flipped, resized, passed; long out_px_max; bool bgra; int live; unsigned live_gclass;
+    bool framed;
     GraphKey(const Call& c, const Plan& p, long px_max)
         : n(c.n), fmt(c.fmt), in(c.in), pitch(c.pitch), uv(c.uv), stride(c.stride), out(c.out), video(c.video), mask(c.mask),
           ostride(c.out ? c.out_stride : 0), vstride(c.video ? c.video_stride : 0), mstride(c.mask ? c.mask_stride : 0),
           mode(p.mode), gclass(p.gclass), all_blur(p.all_blur), flipped(p.flipped), resized(p.resized), passed(p.passed),
-          out_px_max(px_max), bgra(p.bgra), live(p.live), live_gclass(p.live_gclass), seg(p.m) {}
+          out_px_max(px_max), bgra(p.bgra), live(p.live), live_gclass(p.live_gclass), framed(p.framed), seg(p.m) {}
     int seg;                         // the CNN batch m (n: every frame segmented, the parent's launches)
     auto tie() const {
       return std::tie(n, fmt, in, pitch, uv, stride, out, video, mask, ostride, vstride, mstride, mode, gclass, all_blur, flipped, resized,
-                      passed, out_px_max, bgra, live, live_gclass, seg);
+                      passed, out_px_max, bgra, live, live_gclass, framed, seg);
     }
     bool operator<(const GraphKey& r) const { return tie() < r.tie(); }
   };

@@ -4,6 +4,7 @@
 // frames is B consecutive images.
 #pragma once
 #include "bsb_common.h"
+#include "framing.h"
 
 namespace bsb {
 
@@ -326,7 +327,9 @@ void launch_flip_u8c3(cudaStream_t s, int n, const uint8_t* src, size_t sstride,
 // cv::flip, then cv::resize to the frame's virtual-camera geometry, then the YUYV (or NV12) conversion, from the staged
 // W x H BGR composites (and the BGRA output from the staged BGRA frames, 8UC4).  The flip mirrors each tap's source coordinate and keeps the weights; ow == W and oh == H is a
 // mirrored copy.  Bit-exact against the chain k_flip_u8c3 -> k_resize_u8c3 -> k_rgb_to_yuyv (-> k_yuyv_to_nv12).
-struct TailGeo { int ow, oh; ResizeTab tab; int area2x2; };   // tab: INTER_LINEAR tables W x H -> ow x oh
+struct TailGeo { int ow, oh; ResizeTab tab; int area2x2; };
+// a framed frame's crop (x, y, w, h) and the resize steps (resize_scale) from it to the frame's output size
+struct FrameCrop { int x, y, w, h; double sx, sy; };   // tab: INTER_LINEAR tables W x H -> ow x oh
 struct TailArgs {
   int n, W, H;
   const uint8_t* src; size_t src_stride;   // staged composites, rows W*3 bytes
@@ -339,9 +342,32 @@ struct TailArgs {
   // bgra != 0: `out` is BGRA (tightly packed rows ow*4 bytes), flipped and resized channel by channel from the staged
   // W x H BGRA frames `src4` (rows W*4 bytes); `src` is then read only for the video output
   const uint8_t* src4; size_t src4_stride; int bgra;
+  // framed calls (bsb_set_framing; a separate k_tail instantiation): non-null (DEVICE) frame b shows crop
+  // crop[crop_idx[b]] of its staged frame, flipped within the crop and resized to its geometry's ow x oh with taps
+  // computed on the fly (resize_taps.h; a crop of the output size is a copy, an exact 2x crop the INTER_AREA mean).  The
+  // geometry's tables are not read.
+  const FrameCrop* crop; const int* crop_idx;
 };
 // max_px: the largest ow * oh a frame of the call can have (the grid covers it; smaller frames' extra CTAs exit)
 void launch_tail(cudaStream_t s, const TailArgs& a, long max_px);
+
+// Framing (framing.h): one CTA per frame reduces the frame's small mask (ofinal, inside out_roidim) to the person count
+// and bounding box; AUTO frames then step their camera's state and write their crop, RECT / OFF frames copy the table's
+// rectangle.  tab: DEVICE [FRAMING_ROWS][mb] rows mode | jump (the camera has no state yet) | state slot | ow | oh | x | y
+// | w | h | crop index.  Sources calls: every frame steps state[slot] in parallel (distinct ids).  Plain calls (`plain`):
+// every frame steps state[0] in frame order, in the CTA that arrives last (targets: [n][4] scratch, counter:
+// 0 between launches).
+enum { FRAMING_ROWS = 10 };
+struct FramingArgs {
+  int n;
+  const uint8_t* ofinal; int oh, opitch, ox, oy;   // [n][oh][opitch], out_roidim's origin
+  FramingGeo g; FramingParams p;
+  const int* tab; int mb;
+  int* state;                                       // [slots][4] 1/16-pixel states
+  FrameCrop* crop;                                  // written at the crop index
+  int* targets; unsigned* counter; int plain;
+};
+void launch_framing(cudaStream_t s, const FramingArgs& a);
 
 // cv::cvtColor(COLOR_YUV2BGR_YUYV): camera YUYV frames -> BGR (what cv::VideoCapture does for the
 // reference, app/deepseg.cc:553).  n frames of W x H, tightly packed.

@@ -8,6 +8,7 @@
 // cv2 pins); results are bit-exact against the oracle.
 #include "kernels.h"
 #include "post_math.h"
+#include "resize_taps.h"
 
 namespace bsb {
 
@@ -1159,11 +1160,62 @@ BSB_D void tail_px(const uint8_t* src, int W, int H, const TailGeo& g, int flip,
   }
 }
 
-// BGRA: TailArgs::bgra, the output is the transparent BGRA (from src4; the BGR composite is read for the video only)
-template <bool BGRA>
+// pixel (x, y) of a framed frame: crop cr = (x, y, w, h) of the staged W-wide frame, mirrored within the crop, then
+// resized to ow x oh as resize_px does (a crop of the output size is a copy, an exact 2x crop the INTER_AREA mean); the
+// taps come from resize_taps.h, on the fly (sx_scale / sy_scale: resize_scale of the crop to the output)
+template <int CN = 3>
+BSB_D void crop_px(const uint8_t* src, int W, const int4& cr, int ow, int oh, double sx_scale, double sy_scale, int flip, int x, int y,
+                   uint8_t* d) {
+  const size_t sp = (size_t)W * CN;
+  src += (size_t)cr.y * sp + (size_t)cr.x * CN;
+  if (cr.z == ow && cr.w == oh) {
+    const uint8_t* s = src + (size_t)((flip & 2) ? cr.w - 1 - y : y) * sp + (size_t)((flip & 1) ? cr.z - 1 - x : x) * CN;
+#pragma unroll
+    for (int c = 0; c < CN; ++c) d[c] = s[c];
+    return;
+  }
+  if (cr.z == 2 * ow && cr.w == 2 * oh) {
+    int x0 = 2 * x, x1 = 2 * x + 1, y0 = 2 * y, y1 = 2 * y + 1;
+    if (flip & 1) { x0 = cr.z - 1 - x0; x1 = cr.z - 1 - x1; }
+    if (flip & 2) { y0 = cr.w - 1 - y0; y1 = cr.w - 1 - y1; }
+    const uint8_t* s0 = src + (size_t)y0 * sp;
+    const uint8_t* s1 = src + (size_t)y1 * sp;
+#pragma unroll
+    for (int c = 0; c < CN; ++c) d[c] = (uint8_t)((s0[CN * x0 + c] + s0[CN * x1 + c] + s1[CN * x0 + c] + s1[CN * x1 + c] + 2) >> 2);
+    return;
+  }
+  int sx, a0, a1, y0, y1, b0, b1;
+  resize_tap_x(x, sx_scale, cr.z, &sx, &a0, &a1);
+  resize_tap_y(y, sy_scale, cr.w, &y0, &y1, &b0, &b1);
+  int sx1 = min(sx + 1, cr.z - 1);
+  if (flip & 1) { sx = cr.z - 1 - sx; sx1 = cr.z - 1 - sx1; }
+  if (flip & 2) { y0 = cr.w - 1 - y0; y1 = cr.w - 1 - y1; }
+  const uint8_t* r0 = src + (size_t)y0 * sp;
+  const uint8_t* r1 = src + (size_t)y1 * sp;
+#pragma unroll
+  for (int c = 0; c < CN; ++c) d[c] = lin_v(lin_h(r0, sx, sx1, CN, c, a0, a1), lin_h(r1, sx, sx1, CN, c, a0, a1), b0, b1);
+}
+
+// the frame's crop and its resize steps (framed calls)
+struct TailCrop { int4 cr; double sx, sy; };
+
+template <int CN = 3, bool CROP = false>
+BSB_D void tail_pick(const uint8_t* src, int W, int H, const TailGeo& g, const TailCrop& k, int flip, int x, int y, uint8_t* d) {
+  if (CROP) crop_px<CN>(src, W, k.cr, g.ow, g.oh, k.sx, k.sy, flip, x, y, d);
+  else tail_px<CN>(src, W, H, g, flip, x, y, d);
+}
+
+// BGRA: TailArgs::bgra, the output is the transparent BGRA (from src4; the BGR composite is read for the video only).
+// CROP: TailArgs::crop, a framed call (a separate instantiation: the unframed tails compile as before)
+template <bool BGRA, bool CROP = false>
 __global__ void __launch_bounds__(256) k_tail(TailArgs a) {
   const int b = blockIdx.y;
   const TailGeo g = a.slot ? a.geos[__ldg(a.slot + b)] : a.geo;
+  TailCrop k{};
+  if (CROP) {
+    const FrameCrop& c = a.crop[__ldg(a.crop_idx + b)];
+    k.cr = make_int4(c.x, c.y, c.w, c.h); k.sx = c.sx; k.sy = c.sy;
+  }
   const int fl = a.flips ? __ldg(a.flips + b) : a.flip;
   const long i = (long)blockIdx.x * blockDim.x + threadIdx.x;
   const long npx = (long)g.ow * g.oh;
@@ -1176,17 +1228,17 @@ __global__ void __launch_bounds__(256) k_tail(TailArgs a) {
     const int hw = g.ow / 2, x = (int)(i % hw) * 2, y = (int)(i / hw) * 2;
     uint8_t px[12];                                   // (x, y) (x+1, y) | (x, y+1) (x+1, y+1)
     if (!BGRA || vid) {
-      tail_px(src, a.W, a.H, g, fl, x, y, px);
-      tail_px(src, a.W, a.H, g, fl, x + 1, y, px + 3);
-      tail_px(src, a.W, a.H, g, fl, x, y + 1, px + 6);
-      tail_px(src, a.W, a.H, g, fl, x + 1, y + 1, px + 9);
+      tail_pick<3, CROP>(src, a.W, a.H, g, k, fl, x, y, px);
+      tail_pick<3, CROP>(src, a.W, a.H, g, k, fl, x + 1, y, px + 3);
+      tail_pick<3, CROP>(src, a.W, a.H, g, k, fl, x, y + 1, px + 6);
+      tail_pick<3, CROP>(src, a.W, a.H, g, k, fl, x + 1, y + 1, px + 9);
     }
     if (BGRA && out) {
       uint8_t* o = out + ((size_t)y * g.ow + x) * 4;
-      tail_px<4>(src4, a.W, a.H, g, fl, x, y, o);
-      tail_px<4>(src4, a.W, a.H, g, fl, x + 1, y, o + 4);
-      tail_px<4>(src4, a.W, a.H, g, fl, x, y + 1, o + (size_t)g.ow * 4);
-      tail_px<4>(src4, a.W, a.H, g, fl, x + 1, y + 1, o + (size_t)g.ow * 4 + 4);
+      tail_pick<4, CROP>(src4, a.W, a.H, g, k, fl, x, y, o);
+      tail_pick<4, CROP>(src4, a.W, a.H, g, k, fl, x + 1, y, o + 4);
+      tail_pick<4, CROP>(src4, a.W, a.H, g, k, fl, x, y + 1, o + (size_t)g.ow * 4);
+      tail_pick<4, CROP>(src4, a.W, a.H, g, k, fl, x + 1, y + 1, o + (size_t)g.ow * 4 + 4);
     } else if (out) {
       uint8_t* o = out + ((size_t)y * g.ow + x) * 3;
 #pragma unroll
@@ -1200,12 +1252,12 @@ __global__ void __launch_bounds__(256) k_tail(TailArgs a) {
   const bool pair = p + 1 < npx;
   uint8_t px[6];
   if (!BGRA || vid) {
-    tail_px(src, a.W, a.H, g, fl, (int)(p % g.ow), (int)(p / g.ow), px);
-    if (pair) tail_px(src, a.W, a.H, g, fl, (int)((p + 1) % g.ow), (int)((p + 1) / g.ow), px + 3);
+    tail_pick<3, CROP>(src, a.W, a.H, g, k, fl, (int)(p % g.ow), (int)(p / g.ow), px);
+    if (pair) tail_pick<3, CROP>(src, a.W, a.H, g, k, fl, (int)((p + 1) % g.ow), (int)((p + 1) / g.ow), px + 3);
   }
   if (BGRA && out) {
-    tail_px<4>(src4, a.W, a.H, g, fl, (int)(p % g.ow), (int)(p / g.ow), out + 4 * p);
-    if (pair) tail_px<4>(src4, a.W, a.H, g, fl, (int)((p + 1) % g.ow), (int)((p + 1) / g.ow), out + 4 * p + 4);
+    tail_pick<4, CROP>(src4, a.W, a.H, g, k, fl, (int)(p % g.ow), (int)(p / g.ow), out + 4 * p);
+    if (pair) tail_pick<4, CROP>(src4, a.W, a.H, g, k, fl, (int)((p + 1) % g.ow), (int)((p + 1) / g.ow), out + 4 * p + 4);
   } else if (out) {
     uint8_t* o = out + 3 * p;
     o[0] = px[0]; o[1] = px[1]; o[2] = px[2];
@@ -1224,8 +1276,104 @@ __global__ void __launch_bounds__(256) k_tail(TailArgs a) {
 
 void launch_tail(cudaStream_t s, const TailArgs& a, long max_px) {
   const long threads = (max_px + 1) / 2;
-  if (a.bgra) { auto k = k_tail<true>; BSB_LAUNCH(k, dim3((unsigned)((threads + 255) / 256), (unsigned)a.n), dim3(256), 0, s, a); }
-  else { auto k = k_tail<false>; BSB_LAUNCH(k, dim3((unsigned)((threads + 255) / 256), (unsigned)a.n), dim3(256), 0, s, a); }
+  const dim3 grid((unsigned)((threads + 255) / 256), (unsigned)a.n);
+  if (a.crop) {
+    if (a.bgra) { auto k = k_tail<true, true>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+    else { auto k = k_tail<false, true>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  } else if (a.bgra) { auto k = k_tail<true>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  else { auto k = k_tail<false>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  count_launch();
+}
+
+// ---------------------------------------------------------------------------
+// Framing (framing.h): one CTA = one frame's small mask; warps walk rows, lanes columns (coalesced), then a warp and a
+// block reduction of the person count and box.  Plain calls step the context's one state in frame order, so the CTA
+// that arrives last (as k_rowsum_fc's tail does) walks the frames' boxes; sources frames step distinct states at once.
+// ---------------------------------------------------------------------------
+// the crop record of one frame: the crop and the resize steps from it to the frame's output size
+BSB_D void framing_put(FrameCrop* o, const int* c, int ow, int oh) {
+  o->x = c[0]; o->y = c[1]; o->w = c[2]; o->h = c[3];
+  o->sx = resize_scale(c[2], ow); o->sy = resize_scale(c[3], oh);
+}
+
+__global__ void __launch_bounds__(256) k_framing(FramingArgs a) {
+  const int b = blockIdx.x, mb = a.mb;
+  const int mode = __ldg(a.tab + b), ci = __ldg(a.tab + 9 * mb + b);
+  const int ow = __ldg(a.tab + 3 * mb + b), oh = __ldg(a.tab + 4 * mb + b);
+  if (mode != FRAMING_AUTO) {
+    if (threadIdx.x == 0) {
+      int c[4];
+      for (int k = 0; k < 4; ++k) c[k] = __ldg(a.tab + (5 + k) * mb + b);
+      framing_put(a.crop + ci, c, ow, oh);
+    }
+    return;
+  }
+  const int sw = a.g.sw, sh = a.g.sh, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const uint8_t* m = a.ofinal + ((size_t)b * a.oh + a.oy) * a.opitch + a.ox;
+  int v[5] = {0, 1 << 30, 1 << 30, -1, -1};          // count, j0, i0, j1, i1
+  for (int i = warp; i < sh; i += 8)
+    for (int j = lane; j < sw; j += 32)
+      if (m[(size_t)i * a.opitch + j] < 128) {
+        ++v[0]; v[1] = min(v[1], j); v[2] = min(v[2], i); v[3] = max(v[3], j); v[4] = max(v[4], i);
+      }
+#pragma unroll
+  for (int o = 16; o; o >>= 1) {
+    v[0] += __shfl_xor_sync(0xffffffffu, v[0], o);
+    v[1] = min(v[1], __shfl_xor_sync(0xffffffffu, v[1], o)); v[2] = min(v[2], __shfl_xor_sync(0xffffffffu, v[2], o));
+    v[3] = max(v[3], __shfl_xor_sync(0xffffffffu, v[3], o)); v[4] = max(v[4], __shfl_xor_sync(0xffffffffu, v[4], o));
+  }
+  __shared__ int part[8][5];
+  __shared__ int last;
+  if (lane == 0)
+    for (int k = 0; k < 5; ++k) part[warp][k] = v[k];
+  __syncthreads();
+  int t[4];
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < 8; ++w) {
+      v[0] += part[w][0];
+      v[1] = min(v[1], part[w][1]); v[2] = min(v[2], part[w][2]); v[3] = max(v[3], part[w][3]); v[4] = max(v[4], part[w][4]);
+    }
+    framing_target(FramingBox{v[0], v[1], v[2], v[3], v[4]}, a.g, a.p, ow, oh, t);
+    if (!a.plain) {
+      int c[4];
+      int* st = a.state + 4 * __ldg(a.tab + 2 * mb + b);
+      framing_step(st, t, a.p.speed, __ldg(a.tab + mb + b) != 0);
+      framing_crop(st, a.g.W, a.g.H, c);
+      framing_put(a.crop + ci, c, ow, oh);
+    } else {
+      // the targets need no state, so every CTA makes its own; the CTA that arrives last steps them in frame order
+      for (int k = 0; k < 4; ++k) a.targets[4 * b + k] = t[k];
+      __threadfence();
+      last = atomicAdd(a.counter, 1u) == (unsigned)a.n - 1;
+    }
+  }
+  if (!a.plain) return;
+  __syncthreads();
+  if (!last) return;
+  __shared__ int tg[4 * 256];
+  __threadfence();
+  int st[4];
+  for (int k = 0; k < 4; ++k) st[k] = a.state[k];
+  for (int f0 = 0; f0 < a.n; f0 += 256) {               // the targets of 256 frames at a time, loaded in parallel
+    const int nf = min(256, a.n - f0);
+    __syncthreads();
+    for (int k = threadIdx.x; k < 4 * nf; k += blockDim.x) tg[k] = __ldcg(a.targets + 4 * f0 + k);
+    __syncthreads();
+    if (threadIdx.x == 0)
+      for (int f = f0; f < f0 + nf; ++f) {
+        int c[4];
+        framing_step(st, tg + 4 * (f - f0), a.p.speed, __ldg(a.tab + mb + f) != 0);
+        framing_crop(st, a.g.W, a.g.H, c);
+        framing_put(a.crop + __ldg(a.tab + 9 * mb + f), c, __ldg(a.tab + 3 * mb + f), __ldg(a.tab + 4 * mb + f));
+      }
+  }
+  if (threadIdx.x) return;
+  for (int k = 0; k < 4; ++k) a.state[k] = st[k];
+  *a.counter = 0;                                    // the next launch starts from 0 (stream order)
+}
+
+void launch_framing(cudaStream_t s, const FramingArgs& a) {
+  BSB_LAUNCH(k_framing, dim3((unsigned)a.n), dim3(256), 0, s, a);
   count_launch();
 }
 

@@ -173,6 +173,47 @@ BSB_API int bsb_set_mask_interval(bsb_ctx* ctx, int interval);
  * every source to -1; bsb_reset_source keeps it.  No bsb_set_sources yet, a source id out of range or an interval out of
  * range returns 0 with a bsb_last_error() message and changes nothing. */
 BSB_API int bsb_set_source_mask_interval(bsb_ctx* ctx, int source, int interval);
+/* Framing: each frame's output shows a crop of its camera frame, a fixed rectangle (a digital pan / zoom onto a
+ * whiteboard, one seat of a room camera) or one that keeps the person the mask finds centred and sized (auto-framing).
+ * C is the frame's W x H composite (BGR; the BGRA frame in the BGRA output format; the camera frame when its filter is off)
+ * and crop_b = (x, y, w, h) lies in the unflipped camera frame.  Frame b's output is
+ *   out_b = cv::resize(cv::flip(C[crop_b]), (ow_b, oh_b), INTER_LINEAR)
+ * with the frame's own flip and output size (bsb_set_output, or the source's); the YUYV / NV12 output is derived from
+ * out_b as always, and the mask stays W x H, unflipped and uncropped.  A crop of the output size is a copy and an exact 2x
+ * crop the INTER_AREA mean, as OpenCV does; the crop (0, 0, W, H) gives the bytes of an unframed call.
+ *   BSB_FRAMING_OFF: the whole frame (the default).
+ *   BSB_FRAMING_RECT: crop_b = (x, y, w, h), inside the frame with w, h >= 1 (else refused); the aspect is not forced.
+ *     Host bookkeeping only: a new rectangle every call replays the captured call.
+ *   BSB_FRAMING_AUTO: crop_b follows one state per camera (the plain stream, each source), stepped once per call frame,
+ *     in frame order, on that frame's small mask (bsb_get_stage_u8 stage 2): the box of its person pixels (ofinal < 128
+ *     inside the output ROI; fewer than max(1, w*h/1000) of them: the whole frame) mapped to the frame through the ROI,
+ *     widened to the frame's output aspect with margin_pct of the box height as headroom and on each side, at most
+ *     max_zoom_pct zoom, shifted into the frame, then smoothed by `speed` (bsb_set_framing_auto).  A camera without a state
+ *     (its first AUTO frame, after bsb_reset_state / bsb_reset_source / bsb_set_sources, or after a frame not in AUTO)
+ *     jumps to its target.  DESIGN.md §4 states the formula.
+ * Interactions: held frames (bsb_set_mask_interval) step the state on the small mask they are composited with; frames
+ * with the filter off are framed like any other; fed calls (bsb_test_feed, both stages) step the state; ring cursors,
+ * live backgrounds and callbacks are unchanged; a split host-buffer call carries the state across its chunks in stream
+ * order; bs_maskgen_process and the bsb_calcmask_* front end never frame.  A call without a framed frame runs exactly the
+ * kernels it ran before framing existed.
+ * mode: BSB_FRAMING_*; x, y, w, h are read for BSB_FRAMING_RECT only.  An unknown mode or a rectangle outside the frame
+ * returns 0 with a bsb_last_error() message and changes nothing. */
+enum { BSB_FRAMING_OFF = 0, BSB_FRAMING_RECT = 1, BSB_FRAMING_AUTO = 2 };
+BSB_API int bsb_set_framing(bsb_ctx* ctx, int mode, int x, int y, int w, int h);
+/* Auto-framing parameters of the context (every camera): max_zoom_pct 100..1000 (the crop is at least H*100/max_zoom_pct
+ * rows high; default 300), margin_pct 0..100 (default 10), speed 1..256 (the share of the remaining distance, in 1/256,
+ * the crop moves per frame; 256 jumps; default 32).  Out of range returns 0 with a bsb_last_error() message and changes
+ * nothing.  Captured calls are dropped (the parameters are kernel arguments). */
+BSB_API int bsb_set_framing_auto(bsb_ctx* ctx, int max_zoom_pct, int margin_pct, int speed);
+/* One source's framing: mode -1 follows bsb_set_framing (its rectangle included, and later changes), else the source's
+ * own mode and rectangle.  bsb_set_sources resets every source to -1; bsb_reset_source keeps it.  Host bookkeeping only:
+ * it reaches the device in the call's framing table.  No bsb_set_sources yet, a source id out of range, an unknown mode
+ * or a rectangle outside the frame returns 0 with a bsb_last_error() message and changes nothing. */
+BSB_API int bsb_set_source_framing(bsb_ctx* ctx, int source, int mode, int x, int y, int w, int h);
+/* The crop (x, y, w, h) frame `frame` of the last call used (frames of a split host-buffer call by their index in the
+ * caller's call); (0, 0, W, H) when that call was not framed.  Synchronises the context's stream.  A frame outside the
+ * last call returns 0 with a bsb_last_error() message. */
+BSB_API int bsb_get_framing(bsb_ctx* ctx, int frame, int rect[4]);
 /* Live backgrounds (the reference's `-b` takes any OpenCV source and blends its newest frame every loop iteration,
  * app/deepseg.cc:522-524,648-661): device images the caller already holds (decoded video surfaces, screen captures, a
  * second camera) are resized, blurred and blended inside the call, with no host copy and no launch outside it.
