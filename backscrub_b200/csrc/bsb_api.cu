@@ -668,8 +668,9 @@ bool stage_begin(int device) {
   if (device < 0 || device >= n || cudaSetDevice(device) != cudaSuccess) { g_last_error = "invalid CUDA device"; return false; }
   return true;
 }
+// the helpers run on the legacy default stream; a device-wide synchronise would break another thread's graph capture
 bool stage_end() {
-  cudaError_t e = cudaDeviceSynchronize();
+  cudaError_t e = cudaStreamSynchronize(0);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) { g_last_error = std::string("CUDA error: ") + cudaGetErrorString(e); return false; }
   return true;

@@ -919,7 +919,10 @@ bool Engine::upload(std::string* err) {
   if (!refresh_bg_yuyv(err)) return false;
   // the Gaussian's tap tables must exist before a launch is captured into a graph
   if (!gauss_tables_ready()) { *err = "could not allocate the Gaussian tap tables"; return false; }
-  CUDA_OK(cudaDeviceSynchronize());
+  // wait for the copies and kernels above: they ran on the legacy default stream and on stream_.  Not a device-wide
+  // synchronise: that is refused while another thread's context captures a graph, and it breaks that capture.
+  CUDA_OK(cudaStreamSynchronize(0));
+  CUDA_OK(cudaStreamSynchronize(stream_));
   return true;
 }
 

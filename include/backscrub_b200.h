@@ -15,7 +15,18 @@
  *   - errors: NULL / negative return + message via the ondebug callback (or stderr) and
  *     bsb_last_error(); no exceptions cross the boundary;
  *   - one context is used by one thread at a time; contexts are independent (one per
- *     stream / GPU); the library has no global mutable state except the error string.
+ *     stream / GPU) and may be used from several threads at once.  What they share:
+ *       - the bsb_set_tuning switches: process-wide, set before contexts are created,
+ *         and never changed while any call is in flight;
+ *       - per-device caches built on first use under mutexes: the kernels' shared-memory
+ *         attributes, the encoder carveouts, the Gaussian tap tables;
+ *       - the process-wide launch total, bsb_total_launches (bsb_launches_per_call counts
+ *         the launches of the calling thread only);
+ *     the error string is per thread.  tests/test_concurrent_contexts.py runs contexts,
+ *     the bsb_calcmask_* worker and refused calls from several threads at once, in a
+ *     process whose first context builds the caches, and checks every output,
+ *     launches_per_call and each thread's error string against the same calls made one
+ *     thread at a time.  It keeps the switches at their defaults throughout.
  *   - There is NO CPU fallback: every entry point that computes requires a CUDA device
  *     and fails loudly without one.
  */
