@@ -83,3 +83,9 @@ def set_tuning(name: str, value: int) -> None:
     """Process-wide launcher switch (include/backscrub_b200.h: bsb_set_tuning); selects between bit-identical kernels."""
     if not lib().bsb_set_tuning(name.encode(), int(value)):
         raise BackscrubError(lib().bsb_last_error().decode())
+
+
+def mask_refine_weights(sigma: int):
+    """The range weights R_sigma[d], d = 0..255, of mask refinement strength sigma 1..255 (include/backscrub_b200.h:
+    bsb_mask_refine_weights), as an int64 array."""
+    return api.mask_refine_weights(lib(), sigma)

@@ -120,6 +120,12 @@ class MaskGen:
         if not self._lib.bsb_set_mask_interval(self._h, int(k)):
             self._fail("bsb_set_mask_interval")
 
+    def set_mask_refine(self, sigma: int):
+        """mask edge refinement strength 0..255 (0 = off, the default): each frame's mask is upsampled guided by its own
+        camera frame (include/backscrub_b200.h, bsb_set_mask_refine)"""
+        if not self._lib.bsb_set_mask_refine(self._h, int(sigma)):
+            self._fail("bsb_set_mask_refine")
+
     _FRAMING = {"off": 0, "rect": 1, "auto": 2}
 
     def _framing_args(self, what, mode, rect):
@@ -405,6 +411,11 @@ class MaskGen:
         if not self._lib.bsb_set_source_mask_interval(self._h, int(source), -1 if k is None else int(k)):
             self._fail("bsb_set_source_mask_interval")
 
+    def set_source_mask_refine(self, source: int, sigma=None):
+        """mask refinement strength of one source: None = follow set_mask_refine, including later changes; otherwise 0..255"""
+        if not self._lib.bsb_set_source_mask_refine(self._h, int(source), -1 if sigma is None else int(sigma)):
+            self._fail("bsb_set_source_mask_refine")
+
     def set_source_output(self, source: int, out_size=None):
         """virtual-camera size of one source (cv::resize after the flip, app/deepseg.cc:677-679): out_size = (w, h), or
         None to follow set_output's size, including later changes.  The mask stays W x H."""
@@ -607,6 +618,14 @@ def gaussian_taps(lib, ksize):
     if not lib.bsb_gaussian_taps(int(ksize), q):
         raise BackscrubError(lib.bsb_last_error().decode())
     return np.array(q[:ksize], np.int64)
+
+
+def mask_refine_weights(lib, sigma):
+    """the range weights R_sigma[d], d = 0..255, of mask refinement strength sigma 1..255 (bsb_mask_refine_weights)"""
+    w = (C.c_int * 256)()
+    if not lib.bsb_mask_refine_weights(int(sigma), w):
+        raise BackscrubError(lib.bsb_last_error().decode())
+    return np.array(w[:], np.int64)
 
 
 def flip(lib, src, flip_h, flip_v, device=0):

@@ -341,9 +341,9 @@ int bsb_maskgen_process(bsb_ctx* ctx, const uint8_t* frame, size_t frame_pitch, 
   if (!check_ctx(ctx)) return 0;
   Engine* e = ctx->eng;
   const size_t npix = (size_t)e->W() * e->H();
-  if (!host_call(ctx, {1, bsb::IN_BGR, frame, frame_pitch, 0, npix * 3, nullptr, nullptr, 0, nullptr, 0, e->h_mask(), npix, true},
-                 "failed to interpret video frame: "))
-    return 0;
+  bsb::Call c{1, bsb::IN_BGR, frame, frame_pitch, 0, npix * 3, nullptr, nullptr, 0, nullptr, 0, e->h_mask(), npix, true};
+  c.mask_only_api = true;                      // the drop-in mask API is never refined
+  if (!host_call(ctx, c, "failed to interpret video frame: ")) return 0;
   if (mask) *mask = e->h_mask();
   if (mask_pitch) *mask_pitch = (size_t)e->W();
   return 1;
@@ -423,6 +423,20 @@ int bsb_set_source_framing(bsb_ctx* ctx, int source, int mode, int x, int y, int
   if (!check_ctx(ctx)) return 0;
   std::string err;
   if (!ctx->eng->set_source_framing(source, mode, x, y, w, h, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
+int bsb_set_mask_refine(bsb_ctx* ctx, int sigma) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_mask_refine(sigma, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
+int bsb_set_source_mask_refine(bsb_ctx* ctx, int source, int sigma) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_source_mask_refine(source, sigma, &err)) { report(&ctx->cb, "error: " + err); return 0; }
   return 1;
 }
 
@@ -736,6 +750,11 @@ int bsb_gaussian_taps(int ksize, int* taps) {
   bsb::GaussTaps t{};
   if (!taps || !bsb::gauss_taps(ksize, &t)) { g_last_error = "strength value must be odd (1..255)"; return 0; }
   for (int i = 0; i < ksize; ++i) taps[i] = t.q[i];
+  return 1;
+}
+
+int bsb_mask_refine_weights(int sigma, int* w) {
+  if (!w || !bsb::refine_weights(sigma, w)) { g_last_error = "mask refinement strength must be 1..255 (and w non-null)"; return 0; }
   return 1;
 }
 

@@ -915,6 +915,28 @@ bool Engine::upload(std::string* err) {
     for (int tx = 0; tx < ntx128; ++tx) geo[geo_nty_ + geo_ntx64_ + tx] = span(tx * 128 - roi_x - 2, 132, roi_w, up.xofs, up.xofs, 1, sw - 1);
     CUDA_OK(cudaMalloc((void**)&d_tile_geo_, geo.size() * sizeof(int2)));
     CUDA_OK(cudaMemcpy(d_tile_geo_, geo.data(), geo.size() * sizeof(int2), cudaMemcpyHostToDevice));
+    // mask edge refinement: the unclamped cv::resize position of every ROI column / row, and the patch a tile's
+    // refinement reaches (taps s - 1 .. s + 2 of its ROI pixels, clamped into the small mask)
+    const int sh = out_roidim_[3];
+    std::vector<unsigned> taps((size_t)roi_w + roi_h);
+    const double scx = resize_scale(sw, roi_w), scy = resize_scale(sh, roi_h);
+    for (int x = 0; x < roi_w; ++x) taps[x] = refine_tap(x, scx);
+    for (int y = 0; y < roi_h; ++y) taps[(size_t)roi_w + y] = refine_tap(y, scy);
+    auto rspan = [&](int lo, int len, int origin, int n_roi, const unsigned* t, int n) {
+      const int a = std::max(lo - origin, 0), b = std::min(lo + len - 1 - origin, n_roi - 1);
+      if (a > b) return make_int2(0, 1);        // no ROI pixel: the tile loads no patch
+      const int r0 = std::max((int)(t[a] & 0xffffu) - 2, 0), r1 = std::min((int)(t[b] & 0xffffu) + 1, n - 1);
+      return make_int2(r0, r1 - r0 + 1);
+    };
+    std::vector<int2> geo_r(geo.size());
+    for (int ty = 0; ty < geo_nty_; ++ty) geo_r[ty] = rspan(ty * 32, 32, roi_y, roi_h, taps.data() + roi_w, sh);
+    for (int tx = 0; tx < geo_ntx64_; ++tx) geo_r[geo_nty_ + tx] = rspan(tx * 64, 64, roi_x, roi_w, taps.data(), sw);
+    for (int tx = 0; tx < ntx128; ++tx) geo_r[geo_nty_ + geo_ntx64_ + tx] = rspan(tx * 128, 128, roi_x, roi_w, taps.data(), sw);
+    CUDA_OK(cudaMalloc((void**)&d_refine_taps_, taps.size() * sizeof(unsigned)));
+    CUDA_OK(cudaMemcpy(d_refine_taps_, taps.data(), taps.size() * sizeof(unsigned), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMalloc((void**)&d_tile_geo_r_, geo_r.size() * sizeof(int2)));
+    CUDA_OK(cudaMemcpy(d_tile_geo_r_, geo_r.data(), geo_r.size() * sizeof(int2), cudaMemcpyHostToDevice));
+    CUDA_OK(cudaMalloc((void**)&d_refine_, (size_t)max_batch_ * sizeof(int)));
   }
   if (!refresh_bg_yuyv(err)) return false;
   // the Gaussian's tap tables must exist before a launch is captured into a graph
@@ -940,7 +962,8 @@ Engine::~Engine() {
   for (ChainPlan& cp : chains_) if (cp.d_ops) cudaFree(cp.d_ops);
   free_sources();
   for (void* p : {(void*)d_src_tab_, (void*)d_src_raw_, tab_src_.blob, (void*)d_pass_all_, (void*)d_live_tab_, (void*)d_live_stage_, (void*)d_seg_tab_,
-                  (void*)d_frame_tab_, (void*)d_crop_, (void*)d_frame_box_, (void*)d_frame_counter_, (void*)d_frame_state_})
+                  (void*)d_frame_tab_, (void*)d_crop_, (void*)d_frame_box_, (void*)d_frame_counter_, (void*)d_frame_state_,
+                  (void*)d_refine_, (void*)d_refine_taps_, (void*)d_tile_geo_r_})
     if (p) cudaFree(p);
   for (LiveSize& l : live_sizes_) if (l.tab.blob) cudaFree(l.tab.blob);
   if (h_mask_) cudaFreeHost(h_mask_);
@@ -1277,6 +1300,20 @@ bool check_framing(int mode, int x, int y, int w, int h, int W, int H, bool foll
 }
 }  // namespace
 
+bool Engine::set_mask_refine(int sigma, std::string* err) {
+  if (sigma < 0 || sigma > 255) { *err = "mask refinement strength must be 0 (off) .. 255"; return false; }
+  refine_ = sigma;
+  return true;
+}
+
+bool Engine::set_source_mask_refine(int source, int sigma, std::string* err) {
+  if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
+  if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
+  if (sigma < -1 || sigma > 255) { *err = "source mask refinement strength must be -1 (follow the context) or 0 (off) .. 255"; return false; }
+  src_refine_[source] = (short)sigma;
+  return true;
+}
+
 bool Engine::set_framing(int mode, int x, int y, int w, int h, std::string* err) {
   if (!check_framing(mode, x, y, w, h, W_, H_, false, err)) return false;
   framing_ = Framing{mode, {x, y, w, h}};
@@ -1376,6 +1413,12 @@ PostArgs Engine::post_args(const Call& c, const Plan& p) const {
   // any passes no table, and its post kernel runs as before.
   if (p.passed) a.pass = p.mode == CALL_PLAIN ? d_pass_all_ : d_src_tab_ + 5 * (size_t)max_batch_;
   a.geo_rows = d_tile_geo_; a.geo_cols64 = d_tile_geo_ + geo_nty_; a.geo_cols128 = d_tile_geo_ + geo_nty_ + geo_ntx64_;
+  // refined frames: the strength table, written before the launch.  A call without one passes no table, and its post
+  // kernel runs as before.
+  if (p.refined) {
+    a.refine = d_refine_; a.refine_w = refine_w_; a.refine_x = d_refine_taps_; a.refine_y = d_refine_taps_ + roidim_[2];
+    a.geo_r_rows = d_tile_geo_r_; a.geo_r_cols64 = d_tile_geo_r_ + geo_nty_; a.geo_r_cols128 = d_tile_geo_r_ + geo_nty_ + geo_ntx64_;
+  }
   return a;
 }
 
@@ -1617,6 +1660,15 @@ bool Engine::run(const Call& c, std::string* err) {
   if (c.fmt != IN_BGR && (W_ & 1)) { *err = "YUYV ingest needs an even width"; return false; }
   std::vector<int> ftab;
   p.framed = framing_rows(c, &ftab);
+  // mask edge refinement: each frame's strength (the source's own, else the context's); the mask-only API never refines
+  std::vector<int> rtab;
+  if (!c.mask_only_api) {
+    rtab.assign((size_t)n, 0);
+    for (int b = 0; b < n; ++b) {
+      rtab[b] = c.ids && src_refine_[c.ids[b]] >= 0 ? src_refine_[c.ids[b]] : refine_;
+      p.refined = p.refined || rtab[b] != 0;
+    }
+  }
   std::vector<int> seg;
   p.m = segment(c, &seg);
   if (c.ids && p.m < n) std::copy(seg.begin(), seg.begin() + 2 * (size_t)max_batch_, tab.begin() + SRC_TAB_SEG * (size_t)max_batch_);
@@ -1639,6 +1691,11 @@ bool Engine::run(const Call& c, std::string* err) {
     if (!d_seg_tab_) CUDA_OK(cudaMalloc((void**)&d_seg_tab_, seg.size() * sizeof(int)));
     CUDA_OK(cudaMemcpyAsync(d_seg_tab_, seg.data(), seg.size() * sizeof(int), cudaMemcpyHostToDevice, stream_));
   }
+  if (p.refined) {
+    if (!refine_w_ && !(refine_w_ = refine_tables())) { *err = "could not allocate the mask refinement tables"; return false; }
+    // outside the graph, before its launch, like the source table
+    CUDA_OK(cudaMemcpyAsync(d_refine_, rtab.data(), rtab.size() * sizeof(int), cudaMemcpyHostToDevice, stream_));
+  }
   if (c.ids) {
     if (((p.gclass | p.live_gclass) & GAUSS_SEPARABLE) && !ensure_gauss_tmp(err)) return false;
     // outside the graph, before its launch: stream order keeps the previous launch's reads ahead of this write
@@ -1657,10 +1714,11 @@ bool Engine::run(const Call& c, std::string* err) {
   eager = true;
 #endif
   static const char* kNoMirror = "the post kernel cannot write this call's mirrored frames";
+  static const char* kNoRefine = "the post kernel cannot take this call's mask refinement (or mirrored frames) at this geometry";
   if (eager) {
     if (!plan_launch(c, &p, err)) return false;
     last_native_ = p.native;
-    if (!enqueue_all(c, p)) { *err = kNoMirror; return false; }
+    if (!enqueue_all(c, p)) { *err = p.refined ? kNoRefine : kNoMirror; return false; }
     CUDA_OK(cudaGetLastError());
     move_cursors(c);
     count_frames(c);
@@ -1683,7 +1741,7 @@ bool Engine::run(const Call& c, std::string* err) {
     if (!enq) {
       if (graph) cudaGraphDestroy(graph);
       cudaGetLastError();
-      *err = kNoMirror;
+      *err = p.refined ? kNoRefine : kNoMirror;
       return false;
     }
     if (ce != cudaSuccess || !graph) {
@@ -1996,6 +2054,7 @@ void Engine::free_sources() {
   src_filter_.clear();
   src_size_.clear();
   src_interval_.clear();
+  src_refine_.clear();
   src_frames_.clear();
   src_framing_.clear();
   src_jump_.clear();
@@ -2048,6 +2107,7 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   src_size_.assign((size_t)n_sources, -1);
   src_live_.assign((size_t)n_sources, Live{});
   src_interval_.assign((size_t)n_sources, -1);
+  src_refine_.assign((size_t)n_sources, -1);
   src_frames_.assign((size_t)n_sources, 0);
   src_framing_.assign((size_t)n_sources, Framing{});
   src_jump_.assign((size_t)n_sources, 1);

@@ -86,6 +86,7 @@ struct Call {
   uint8_t* mask = nullptr; size_t mask_stride = 0;     // W x H
   bool callbacks = false;            // fire the stage callbacks (the call then runs eagerly, synchronised at each stage)
   int frame0 = 0;                    // frame 0's index in the caller's call (a chunk of a split call): plain live backgrounds
+  bool mask_only_api = false;        // bs_maskgen_process: the drop-in mask API, never refined (set_mask_refine)
 };
 
 class Engine {
@@ -148,6 +149,11 @@ class Engine {
   bool set_source_framing(int source, int mode, int x, int y, int w, int h, std::string* err);
   // the crop (x, y, w, h) frame `frame` of the last call showed (synchronises)
   bool get_framing(int frame, int* rect, std::string* err);
+  // Mask edge refinement (include/backscrub_b200.h, bsb_set_mask_refine): strength 0..255, 0 off.  Host state only: each
+  // frame's strength reaches the device as table data with the call.
+  bool set_mask_refine(int sigma, std::string* err);
+  // one source's strength: -1 follows set_mask_refine, else 0..255
+  bool set_source_mask_refine(int source, int sigma, std::string* err);
 
   // Independent sources (camera streams) batched one frame each into a call.  set_sources allocates n zeroed smoother
   // states and the per-source background bank (again: everything reallocated and zeroed, graphs dropped).
@@ -271,6 +277,7 @@ class Engine {
     int m = 0;                       // frames segmented (the CNN batch); m == n: every frame, the parent path with no table
     bool framed = false;             // some frame is framed (RECT or AUTO): k_framing runs and every frame goes through the
                                      // cropping tail from unflipped staging
+    bool refined = false;            // some frame's mask is refined: the post kernel takes the strength table d_refine_
   };
   // the call blends a composite: it has a video output, or a BGR composite output.  A call that does not reads no
   // background and blurs nothing.
@@ -449,6 +456,13 @@ class Engine {
   bool plain_jump_ = true;
   std::vector<char> src_jump_;
   int* d_frame_tab_ = nullptr;       // [FRAMING_ROWS][max_batch] the framing rows of a framed call, written before its launch
+  // ---- mask edge refinement ----
+  int refine_ = 0;                   // the context's strength (plain calls, and sources that follow it)
+  std::vector<short> src_refine_;    // per source: -1 = refine_, else its own
+  int* d_refine_ = nullptr;          // [max_batch] the strength of each frame of a refined call, written before its launch
+  unsigned* d_refine_taps_ = nullptr;   // refine_tap of each ROI column [roi_w] | row [roi_h]
+  int2* d_tile_geo_r_ = nullptr;     // the refinement's patch geometry, laid out as d_tile_geo_
+  const unsigned short* refine_w_ = nullptr;   // the device's range weights (refine_tables), taken before the first refined call
   FrameCrop* d_crop_ = nullptr;      // [max_batch] the crop of each frame of the last framed call (the tail reads it)
   int* d_frame_box_ = nullptr;       // [max_batch][4] targets of a plain call (k_framing scratch)
   unsigned* d_frame_counter_ = nullptr;
@@ -526,23 +540,24 @@ class Engine {
   // are filtered off is table data), resized and the largest output size of the sources, which the tail's grid covers
   // (which frame has which size is table data too), the output format, whether frames blend live backgrounds, with
   // the Gaussian classes they add (their images, sizes and strengths within the classes are the live table's data), and the
-  // CNN batch of a call with held frames (which frames are segmented is the segment rows' data), and whether the call is
-  // framed (modes, rectangles and crops are table data).  The rest of the plan is
+  // CNN batch of a call with held frames (which frames are segmented is the segment rows' data), whether the call is
+  // framed (modes, rectangles and crops are table data), and whether it refines a mask (the strengths are table data).  The
+  // rest of the plan is
   // decided from these.
   struct GraphKey {
     int n, fmt; const void* in; size_t pitch, uv, stride;
     const void* out; const void* video; const void* mask; size_t ostride, vstride, mstride;
     int mode; unsigned gclass; bool all_blur, flipped, resized, passed; long out_px_max; bool bgra; int live; unsigned live_gclass;
-    bool framed;
+    bool framed, refined;
     GraphKey(const Call& c, const Plan& p, long px_max)
         : n(c.n), fmt(c.fmt), in(c.in), pitch(c.pitch), uv(c.uv), stride(c.stride), out(c.out), video(c.video), mask(c.mask),
           ostride(c.out ? c.out_stride : 0), vstride(c.video ? c.video_stride : 0), mstride(c.mask ? c.mask_stride : 0),
           mode(p.mode), gclass(p.gclass), all_blur(p.all_blur), flipped(p.flipped), resized(p.resized), passed(p.passed),
-          out_px_max(px_max), bgra(p.bgra), live(p.live), live_gclass(p.live_gclass), framed(p.framed), seg(p.m) {}
+          out_px_max(px_max), bgra(p.bgra), live(p.live), live_gclass(p.live_gclass), framed(p.framed), refined(p.refined), seg(p.m) {}
     int seg;                         // the CNN batch m (n: every frame segmented, the parent's launches)
     auto tie() const {
       return std::tie(n, fmt, in, pitch, uv, stride, out, video, mask, ostride, vstride, mstride, mode, gclass, all_blur, flipped, resized,
-                      passed, out_px_max, bgra, live, live_gclass, framed, seg);
+                      passed, out_px_max, bgra, live, live_gclass, framed, refined, seg);
     }
     bool operator<(const GraphKey& r) const { return tie() < r.tie(); }
   };

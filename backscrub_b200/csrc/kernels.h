@@ -270,7 +270,20 @@ struct PostArgs {
   // with alpha 255 - mask, or 255 for a frame whose filter is off.  Written mirrored by `flip` like `out`.  Every post
   // kernel compiles it into separate instantiations; with neither `out` nor a video output the call reads no background.
   uint8_t* bgra; size_t bgra_pitch, bgra_stride;
+  // Mask edge refinement (include/backscrub_b200.h, bsb_set_mask_refine; post_math.h refine_px): non-null (DEVICE [B]) when
+  // some frame of the call is refined, frame b at strength refine[b] (0: the blurred upsample as without a table).  Every
+  // table-taking post kernel compiles it into separate instantiations.  refine_w: the range weights of every strength
+  // (refine_tables, row sigma - 1); refine_x [roi_w] / refine_y [roi_h]: refine_tap of each ROI column / row; geo_r_*: the
+  // patch of the small mask a tile's refinement reaches (taps s - 1 .. s + 2 of its pixels), as geo_rows / geo_cols*.
+  const int* refine; const unsigned short* refine_w; const unsigned* refine_x; const unsigned* refine_y;
+  const int2* geo_r_rows; const int2* geo_r_cols64; const int2* geo_r_cols128;
 };
+// Mask edge refinement: R_sigma[d] = max(1, floor(256 exp(-d^2 / (2 sigma^2)) + 0.5)), d = 0..255, in double (the host
+// table of bsb_mask_refine_weights); false for sigma outside 1..255
+bool refine_weights(int sigma, int* w);
+// the [255][256] u16 range weights of every strength on the CURRENT device, built on first use (one per device, under a
+// mutex like the Gaussian tap tables); null when the allocation fails
+const unsigned short* refine_tables();
 // false (nothing launched) when a.flip is set and k_post_tma cannot take the arguments
 bool launch_post(cudaStream_t s, const PostArgs& a);
 // true if launch_post will take the TMA kernel for these arguments (the only one that can read a.yuyv_in / a.nv12_in)

@@ -10,6 +10,11 @@
 #include "post_math.h"
 #include "resize_taps.h"
 
+#include <cmath>
+#include <map>
+#include <mutex>
+#include <vector>
+
 namespace bsb {
 
 void count_launch();
@@ -666,7 +671,10 @@ __global__ void __launch_bounds__(256) k_post(PostArgs a) {
 
 // PASS: the launch has a filter table (PostArgs::pass); without one the kernel is compiled without the pass-through.
 // BGRA: the launch writes the transparent output (PostArgs::bgra); without OUT and YUYV it reads no background.
-template <bool OUT, bool YUYV, bool PASS, bool BGRA = false>
+// REFINE: the launch has a refinement table (PostArgs::refine).  A mixed tile of a refined frame loads the patch its
+// refinement reaches, puts it with the guide lumas into Hs and the frame's range row into Us, and computes each thread's
+// mask from the camera bytes after they are loaded (refine_mask16, staged through Vs); A1 / A2 / B do not run.
+template <bool OUT, bool YUYV, bool PASS, bool BGRA = false, bool REFINE = false>
 __global__ void __launch_bounds__(256, 4) k_post_fast(PostArgs a) {
   __shared__ __align__(16) unsigned short Hs[PF_RMAX * PF_US];
   __shared__ __align__(16) unsigned short Us[PF_UH * PF_US];
@@ -680,6 +688,8 @@ __global__ void __launch_bounds__(256, 4) k_post_fast(PostArgs a) {
   const bool pass = PASS && __ldg(a.pass + b) != 0;
   const bool hits_roi = (!pass || a.mask) && tx0 < a.roi_x + a.roi_w && tx0 + PF_W > a.roi_x && ty0 < a.roi_y + a.roi_h && ty0 + PF_H > a.roi_y;
   int tile_const = -1;                       // 255 / 0 when the whole mask tile is known to be constant
+  const int sig = REFINE ? __ldg(a.refine + b) : 0;
+  int rmin = 0, cmin = 0;                    // the patch's first small row / column
   {
     // pull this thread's 48 bytes of camera frame into L2 while the mask tile is being built
     const int px0 = tx0 + (tid & 7) * PF_PX, py = ty0 + (tid >> 3);
@@ -695,10 +705,19 @@ __global__ void __launch_bounds__(256, 4) k_post_fast(PostArgs a) {
     const int gx_lo = tx0 - a.roi_x - 2, gx_hi = gx_lo + PF_UW - 1;
     const int gx_min = gx_lo < 0 ? 0 : min(gx_lo, a.roi_w - 1);
     const int gx_max = gx_hi >= a.roi_w ? a.roi_w - 1 : max(gx_hi, 0);
-    const int rmin = __ldg(a.tab.yofs0 + gy_min);
-    const int nrows = __ldg(a.tab.yofs1 + gy_max) - rmin + 1;
-    const int cmin = (int)(__ldg(&a.tab.xcol[gx_min].x) & 0xffffu);
-    const int ncols = (int)(__ldg(&a.tab.xcol[gx_max].x) >> 16) - cmin + 1;
+    rmin = __ldg(a.tab.yofs0 + gy_min);
+    int nrows = __ldg(a.tab.yofs1 + gy_max) - rmin + 1;
+    cmin = (int)(__ldg(&a.tab.xcol[gx_min].x) & 0xffffu);
+    int ncols = (int)(__ldg(&a.tab.xcol[gx_max].x) >> 16) - cmin + 1;
+    if (REFINE && sig) {
+      // a refined frame: the small rows / columns taps s - 1 .. s + 2 of the tile's ROI pixels reach
+      const int ylo = max(ty0, a.roi_y) - a.roi_y, yhi = min(ty0 + PF_H, a.roi_y + a.roi_h) - 1 - a.roi_y;
+      const int xlo = max(tx0, a.roi_x) - a.roi_x, xhi = min(tx0 + PF_W, a.roi_x + a.roi_w) - 1 - a.roi_x;
+      rmin = max((int)(__ldg(a.refine_y + ylo) & 0xffffu) - 2, 0);
+      nrows = min((int)(__ldg(a.refine_y + yhi) & 0xffffu) + 1, a.out_h - 1) - rmin + 1;
+      cmin = max((int)(__ldg(a.refine_x + xlo) & 0xffffu) - 2, 0);
+      ncols = min((int)(__ldg(a.refine_x + xhi) & 0xffffu) + 1, a.out_w - 1) - cmin + 1;
+    }
     // ---- P: source patch of the small mask -> shared memory (coalesced); row parameters for A2.
     //      If every source pixel of the patch is 255 (or 0) the upsampled + blurred tile is 255 (or 0)
     //      whatever the interpolation weights are (their sums are 2048 +- 1), so A1/A2/B are skipped. ----
@@ -723,7 +742,16 @@ __global__ void __launch_bounds__(256, 4) k_post_fast(PostArgs a) {
     const int all_hi = __syncthreads_and(p_and == 255u);
     const int all_lo = all_hi ? 0 : __syncthreads_and(p_or == 0u);
     tile_const = all_hi ? 255 : (all_lo ? 0 : -1);
-    if (tile_const < 0) {
+    if (REFINE && sig && tile_const < 0) {
+      // ---- R: the refinement patch (mask | guide luma << 8) -> Hs, the frame's range row -> Us ----
+      const uint8_t* fr = a.frames + (size_t)b * a.frame_stride;
+      refine_patch(a, Ps, PF_PS, rmin, nrows, cmin, ncols, Hs, PF_US, tid, 256, [&](int x, int yy, int* bgr) {
+        const uint8_t* p = fr + (size_t)yy * a.frame_pitch + (size_t)x * 3;
+        bgr[0] = p[0]; bgr[1] = p[1]; bgr[2] = p[2];
+      });
+      Us[tid] = __ldg(a.refine_w + (size_t)(sig - 1) * 256 + tid);
+      __syncthreads();
+    } else if (tile_const < 0) {
     // ---- A1: horizontal pass of cv::resize on the patch rows: Hs = (s[sx]*a0 + s[sx1]*a1) >> 4.
     //      A thread owns a column (parameters in registers) and walks every second patch row. ----
     {
@@ -781,7 +809,8 @@ __global__ void __launch_bounds__(256, 4) k_post_fast(PostArgs a) {
 
   // ---- issue the streaming loads early ----
   unsigned f[12], g[12];
-  if (OUT || YUYV || BGRA) {
+  const bool refined = REFINE && sig && hits_roi && tile_const < 0;    // the refined mask reads the camera bytes
+  if (OUT || YUYV || BGRA || refined) {
     const uint8_t* fp = a.frames + (size_t)b * a.frame_stride + (size_t)y * a.frame_pitch + (size_t)x0 * 3;
     const uint8_t* gp = a.bg + bg_frame_offset(a, b) + (size_t)y * a.bg_pitch + (size_t)x0 * 3;
 #pragma unroll
@@ -796,7 +825,8 @@ __global__ void __launch_bounds__(256, 4) k_post_fast(PostArgs a) {
   // ---- C: horizontal 5-sums on packed lanes -> 16 mask values ----
   unsigned m[PF_PX];
   const bool row_in = hits_roi && y >= a.roi_y && y < a.roi_y + a.roi_h;
-  post_mask16(a, row_in, tile_const, x0, Vs + ly * PF_US + lx, m);
+  if (refined) refine_mask16(a, row_in, x0, y, f, Hs, PF_US, rmin, cmin, Us, reinterpret_cast<uint8_t*>(Vs) + ly * PF_W + lx, m);
+  else post_mask16(a, row_in, tile_const, x0, Vs + ly * PF_US + lx, m);
 
   if (a.mask) {
     uint4 mv;
@@ -849,17 +879,25 @@ static bool post_fast_ok(const PostArgs& a) {
   if ((int)(PF_UH * scale_y) + 3 > PF_RMAX) return false;
   const double scale_x = (double)a.out_w / (double)a.roi_w;
   if ((int)(PF_UW * scale_x) + 4 > PF_PS || a.tab.xcol == nullptr) return false;
+  // a refined tile's patch: taps s - 1 .. s + 2 of its 32 rows / 128 columns, in Ps and (u16, PF_US apart) in Hs
+  if (a.refine && ((int)((PF_H - 1) * scale_y) + 6 > PF_RMAX || (int)((PF_W - 1) * scale_x) + 6 > PF_US || !a.refine_x)) return false;
   return true;
 }
 
 bool launch_post_tma(cudaStream_t s, const PostArgs& a);   // kernels_post.cu
 
-template <bool PASS, bool BGRA = false>
+template <bool PASS, bool BGRA = false, bool REFINE = false>
 static void launch_post_fast(cudaStream_t s, dim3 grid, const PostArgs& a) {
-  if (a.yuyv && a.out) { auto k = k_post_fast<true, true, PASS, BGRA>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
-  else if (a.yuyv) { auto k = k_post_fast<false, true, PASS, BGRA>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
-  else if (a.out) { auto k = k_post_fast<true, false, PASS, BGRA>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
-  else { auto k = k_post_fast<false, false, PASS, BGRA>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  if (a.yuyv && a.out) { auto k = k_post_fast<true, true, PASS, BGRA, REFINE>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  else if (a.yuyv) { auto k = k_post_fast<false, true, PASS, BGRA, REFINE>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  else if (a.out) { auto k = k_post_fast<true, false, PASS, BGRA, REFINE>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+  else { auto k = k_post_fast<false, false, PASS, BGRA, REFINE>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
+}
+template <bool REFINE>
+static void launch_post_fast_r(cudaStream_t s, dim3 grid, const PostArgs& a) {
+  if (a.bgra) { if (a.pass) launch_post_fast<true, true, REFINE>(s, grid, a); else launch_post_fast<false, true, REFINE>(s, grid, a); }
+  else if (a.pass) launch_post_fast<true, false, REFINE>(s, grid, a);
+  else launch_post_fast<false, false, REFINE>(s, grid, a);
 }
 
 bool launch_post(cudaStream_t s, const PostArgs& a_in) {
@@ -870,12 +908,13 @@ bool launch_post(cudaStream_t s, const PostArgs& a_in) {
   a.frame_l1 = tuning().post_l1;                 // measurement switch: frame loads allocate in L1
   if (post_fast_ok(a)) {
     dim3 grid((unsigned)ceil_div(a.W, PF_W), (unsigned)ceil_div(a.H, PF_H), (unsigned)a.B);
-    if (a.bgra) { if (a.pass) launch_post_fast<true, true>(s, grid, a); else launch_post_fast<false, true>(s, grid, a); }
-    else if (a.pass) launch_post_fast<true>(s, grid, a);
-    else launch_post_fast<false>(s, grid, a);
+    if (a.refine) launch_post_fast_r<true>(s, grid, a);
+    else launch_post_fast_r<false>(s, grid, a);
     count_launch();
     return true;
   }
+  // refined frames are taken by k_post_tma and k_post_fast only: a refinement table neither can take is an error
+  if (a.refine) return false;
   dim3 grid((unsigned)ceil_div(a.W, PT_W), (unsigned)ceil_div(a.H, PT_H), (unsigned)a.B);
   if (a.bgra) {
     if (a.pass) { auto k = k_post<true, true>; BSB_LAUNCH(k, grid, dim3(256), 0, s, a); }
@@ -1375,6 +1414,39 @@ __global__ void __launch_bounds__(256) k_framing(FramingArgs a) {
 void launch_framing(cudaStream_t s, const FramingArgs& a) {
   BSB_LAUNCH(k_framing, dim3((unsigned)a.n), dim3(256), 0, s, a);
   count_launch();
+}
+
+// ---------------------------------------------------------------------------
+// Mask edge refinement: the range weights (include/backscrub_b200.h, bsb_mask_refine_weights)
+// ---------------------------------------------------------------------------
+bool refine_weights(int sigma, int* w) {
+  if (sigma < 1 || sigma > 255) return false;
+  for (int d = 0; d < 256; ++d) {
+    const int v = (int)std::floor(256.0 * std::exp(-(double)d * d / (2.0 * sigma * sigma)) + 0.5);
+    w[d] = v < 1 ? 1 : v;
+  }
+  return true;
+}
+
+const unsigned short* refine_tables() {
+  static std::mutex mu;
+  static std::map<int, unsigned short*> tabs;
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
+  std::lock_guard<std::mutex> lock(mu);
+  auto it = tabs.find(dev);
+  if (it != tabs.end()) return it->second;
+  std::vector<unsigned short> h((size_t)255 * 256);
+  int w[256];
+  for (int sg = 1; sg <= 255; ++sg) {
+    refine_weights(sg, w);
+    for (int d = 0; d < 256; ++d) h[(size_t)(sg - 1) * 256 + d] = (unsigned short)w[d];
+  }
+  unsigned short* d = nullptr;
+  if (cudaMalloc((void**)&d, h.size() * sizeof(unsigned short)) != cudaSuccess) return nullptr;
+  if (cudaMemcpy(d, h.data(), h.size() * sizeof(unsigned short), cudaMemcpyHostToDevice) != cudaSuccess) { cudaFree(d); return nullptr; }
+  tabs[dev] = d;
+  return d;
 }
 
 }  // namespace bsb

@@ -20,7 +20,11 @@
 //   * a launch with the transparent output (PostArgs::bgra) loads the camera tile of every tile, and background tiles
 //     take the mixed-tile path (the blend of mask 255 is the background, bit for bit); each thread writes its 16 BGRA
 //     pixels (camera bytes, alpha 255 - mask) with 16-byte stores straight from registers, mirrored in place for a
-//     flipped frame.  Without a composite or video output it loads no background at all.
+//     flipped frame.  Without a composite or video output it loads no background at all;
+//   * a launch with a refinement table (PostArgs::refine) loads, for a refined frame, the patch of the small mask its
+//     refinement reaches (geo_r_*); a mixed tile gathers the guide luma of every patch entry from the camera frame in its
+//     wire format, takes the frame's range row into shared memory and computes each pixel's mask from the camera tile
+//     (post_math.h refine_mask16) instead of the resize + blur passes.  Uniform tiles keep their copy path.
 // Arithmetic is shared with k_post_fast through post_math.h, so both kernels produce the oracle's bits.
 #include "kernels.h"
 #include "post_math.h"
@@ -143,8 +147,9 @@ template <int TW> struct PtL {
 // FMT: IN_BGR / IN_YUYV frames with YUYV video output, or IN_NV12 frames with NV12 video output.  FLIP: the launch has a
 // flip table (sources calls); without one the kernel is compiled without the mirroring paths.  PASS: the launch has a
 // filter table; without one the kernel is compiled without the pass-through paths.  BGRA: the launch writes the
-// transparent output; without it the kernel is compiled without those paths.
-template <int FMT, int TW, bool FLIP, bool PASS, bool BGRA>
+// transparent output; without it the kernel is compiled without those paths.  REFINE: the launch has a refinement table;
+// without one the kernel is compiled without the refinement.
+template <int FMT, int TW, bool FLIP, bool PASS, bool BGRA, bool REFINE>
 __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const __grid_constant__ PostMapsOf<FMT> tm, const PostArgs a, const PostTmaCfg cfg) {
   using L = PtL<TW>;
   constexpr bool IN_YUYV = FMT == InFmt::IN_YUYV, NV12 = FMT == InFmt::IN_NV12;
@@ -167,8 +172,8 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
   const int ty0 = blockIdx.y * PF_H, tx0 = blockIdx.x * TW;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   int* geo = reinterpret_cast<int*>(smem + L::OFF_GEO);                 // tile geometry, published by thread 0
-  // geo[9]: the frame's flip code, and with PASS its filter-off flag in bit 2
-  auto flip_code = [&]() -> int { return FLIP ? (PASS ? (geo[9] & 3) : geo[9]) : 0; };
+  // geo[9]: the frame's flip code, with PASS its filter-off flag in bit 2, with REFINE its refinement strength from bit 8
+  auto flip_code = [&]() -> int { return FLIP ? ((PASS || REFINE) ? (geo[9] & 3) : geo[9]) : 0; };
   // a transparent output alone blends nothing: no background tile is loaded or waited for
   const bool bgra_only = BGRA && !cfg.has_out && !cfg.has_yuyv;
 
@@ -180,13 +185,19 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
     tma::fence_barrier_init();
     // a filtered-off frame needs the mask patch only for the mask output
     const bool pass = PASS && __ldg(a.pass + b) != 0;
+    const int sig = REFINE ? __ldg(a.refine + b) : 0;
     const bool hit = (!pass || cfg.has_mask) && tx0 < a.roi_x + a.roi_w && tx0 + TW > a.roi_x && ty0 < a.roi_y + a.roi_h && ty0 + PF_H > a.roi_y;
     // the patch of the small mask this tile touches comes from two per-context tables (engine.cu): two independent
     // loads whose addresses need nothing but the block index, then the patch request — the head of the CTA's critical
     // path — goes out first ...
     int gy_lo = 0, gx_lo = 0, rmin = 0, nrows = 0, cmin = 0, ncols = 0, coff = 0;
     if (hit) {
-      const int2 gr = __ldg(a.geo_rows + blockIdx.y), gc = __ldg((TW == 64 ? a.geo_cols64 : a.geo_cols128) + blockIdx.x);
+      int2 gr = __ldg(a.geo_rows + blockIdx.y), gc = __ldg((TW == 64 ? a.geo_cols64 : a.geo_cols128) + blockIdx.x);
+      if (REFINE) {
+        // (both patches are requested at once: the strength selects without a dependent load)
+        const int2 rr = __ldg(a.geo_r_rows + blockIdx.y), rc = __ldg((TW == 64 ? a.geo_r_cols64 : a.geo_r_cols128) + blockIdx.x);
+        if (sig) { gr = rr; gc = rc; }
+      }
       gy_lo = ty0 - a.roi_y - 2; gx_lo = tx0 - a.roi_x - 2;
       rmin = gr.x; nrows = gr.y; cmin = gc.x; ncols = gc.y;
       coff = (a.out_x + cmin) & 15;                     // the patch's first column inside the 16-byte aligned box
@@ -201,6 +212,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
     else if (a.bg_stride) bgi = b;
     if (FLIP) geo[9] = __ldg(a.flip + b);             // the frame's flip code, read by every thread after the first barrier
     if (PASS) geo[9] = (FLIP ? geo[9] : 0) | (pass ? 4 : 0);
+    if (REFINE) geo[9] = ((FLIP || PASS) ? geo[9] : 0) | (sig << 8);
     if (!pass && !bgra_only) {                         // (a filtered-off frame arms no background barrier, nor waits on it)
       tma::mbar_expect_tx(barB, (unsigned)L::F_BYTES + (cfg.has_bgy ? (NV12 ? (unsigned)L::N_BYTES : (unsigned)L::Y_BYTES) : 0u));
       tma::load_3d(sB, &tm.bg, blockIdx.x * (TW * 3 / 4), ty0, bgi, barB);
@@ -236,6 +248,8 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
   const bool pz = PASS && (geo[9] & 4) != 0;            // the frame's filter is off
   const bool nobg = pz || bgra_only;                     // no background tile was loaded
   const int gy_lo = g0.y, gx_lo = g0.z, rmin = g0.w, nrows = g1.x, cmin = g1.y, ncols = g1.z, coff = g1.w;
+  const int sig = REFINE ? (geo[9] >> 8) : 0;            // the frame's refinement strength
+  unsigned short* Rs = reinterpret_cast<unsigned short*>(smem + L::OFF_US + L::M_BYTES);   // its range row (refined tiles)
 
   const int lx = (tid % (TW / PF_PX)) * PF_PX, ly = tid / (TW / PF_PX);
   const int y = ty0 + ly;
@@ -277,7 +291,25 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
     tile_const = tk.x; kind = tk.y;
   }
 
-  if (kind == 2 && tile_const < 0) {
+  const bool refined = REFINE && sig && kind == 2 && tile_const < 0;
+  if (refined) {
+    // ---- R: the refinement patch (mask | guide luma << 8, PCOLS apart) over Hs, the frame's range row after the mask
+    //      staging tile.  The guide lumas are gathered from the camera frame in its wire format. ----
+    auto px = [&](int x, int yy, int* bgr) {
+      if constexpr (NV12) {
+        nv12_px_to_bgr(a.nv12_in + (size_t)b * a.nv12_in_stride, a.nv12_in_pitch, a.nv12_in_uv, x, yy, bgr);
+      } else if constexpr (IN_YUYV) {
+        yuyv_px_to_bgr(a.yuyv_in + (size_t)b * a.yuyv_in_stride + (size_t)yy * a.W * 2, x, bgr);
+      } else {
+        const uint8_t* p = a.frames + (size_t)b * a.frame_stride + (size_t)yy * a.frame_pitch + (size_t)x * 3;
+        bgr[0] = p[0]; bgr[1] = p[1]; bgr[2] = p[2];
+      }
+    };
+    refine_patch(a, sP + coff, PW, rmin, nrows, cmin, ncols, Hs, L::PCOLS, tid, NT, px);
+    const unsigned* rw = reinterpret_cast<const unsigned*>(a.refine_w + (size_t)(sig - 1) * 256);
+    for (int i = tid; i < 128; i += NT) reinterpret_cast<unsigned*>(Rs)[i] = __ldg(rw + i);
+    __syncthreads();
+  } else if (kind == 2 && tile_const < 0) {
     // ---- A1: horizontal pass of cv::resize on the patch rows (see k_post_fast) ----
     {
       constexpr int HALF = NT / 2;
@@ -413,6 +445,7 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
 #pragma unroll
       for (int i = 0; i < PF_PX; ++i) m[i] = 0u;
     } else if (!pz || cfg.has_mask) {
+      // (a refined tile's values are replaced below, once its camera bytes are known)
       const bool row_in = (!(PASS || BGRA) || hits_roi) && y >= a.roi_y && y < a.roi_y + a.roi_h;
       post_mask16(a, row_in, tile_const, x0, Vs + ly * US + lx, m);
     }
@@ -436,6 +469,9 @@ __global__ void __launch_bounds__(PtL<TW>::NT, PtL<TW>::CTAS) k_post_tma(const _
       const uint4 f0 = fq[0], f1 = fq[1], f2 = fq[2];
       f[0] = f0.x; f[1] = f0.y; f[2] = f0.z; f[3] = f0.w; f[4] = f1.x; f[5] = f1.y; f[6] = f1.z; f[7] = f1.w;
       f[8] = f2.x; f[9] = f2.y; f[10] = f2.z; f[11] = f2.w;
+    }
+    if constexpr (REFINE) {
+      if (refined) refine_mask16(a, y >= a.roi_y && y < a.roi_y + a.roi_h, x0, y, f, Hs, L::PCOLS, rmin, cmin, Rs, sM + ly * TW + lx, m);
     }
     if (BGRA) {
       // the transparent output, from the camera bytes before the blend overwrites the tile: straight to global memory,
@@ -651,7 +687,11 @@ static bool post_tma_shape_ok(const PostArgs& a) {
   if (a.ow > 32000 || a.oh > 32000 || a.roi_w < 8 || a.roi_h < 8) return false;
   const double scale_y = (double)a.out_h / (double)a.roi_h, scale_x = (double)a.out_w / (double)a.roi_w;
   const int tw = post_tile_width(a);
-  if ((int)(PF_UH * scale_y) + 3 > PT_RMAX || (int)((tw + 4) * scale_x) + 4 > (tw == 128 ? PtL<128>::PCOLS : PtL<64>::PCOLS)) return false;
+  const int pcols = tw == 128 ? PtL<128>::PCOLS : PtL<64>::PCOLS;
+  if ((int)(PF_UH * scale_y) + 3 > PT_RMAX || (int)((tw + 4) * scale_x) + 4 > pcols) return false;
+  // a refined tile's patch: taps s - 1 .. s + 2 of its 32 rows / tw columns
+  if (a.refine && (!a.refine_w || !a.refine_x || !a.geo_r_rows || (int)((PF_H - 1) * scale_y) + 6 > PT_RMAX || (int)((tw - 1) * scale_x) + 6 > pcols))
+    return false;
   return true;
 }
 
@@ -660,25 +700,29 @@ bool post_tma_eligible(const PostArgs& a) {
   return post_tma_shape_ok(a) && build_post_maps(a, &tm, post_tile_width(a), &tm);
 }
 
-template <int FMT, int TW, bool FLIP, bool PASS, bool BGRA>
+template <int FMT, int TW, bool FLIP, bool PASS, bool BGRA, bool REFINE>
 static bool launch_post_tma_f(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
   using L = PtL<TW>;
-  if (!ensure_dyn_smem(reinterpret_cast<const void*>(k_post_tma<FMT, TW, FLIP, PASS, BGRA>), L::SMEM)) return false;
+  if (!ensure_dyn_smem(reinterpret_cast<const void*>(k_post_tma<FMT, TW, FLIP, PASS, BGRA, REFINE>), L::SMEM)) return false;
   const dim3 grid((unsigned)ceil_div(a.W, TW), (unsigned)ceil_div(a.H, PF_H), (unsigned)a.B);
-  k_post_tma<FMT, TW, FLIP, PASS, BGRA><<<grid, L::NT, L::SMEM, s>>>(tm, a, cfg);
+  k_post_tma<FMT, TW, FLIP, PASS, BGRA, REFINE><<<grid, L::NT, L::SMEM, s>>>(tm, a, cfg);
   return true;
 }
-template <int FMT, int TW, bool PASS, bool BGRA>
+template <int FMT, int TW, bool PASS, bool BGRA, bool REFINE>
 static bool launch_post_tma_p(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
-  return a.flip ? launch_post_tma_f<FMT, TW, true, PASS, BGRA>(s, tm, a, cfg) : launch_post_tma_f<FMT, TW, false, PASS, BGRA>(s, tm, a, cfg);
+  return a.flip ? launch_post_tma_f<FMT, TW, true, PASS, BGRA, REFINE>(s, tm, a, cfg) : launch_post_tma_f<FMT, TW, false, PASS, BGRA, REFINE>(s, tm, a, cfg);
 }
-template <int FMT, int TW, bool BGRA>
+template <int FMT, int TW, bool BGRA, bool REFINE>
 static bool launch_post_tma_b(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
-  return a.pass ? launch_post_tma_p<FMT, TW, true, BGRA>(s, tm, a, cfg) : launch_post_tma_p<FMT, TW, false, BGRA>(s, tm, a, cfg);
+  return a.pass ? launch_post_tma_p<FMT, TW, true, BGRA, REFINE>(s, tm, a, cfg) : launch_post_tma_p<FMT, TW, false, BGRA, REFINE>(s, tm, a, cfg);
+}
+template <int FMT, int TW, bool REFINE>
+static bool launch_post_tma_r(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
+  return a.bgra ? launch_post_tma_b<FMT, TW, true, REFINE>(s, tm, a, cfg) : launch_post_tma_b<FMT, TW, false, REFINE>(s, tm, a, cfg);
 }
 template <int FMT, int TW>
 static bool launch_post_tma_t(cudaStream_t s, const PostMapsOf<FMT>& tm, const PostArgs& a, const PostTmaCfg& cfg) {
-  return a.bgra ? launch_post_tma_b<FMT, TW, true>(s, tm, a, cfg) : launch_post_tma_b<FMT, TW, false>(s, tm, a, cfg);
+  return a.refine ? launch_post_tma_r<FMT, TW, true>(s, tm, a, cfg) : launch_post_tma_r<FMT, TW, false>(s, tm, a, cfg);
 }
 
 bool launch_post_tma(cudaStream_t s, const PostArgs& a) {

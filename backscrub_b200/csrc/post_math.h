@@ -159,6 +159,114 @@ BSB_D void post_mask16(const PostArgs& a, bool row_in, int tile_const, int x0, c
 
 }
 
+// ---- mask edge refinement (include/backscrub_b200.h, bsb_set_mask_refine; DESIGN §4) ----
+// A refined frame's mask at pixel p is the joint bilateral upsample of the small mask s against the camera luma L:
+//   M'(p) = (sum w * s[i][j] + (sum w >> 1)) / sum w,  w = ((wx * wy) >> 12) * R[|L(p) - guide(i, j)|]
+// over the 4 x 4 taps of p (refine_w4), R the frame's row of the range weights (refine_weights).  The patch E holds one
+// u16 per small pixel, s[i][j] | guide(i, j) << 8.  Bounds: one w < 2^20, sum w < 2^24, the numerator < 2^32, and
+// sum w >= 1024 (the nearest tap has spatial weight >= 2048 in each axis, R >= 1).
+
+// luma of a BGR pixel: the Y of rgb2yuv
+BSB_HD unsigned luma_bgr(unsigned b, unsigned g, unsigned r) { return (4899u * r + 9617u * g + 1868u * b + 8192u) >> 14; }
+
+// the taps of one axis from its refine_tap entry: patch indices (relative to p0, clamped into the n small pixels so every
+// read stays inside the patch) and spatial weights (0 for a tap outside 0..n-1)
+BSB_D void refine_w4(unsigned pk, int n, int p0, int* idx, unsigned* w) {
+  const int s = (int)(pk & 0xffffu) - 1, a = (int)(pk >> 16);
+  const int wk[4] = {max(0, 1024 - a), 3072 - a, 1024 + a, max(0, a - 1024)};
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const int i = s - 1 + k;
+    w[k] = (i >= 0 && i < n) ? (unsigned)wk[k] : 0u;
+    idx[k] = min(max(i, 0), n - 1) - p0;
+  }
+}
+
+// one refined pixel of luma L: E the patch (row stride es), ri / wy the row taps, ci / wx the column taps, R the range row
+BSB_D unsigned refine_px(const unsigned short* E, int es, const int* ri, const unsigned* wy, const int* ci, const unsigned* wx, unsigned L,
+                         const unsigned short* R) {
+  unsigned sw = 0, sv = 0;
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const unsigned short* er = E + ri[i] * es;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const unsigned e = er[ci[j]];
+      const int d = (int)L - (int)(e >> 8);
+      const unsigned w = ((wx[j] * wy[i]) >> 12) * (unsigned)R[d < 0 ? -d : d];
+      sw += w; sv += w * (e & 255u);
+    }
+  }
+  return (sv + (sw >> 1)) / sw;
+}
+
+// the 16 lumas of a thread's pixels from their BGR bytes f (12 words), packed 4 per word
+BSB_D void luma16(const unsigned* f, unsigned* lw) {
+  const uint8_t* fb = reinterpret_cast<const uint8_t*>(f);
+#pragma unroll
+  for (int q = 0; q < 4; ++q) {
+    unsigned v = 0;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int i = 4 * q + k;
+      v |= luma_bgr(fb[3 * i], fb[3 * i + 1], fb[3 * i + 2]) << (8 * k);
+    }
+    lw[q] = v;
+  }
+}
+
+// the refined mask of one thread's 16 pixels (x0.., row y), through its 16-byte slot `slot` of shared memory (the lumas go
+// in, the masks come out: the pixel loop stays rolled).  E / es / (r0, c0): the patch and its first small row / column;
+// 255 outside the ROI.
+BSB_D void refine_mask16(const PostArgs& a, bool row_in, int x0, int y, const unsigned* f, const unsigned short* E, int es, int r0, int c0,
+                         const unsigned short* R, uint8_t* slot, unsigned* m) {
+  if (!row_in) {
+#pragma unroll
+    for (int i = 0; i < PF_PX; ++i) m[i] = 255u;
+    return;
+  }
+  unsigned lw[4];
+  luma16(f, lw);
+  *reinterpret_cast<uint4*>(slot) = make_uint4(lw[0], lw[1], lw[2], lw[3]);
+  int ri[4]; unsigned wy[4];
+  refine_w4(__ldg(a.refine_y + (y - a.roi_y)), a.out_h, r0, ri, wy);
+#pragma unroll 1
+  for (int i = 0; i < PF_PX; ++i) {
+    const int x = x0 + i;
+    unsigned v = 255u;
+    if (x >= a.roi_x && x < a.roi_x + a.roi_w) {
+      int ci[4]; unsigned wx[4];
+      refine_w4(__ldg(a.refine_x + (x - a.roi_x)), a.out_w, c0, ci, wx);
+      v = refine_px(E, es, ri, wy, ci, wx, slot[i], R);
+    }
+    slot[i] = (uint8_t)v;
+  }
+  const uint4 q = *reinterpret_cast<const uint4*>(slot);
+  const unsigned w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+  for (int i = 0; i < PF_PX; ++i) m[i] = (w[i >> 2] >> (8 * (i & 3))) & 255u;
+}
+
+// the guide luma of small pixel (i, j): the luma of the frame pixel nearest its centre, read by `px(x, y, bgr)`
+template <class Px>
+BSB_D unsigned refine_guide(const PostArgs& a, int i, int j, Px px) {
+  const int gx = a.roi_x + ((2 * j + 1) * a.roi_w) / (2 * a.out_w), gy = a.roi_y + ((2 * i + 1) * a.roi_h) / (2 * a.out_h);
+  int bgr[3];
+  px(gx, gy, bgr);
+  return luma_bgr((unsigned)bgr[0], (unsigned)bgr[1], (unsigned)bgr[2]);
+}
+
+// the refinement patch of small rows [r0, r0 + nr) x columns [c0, c0 + nc): the mask bytes from P (row stride ps, first
+// byte at column c0) with the guide lumas, into E (row stride es); the thread's share of nr * nc entries
+template <class Px>
+BSB_D void refine_patch(const PostArgs& a, const uint8_t* P, int ps, int r0, int nr, int c0, int nc, unsigned short* E, int es, int tid, int nt,
+                        Px px) {
+  for (int k = tid; k < nr * nc; k += nt) {
+    const int r = k / nc, c = k % nc;
+    E[r * es + c] = (unsigned short)(P[r * ps + c] | (refine_guide(a, r0 + r, c0 + c, px) << 8));
+  }
+}
+
 // the blend weight of a pixel with mask m: m, or 0 when its frame's filter is off (PostArgs::pass), so that alpha_blend
 // returns the camera byte exactly ((f * 255) / 255 == f) and post_blend16 takes its all-person path.  The stored mask
 // is m either way.

@@ -33,4 +33,13 @@ BSB_HD void resize_tap_y(int dy, double scale, int sh, int* y0, int* y1, int* w0
   *w1 = (int)lrintf(fy * 2048.f);
 }
 
+// Mask edge refinement (post_math.h, refine_px): the unclamped source position of output index d (relative to the ROI),
+// packed (s + 1) | a << 16 with s = floor(f) >= -1 and a = lrintf((f - s) * 2048) in 0..2048
+BSB_HD unsigned refine_tap(int d, double scale) {
+  const float f = (float)((d + 0.5) * scale - 0.5);
+  const int s = (int)floorf(f);
+  const int a = (int)lrintf((f - (float)s) * 2048.f);
+  return (unsigned)(s + 1) | ((unsigned)a << 16);
+}
+
 }  // namespace bsb

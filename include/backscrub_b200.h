@@ -160,8 +160,9 @@ BSB_API int bsb_set_out_format(bsb_ctx* ctx, int format);
  *   Segmented frame: pre-processing, the CNN, the decision and one smoother step, exactly as at interval 1.
  *   Held frame: none of those.  Its small mask (ofinal) is the smoother state its camera holds now, i.e. the state after
  *     the camera's latest segmented frame; upsampling, blur, blend, flip, resize, BGRA, YUYV / NV12 and the mask output
- *     then proceed as usual.  So its W x H mask is byte for byte that of the latest segmented frame, and its composite is
- *     that mask applied to the new camera frame.
+ *     then proceed as usual.  So without mask refinement (strength 0, bsb_set_mask_refine) its W x H mask is byte for byte
+ *     that of the latest segmented frame, and its composite is that mask applied to the new camera frame; a refined held
+ *     frame refines the held small mask against its own camera frame.
  *   Plain calls: the context counts the frames of its plain calls from 0 (at creation and after bsb_reset_state); frame c
  *     is segmented iff c % k == 0.  The cadence runs across calls and across the chunks of a split host-buffer call; held
  *     frames before a call's first segmented frame hold the state the previous call left.
@@ -225,6 +226,45 @@ BSB_API int bsb_set_source_framing(bsb_ctx* ctx, int source, int mode, int x, in
  * caller's call); (0, 0, W, H) when that call was not framed.  Synchronises the context's stream.  A frame outside the
  * last call returns 0 with a bsb_last_error() message. */
 BSB_API int bsb_get_framing(bsb_ctx* ctx, int frame, int rect[4]);
+/* Mask edge refinement: the full-size mask of a refined frame follows the edges of its own camera frame instead of the
+ * blocky, ~10-pixel-wide edge of blur(resize(small mask)) (lib/libbackscrub.cc:366-371): a joint bilateral upsample of the
+ * small mask guided by the camera luma (Kopf et al., SIGGRAPH 2007), which keeps hair and shoulders and stops the
+ * background bleeding around them.  It matters most where the matte is magnified or shown: BGRA output, auto-framing,
+ * held frames.  Strength sigma 0..255; 0 is off, the bytes of the unrefined mask.
+ * For a frame with sigma > 0, every pixel p = (x, y) inside roidim gets M'(p) below (outside it the mask stays 255).  s is
+ * the sw x sh out_roidim region of the small mask (ofinal, bsb_get_stage_u8 stage 2), L the camera luma as the composite
+ * reads the frame (BGR as given, YUYV / NV12 after the fused path's conversion): L = (4899 R + 9617 G + 1868 B + 8192) >> 14.
+ *   taps: fx = (float)((x - roi_x + 0.5) * scale - 0.5) (cv::resize's source position, scale = sw / roi_w as OpenCV
+ *     computes it, unclamped), s = floor(fx), a = lrintf((fx - s) * 2048); columns s-1 .. s+2 with spatial weights
+ *     max(0, 1024 - a), 3072 - a, 1024 + a, max(0, a - 1024) (a tent of radius 1.5 small pixels); rows alike.  A tap
+ *     outside 0..sw-1 / 0..sh-1 has weight 0.
+ *   guide(i, j) = L at (roi_x + ((2j + 1) roi_w) / (2 sw), roi_y + ((2i + 1) roi_h) / (2 sh)) (integer division): the
+ *     frame pixel nearest the centre of small pixel (i, j).
+ *   R[d] = max(1, floor(256 exp(-d^2 / (2 sigma^2)) + 0.5)), d = |L(p) - guide(i, j)| (bsb_mask_refine_weights).
+ *   w = ((wx * wy) >> 12) * R[d] per tap;  M'(p) = (sum w * s[i][j] + (sum w >> 1)) / sum w  (uint32; sum w >= 1024).
+ * A small mask that is uniform over a pixel's taps gives exactly that value.  Guidance: sigma ~ 8..16 (about the camera's
+ * noise plus a margin) separates person from background where their luma differs; sigma near 255 weighs every tap alike
+ * and degrades toward a plain tent upsample of the hard small mask, which is blockier than the default blur; where
+ * person and background have the same luma the refinement cannot find the edge.
+ * The refined mask is the mask: the stored W x H mask, the blend weight, BGRA alpha (255 - M').  Flip, resize, framing's
+ * crop and YUYV / NV12 follow from the composite as before; the mask is never flipped.  A frame with its filter off still
+ * stores its refined mask.  Held frames refine the held small mask against their own camera frame.  Unchanged: AUTO
+ * framing (it reads the small mask), bsb_get_stage_u8, rings, live backgrounds and the smoothers; fed calls
+ * (bsb_test_feed) refine like any call; bs_maskgen_process and the bsb_calcmask_* front end never refine.
+ * Host state only: each frame's strength reaches the device in a table with the call, so changing sigma replays the
+ * captured call (a call with some refined frame replays one of at most two graphs per buffer set).  A call with no refined
+ * frame runs exactly the kernels it ran before refinement existed.  A refined call needs the TMA or fast post kernel (frame
+ * width a multiple of 16, a small mask that is up-scaled to the ROI); otherwise the call returns 0 with a bsb_last_error()
+ * message.
+ * sigma: 0..255, default 0.  Out of range returns 0 with a bsb_last_error() message and changes nothing. */
+BSB_API int bsb_set_mask_refine(bsb_ctx* ctx, int sigma);
+/* One source's strength: -1 follows bsb_set_mask_refine (including later changes), else 0..255.  bsb_set_sources resets
+ * every source to -1; bsb_reset_source keeps it.  No bsb_set_sources yet, a source id out of range or a strength out of
+ * range returns 0 with a bsb_last_error() message and changes nothing. */
+BSB_API int bsb_set_source_mask_refine(bsb_ctx* ctx, int source, int sigma);
+/* The range weights R_sigma[d], d = 0..255, of strength sigma 1..255 into w[256] (host only).  Out of range or a null w
+ * returns 0 with a bsb_last_error() message. */
+BSB_API int bsb_mask_refine_weights(int sigma, int* w);
 /* Live backgrounds (the reference's `-b` takes any OpenCV source and blends its newest frame every loop iteration,
  * app/deepseg.cc:522-524,648-661): device images the caller already holds (decoded video surfaces, screen captures, a
  * second camera) are resized, blurred and blended inside the call, with no host copy and no launch outside it.
