@@ -85,6 +85,12 @@ def set_tuning(name: str, value: int) -> None:
         raise BackscrubError(lib().bsb_last_error().decode())
 
 
+def masked_gaussian_blur(src, mask, ksize: int, device: int = 0):
+    """The masked camera blur of bsb_set_blur_mode (include/backscrub_b200.h: bsb_masked_gaussian_blur): src 8UC3 blurred
+    with every tap weighted by mask 8UC1 and normalised by the blurred mask."""
+    return api.masked_gaussian_blur(lib(), src, mask, ksize, device)
+
+
 def mask_refine_weights(sigma: int):
     """The range weights R_sigma[d], d = 0..255, of mask refinement strength sigma 1..255 (include/backscrub_b200.h:
     bsb_mask_refine_weights), as an int64 array."""

@@ -41,6 +41,7 @@ SYMBOLS = [
     "bsb_set_mask_interval", "bsb_set_source_mask_interval",
     "bsb_set_framing", "bsb_set_framing_auto", "bsb_set_source_framing", "bsb_get_framing",
     "bsb_set_mask_refine", "bsb_set_source_mask_refine", "bsb_mask_refine_weights",
+    "bsb_set_blur_mode", "bsb_set_source_blur_mode", "bsb_masked_gaussian_blur",
     "bsb_test_feed_shape", "bsb_test_feed",
 ]
 
@@ -153,6 +154,9 @@ def bind(path: str) -> C.CDLL:
     L.bsb_set_mask_refine.argtypes = [C.c_void_p, C.c_int]
     L.bsb_set_source_mask_refine.argtypes = [C.c_void_p, C.c_int, C.c_int]
     L.bsb_mask_refine_weights.argtypes = [C.c_int, i32p]
+    L.bsb_set_blur_mode.argtypes = [C.c_void_p, C.c_int]
+    L.bsb_set_source_blur_mode.argtypes = [C.c_void_p, C.c_int, C.c_int]
+    L.bsb_masked_gaussian_blur.argtypes = [C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int]
     L.bsb_set_framing.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]
     L.bsb_set_framing_auto.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int]
     L.bsb_set_source_framing.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]

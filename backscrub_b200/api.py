@@ -126,6 +126,14 @@ class MaskGen:
         if not self._lib.bsb_set_mask_refine(self._h, int(sigma)):
             self._fail("bsb_set_mask_refine")
 
+    _BLUR_MODE = {"plain": 0, "masked": 1}
+
+    def set_blur_mode(self, mode: str):
+        """camera blur mode: "plain" (the default) blurs the whole camera frame, "masked" leaves the person out of the
+        background blur (include/backscrub_b200.h, bsb_set_blur_mode)"""
+        if not self._lib.bsb_set_blur_mode(self._h, self._BLUR_MODE.get(mode, -2)):
+            self._fail("bsb_set_blur_mode")
+
     _FRAMING = {"off": 0, "rect": 1, "auto": 2}
 
     def _framing_args(self, what, mode, rect):
@@ -416,6 +424,14 @@ class MaskGen:
         if not self._lib.bsb_set_source_mask_refine(self._h, int(source), -1 if sigma is None else int(sigma)):
             self._fail("bsb_set_source_mask_refine")
 
+    def set_source_blur_mode(self, source: int, mode=None):
+        """camera blur mode of one source: None = follow set_blur_mode, including later changes; otherwise "plain" or
+        "masked"
+        """
+        v = -1 if mode is None else self._BLUR_MODE.get(mode, -2)
+        if not self._lib.bsb_set_source_blur_mode(self._h, int(source), v):
+            self._fail("bsb_set_source_blur_mode")
+
     def set_source_output(self, source: int, out_size=None):
         """virtual-camera size of one source (cv::resize after the flip, app/deepseg.cc:677-679): out_size = (w, h), or
         None to follow set_output's size, including later changes.  The mask stays W x H."""
@@ -609,6 +625,19 @@ def gaussian_blur(lib, src, ksize, device=0):
     src = np.ascontiguousarray(src, np.uint8)
     out = np.empty_like(src)
     if not lib.bsb_gaussian_blur(device, _ptr(src), _ptr(out), src.shape[1], src.shape[0], int(ksize)):
+        raise BackscrubError(lib.bsb_last_error().decode())
+    return out
+
+
+def masked_gaussian_blur(lib, src, mask, ksize, device=0):
+    """the masked camera blur of bsb_set_blur_mode: src 8UC3 blurred with every tap weighted by mask 8UC1
+    (bsb_masked_gaussian_blur)"""
+    src = np.ascontiguousarray(src, np.uint8)
+    mask = np.ascontiguousarray(mask, np.uint8)
+    if mask.shape != src.shape[:2]:
+        raise ValueError("mask must be H x W of src")
+    out = np.empty_like(src)
+    if not lib.bsb_masked_gaussian_blur(device, _ptr(src), _ptr(mask), _ptr(out), src.shape[1], src.shape[0], int(ksize)):
         raise BackscrubError(lib.bsb_last_error().decode())
     return out
 

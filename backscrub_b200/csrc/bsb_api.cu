@@ -440,6 +440,20 @@ int bsb_set_source_mask_refine(bsb_ctx* ctx, int source, int sigma) {
   return 1;
 }
 
+int bsb_set_blur_mode(bsb_ctx* ctx, int mode) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_blur_mode(mode, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
+int bsb_set_source_blur_mode(bsb_ctx* ctx, int source, int mode) {
+  if (!check_ctx(ctx)) return 0;
+  std::string err;
+  if (!ctx->eng->set_source_blur_mode(source, mode, &err)) { report(&ctx->cb, "error: " + err); return 0; }
+  return 1;
+}
+
 int bsb_get_framing(bsb_ctx* ctx, int frame, int rect[4]) {
   if (!check_ctx(ctx)) return 0;
   if (!rect) { report(&ctx->cb, "error: rect is null"); return 0; }
@@ -769,6 +783,25 @@ int bsb_gaussian_blur(int device, const uint8_t* src, uint8_t* dst, int width, i
   cudaMemcpy(a.p, src, nb, cudaMemcpyHostToDevice);
   if (!bsb::launch_gauss_blur(nullptr, 1, a.u8(), (size_t)width * 3, nb, static_cast<uint16_t*>(tmp.p), o.u8(), (size_t)width * 3, nb, width,
                               height, t)) {
+    g_last_error = "could not allocate the Gaussian tap tables";
+    return 0;
+  }
+  if (!stage_end()) return 0;
+  cudaMemcpy(dst, o.p, nb, cudaMemcpyDeviceToHost);
+  return 1;
+}
+
+int bsb_masked_gaussian_blur(int device, const uint8_t* src, const uint8_t* mask, uint8_t* dst, int width, int height, int ksize) {
+  if (!src || !mask || !dst || width <= 0 || height <= 0) { g_last_error = "invalid argument"; return 0; }
+  if (ksize < 1 || !(ksize & 1) || ksize > 255) { g_last_error = "strength value must be odd (1..255)"; return 0; }
+  if (!stage_begin(device)) return 0;
+  const size_t npix = (size_t)width * height, nb = npix * 3;
+  DevBuf a, m, o, tmp;
+  if (!a.alloc(nb) || !m.alloc(npix) || !o.alloc(nb) || !tmp.alloc(npix * sizeof(uint4))) { g_last_error = "cudaMalloc failed"; return 0; }
+  cudaMemcpy(a.p, src, nb, cudaMemcpyHostToDevice);
+  cudaMemcpy(m.p, mask, npix, cudaMemcpyHostToDevice);
+  if (!bsb::launch_masked_gauss(nullptr, 1, a.u8(), (size_t)width * 3, nb, m.u8(), npix, nullptr, ksize, (unsigned)bsb::gauss_class(ksize),
+                                static_cast<uint4*>(tmp.p), o.u8(), (size_t)width * 3, nb, width, height)) {
     g_last_error = "could not allocate the Gaussian tap tables";
     return 0;
   }

@@ -963,7 +963,7 @@ Engine::~Engine() {
   free_sources();
   for (void* p : {(void*)d_src_tab_, (void*)d_src_raw_, tab_src_.blob, (void*)d_pass_all_, (void*)d_live_tab_, (void*)d_live_stage_, (void*)d_seg_tab_,
                   (void*)d_frame_tab_, (void*)d_crop_, (void*)d_frame_box_, (void*)d_frame_counter_, (void*)d_frame_state_,
-                  (void*)d_refine_, (void*)d_refine_taps_, (void*)d_tile_geo_r_})
+                  (void*)d_refine_, (void*)d_refine_taps_, (void*)d_tile_geo_r_, (void*)d_mblur_mask_, (void*)d_mgauss_tmp_})
     if (p) cudaFree(p);
   for (LiveSize& l : live_sizes_) if (l.tab.blob) cudaFree(l.tab.blob);
   if (h_mask_) cudaFreeHost(h_mask_);
@@ -1314,6 +1314,20 @@ bool Engine::set_source_mask_refine(int source, int sigma, std::string* err) {
   return true;
 }
 
+bool Engine::set_blur_mode(int mode, std::string* err) {
+  if (mode != BLUR_PLAIN && mode != BLUR_MASKED) { *err = "blur mode must be BSB_BLUR_PLAIN (0) or BSB_BLUR_MASKED (1)"; return false; }
+  blur_mode_ = mode;
+  return true;
+}
+
+bool Engine::set_source_blur_mode(int source, int mode, std::string* err) {
+  if (!n_sources_) { *err = "no sources: call bsb_set_sources first"; return false; }
+  if (source < 0 || source >= n_sources_) { *err = "source id out of range"; return false; }
+  if (mode < -1 || mode > BLUR_MASKED) { *err = "source blur mode must be -1 (follow the context), BSB_BLUR_PLAIN (0) or BSB_BLUR_MASKED (1)"; return false; }
+  src_blur_mode_[source] = (signed char)mode;
+  return true;
+}
+
 bool Engine::set_framing(int mode, int x, int y, int w, int h, std::string* err) {
   if (!check_framing(mode, x, y, w, h, W_, H_, false, err)) return false;
   framing_ = Framing{mode, {x, y, w, h}};
@@ -1432,6 +1446,13 @@ bool Engine::enqueue_post(const Call& c, const Plan& p) {
   // app/deepseg.cc:652-658: no background source => the background is the blurred camera frame itself (sources: frame b
   // at its own strength into the bank's camera-blur slot b, with the slot's YUYV / NV12; the camera frame is read in
   // its wire format when the post kernel reads it so)
+  // Masked frames first get their masks M: the post kernel's own, from a mask-only launch into d_mblur_mask_
+  if (p.mgclass) {
+    PostArgs m = a;
+    m.out = nullptr; m.yuyv = nullptr; m.nv12 = nullptr; m.bgra = nullptr; m.flip = nullptr;
+    m.mask = d_mblur_mask_; m.mask_stride = mblur_mstride();
+    if (!launch_post(stream_, m)) return false;
+  }
   if (p.mode == CALL_SOURCES_CAMBLUR && blends(c, p)) {
     // the slots' cached video format is the one the post kernel copies: NV12 when it reads the NV12 frames in place, else
     // YUYV (also for an NV12 call that falls back to BGR frames)
@@ -1440,8 +1461,13 @@ bool Engine::enqueue_post(const Call& c, const Plan& p) {
     if (p.native) cam = GaussSrc{c.in, c.pitch, c.stride, c.uv, c.fmt};
     uint8_t* yv = (!p.all_blur && !nv12_in && !(W_ & 1)) ? d_bank_yuyv_ : nullptr;
     uint8_t* nv = (!p.all_blur && nv12_in) ? d_bank_nv12_ : nullptr;
-    launch_gauss_frames(stream_, n, cam, d_src_tab_ + 2 * (size_t)max_batch_, p.gclass, const_cast<uint8_t*>(a.frames), d_gauss_tmp_,
-                        d_bank_, yv, nv, W_, H_);
+    const size_t mb = (size_t)max_batch_;
+    const MaskedFrames mf{d_src_tab_ + SRC_TAB_MASKED * mb, d_src_tab_ + 2 * mb, p.mgclass, d_mblur_mask_, mblur_mstride(), d_mgauss_tmp_};
+    launch_gauss_frames(stream_, n, cam, d_src_tab_ + (p.mgclass ? SRC_TAB_PLAIN : 2) * mb, p.gclass, const_cast<uint8_t*>(a.frames), d_gauss_tmp_,
+                        d_bank_, yv, nv, W_, H_, p.mgclass ? &mf : nullptr);
+  } else if (p.mgclass) {
+    launch_masked_gauss(stream_, n, a.frames, a.frame_pitch, a.frame_stride, d_mblur_mask_, mblur_mstride(), nullptr, bgblur_k_, p.mgclass,
+                        d_mgauss_tmp_, d_bg_frames_, (size_t)W_ * 3, fbytes, W_, H_);
   } else if (p.mode == CALL_PLAIN && !has_bg_ && bgblur_k_ && blends(c, p) && !p.passed && !p.live)
     launch_gauss_blur(stream_, n, a.frames, a.frame_pitch, a.frame_stride, d_gauss_tmp_, d_bg_frames_, (size_t)W_ * 3, fbytes, W_, H_, taps_);
   if (p.live) enqueue_live(c, p);
@@ -1611,6 +1637,8 @@ bool Engine::run(const Call& c, std::string* err) {
     ltab.resize(p.live == 2 ? (size_t)n : 1);
     for (size_t b = 0; b < ltab.size(); ++b) ltab[b] = live_desc(live_, live_.p + ((size_t)c.frame0 + b) * live_.stride, bgblur_k_ != 0);
   }
+  // masked camera blur: a plain call whose background is its blurred camera frame, in the context's mode
+  if (!c.ids && blur_mode_ == BLUR_MASKED && !has_bg_ && bgblur_k_ && blend && !p.passed && !p.live) p.mgclass = (unsigned)gauss_class(bgblur_k_);
   if (c.ids) {
     if (has_bg_ && bg_count_ > 1) { *err = "sources calls need a still context background (animate a source with bsb_set_source_background)"; return false; }
     // frame b: state of source ids[b]; background (source_bg) = the context slot, the source's slot, or its camera frame
@@ -1642,7 +1670,13 @@ bool Engine::run(const Call& c, std::string* err) {
         ltab[b] = live_desc(lv, lv.p, k != 0);
       } else {
         if (from == SRC_FROM_CAMBLUR) slot = b;
-        if (from == SRC_FROM_CAMBLUR && !off && blend) { tab[2 * (size_t)max_batch_ + b] = k; p.gclass |= (unsigned)gauss_class(k); ++n_blur; }
+        if (from == SRC_FROM_CAMBLUR && !off && blend) {
+          tab[2 * (size_t)max_batch_ + b] = k;
+          ++n_blur;
+          const int mode = src_blur_mode_[id] < 0 ? blur_mode_ : src_blur_mode_[id];
+          if (mode == BLUR_MASKED) { tab[SRC_TAB_MASKED * (size_t)max_batch_ + b] = k; p.mgclass |= (unsigned)gauss_class(k); }
+          else { tab[SRC_TAB_PLAIN * (size_t)max_batch_ + b] = k; p.gclass |= (unsigned)gauss_class(k); }
+        }
       }
       tab[(size_t)max_batch_ + b] = (int)slot;
       const int fl = src_flip_[id] < 0 ? ctx_flip : src_flip_[id];
@@ -1654,7 +1688,7 @@ bool Engine::run(const Call& c, std::string* err) {
       p.resized = p.resized || ow != W_ || oh != H_;
     }
     if (!check_source_outputs(c, err)) return false;
-    p.mode = p.gclass ? CALL_SOURCES_CAMBLUR : CALL_SOURCES;
+    p.mode = (p.gclass | p.mgclass) ? CALL_SOURCES_CAMBLUR : CALL_SOURCES;
     p.all_blur = n_blur == n;
   }
   if (c.fmt != IN_BGR && (W_ & 1)) { *err = "YUYV ingest needs an even width"; return false; }
@@ -1695,6 +1729,12 @@ bool Engine::run(const Call& c, std::string* err) {
     if (!refine_w_ && !(refine_w_ = refine_tables())) { *err = "could not allocate the mask refinement tables"; return false; }
     // outside the graph, before its launch, like the source table
     CUDA_OK(cudaMemcpyAsync(d_refine_, rtab.data(), rtab.size() * sizeof(int), cudaMemcpyHostToDevice, stream_));
+  }
+  if (p.mgclass) {
+    // grown once (dropping the graphs), on the first call with masked frames that needs them
+    if (!ensure((void**)&d_mblur_mask_, &mblur_mask_cap_, (size_t)max_batch_ * mblur_mstride(), err)) return false;
+    if ((p.mgclass & GAUSS_SEPARABLE) && !ensure((void**)&d_mgauss_tmp_, &mgauss_tmp_cap_, (size_t)max_batch_ * W_ * H_ * sizeof(uint4), err))
+      return false;
   }
   if (c.ids) {
     if (((p.gclass | p.live_gclass) & GAUSS_SEPARABLE) && !ensure_gauss_tmp(err)) return false;
@@ -2055,6 +2095,7 @@ void Engine::free_sources() {
   src_size_.clear();
   src_interval_.clear();
   src_refine_.clear();
+  src_blur_mode_.clear();
   src_frames_.clear();
   src_framing_.clear();
   src_jump_.clear();
@@ -2108,6 +2149,7 @@ bool Engine::set_sources(int n_sources, std::string* err) {
   src_live_.assign((size_t)n_sources, Live{});
   src_interval_.assign((size_t)n_sources, -1);
   src_refine_.assign((size_t)n_sources, -1);
+  src_blur_mode_.assign((size_t)n_sources, -1);
   src_frames_.assign((size_t)n_sources, 0);
   src_framing_.assign((size_t)n_sources, Framing{});
   src_jump_.assign((size_t)n_sources, 1);

@@ -154,6 +154,11 @@ class Engine {
   bool set_mask_refine(int sigma, std::string* err);
   // one source's strength: -1 follows set_mask_refine, else 0..255
   bool set_source_mask_refine(int source, int sigma, std::string* err);
+  // Camera blur mode (include/backscrub_b200.h, bsb_set_blur_mode): BLUR_PLAIN or BLUR_MASKED.  Host state only: each
+  // frame's mode reaches the device as table data with the call.
+  bool set_blur_mode(int mode, std::string* err);
+  // one source's mode: -1 follows set_blur_mode, else its own
+  bool set_source_blur_mode(int source, int mode, std::string* err);
 
   // Independent sources (camera streams) batched one frame each into a call.  set_sources allocates n zeroed smoother
   // states and the per-source background bank (again: everything reallocated and zeroed, graphs dropped).
@@ -278,6 +283,8 @@ class Engine {
     bool framed = false;             // some frame is framed (RECT or AUTO): k_framing runs and every frame goes through the
                                      // cropping tail from unflipped staging
     bool refined = false;            // some frame's mask is refined: the post kernel takes the strength table d_refine_
+    unsigned mgclass = 0;            // the masked Gaussian launch classes of the call's masked camera-blur frames (0: none, and
+                                     // the call runs the launches it runs in plain mode)
   };
   // the call blends a composite: it has a video output, or a BGR composite output.  A call that does not reads no
   // background and blurs nothing.
@@ -438,7 +445,8 @@ class Engine {
   // of frame b (0 = not blurred, or no live background) | the segment rows gather and cidx (calls with held frames, else
   // unused), written before each launch
   int* d_src_tab_ = nullptr;
-  enum { SRC_TAB_ROWS = 9, SRC_TAB_SEG = 7 };
+  // | with masked frames (Plan::mgclass): the strength of frame b when it blurs in plain mode | when it blurs masked
+  enum { SRC_TAB_ROWS = 11, SRC_TAB_SEG = 7, SRC_TAB_PLAIN = 9, SRC_TAB_MASKED = 10 };
   // ---- mask interval ----
   int mask_interval_ = 1;
   long long plain_frames_ = 0;       // frames of plain calls since creation / reset_state: frame c is segmented iff c % k == 0
@@ -463,6 +471,13 @@ class Engine {
   unsigned* d_refine_taps_ = nullptr;   // refine_tap of each ROI column [roi_w] | row [roi_h]
   int2* d_tile_geo_r_ = nullptr;     // the refinement's patch geometry, laid out as d_tile_geo_
   const unsigned short* refine_w_ = nullptr;   // the device's range weights (refine_tables), taken before the first refined call
+  // ---- camera blur mode ----
+  int blur_mode_ = 0;                // the context's (plain calls, and sources that follow it)
+  std::vector<signed char> src_blur_mode_;   // per source: -1 = blur_mode_, else its own
+  uint8_t* d_mblur_mask_ = nullptr;  // [max_batch][mblur_mstride()] the masks of a call with masked frames, for the masked Gaussian
+  uint4* d_mgauss_tmp_ = nullptr;    // [max_batch][H][W] row sums of the masked row / column Gaussian
+  size_t mblur_mask_cap_ = 0, mgauss_tmp_cap_ = 0;
+  size_t mblur_mstride() const { return ((size_t)W_ * H_ + 15) & ~(size_t)15; }
   FrameCrop* d_crop_ = nullptr;      // [max_batch] the crop of each frame of the last framed call (the tail reads it)
   int* d_frame_box_ = nullptr;       // [max_batch][4] targets of a plain call (k_framing scratch)
   unsigned* d_frame_counter_ = nullptr;
@@ -541,23 +556,24 @@ class Engine {
   // (which frame has which size is table data too), the output format, whether frames blend live backgrounds, with
   // the Gaussian classes they add (their images, sizes and strengths within the classes are the live table's data), and the
   // CNN batch of a call with held frames (which frames are segmented is the segment rows' data), whether the call is
-  // framed (modes, rectangles and crops are table data), and whether it refines a mask (the strengths are table data).  The
-  // rest of the plan is
+  // framed (modes, rectangles and crops are table data), whether it refines a mask (the strengths are table data), and the
+  // masked Gaussian classes (which frames blur masked is table data).  The rest of the plan is
   // decided from these.
   struct GraphKey {
     int n, fmt; const void* in; size_t pitch, uv, stride;
     const void* out; const void* video; const void* mask; size_t ostride, vstride, mstride;
     int mode; unsigned gclass; bool all_blur, flipped, resized, passed; long out_px_max; bool bgra; int live; unsigned live_gclass;
     bool framed, refined;
+    unsigned mgclass;
     GraphKey(const Call& c, const Plan& p, long px_max)
         : n(c.n), fmt(c.fmt), in(c.in), pitch(c.pitch), uv(c.uv), stride(c.stride), out(c.out), video(c.video), mask(c.mask),
           ostride(c.out ? c.out_stride : 0), vstride(c.video ? c.video_stride : 0), mstride(c.mask ? c.mask_stride : 0),
           mode(p.mode), gclass(p.gclass), all_blur(p.all_blur), flipped(p.flipped), resized(p.resized), passed(p.passed),
-          out_px_max(px_max), bgra(p.bgra), live(p.live), live_gclass(p.live_gclass), framed(p.framed), refined(p.refined), seg(p.m) {}
+          out_px_max(px_max), bgra(p.bgra), live(p.live), live_gclass(p.live_gclass), framed(p.framed), refined(p.refined), mgclass(p.mgclass), seg(p.m) {}
     int seg;                         // the CNN batch m (n: every frame segmented, the parent's launches)
     auto tie() const {
       return std::tie(n, fmt, in, pitch, uv, stride, out, video, mask, ostride, vstride, mstride, mode, gclass, all_blur, flipped, resized,
-                      passed, out_px_max, bgra, live, live_gclass, framed, refined, seg);
+                      passed, out_px_max, bgra, live, live_gclass, framed, refined, mgclass, seg);
     }
     bool operator<(const GraphKey& r) const { return tie() < r.tie(); }
   };

@@ -321,6 +321,8 @@ bool launch_gauss_blur(cudaStream_t s, int n, const uint8_t* src, size_t spitch,
                        uint8_t* dst, size_t dpitch, size_t dstride, int W, int H, const GaussTaps& g);
 // Launch classes of the Gaussian: the fused tile kernel (strengths 3..31) or the row / column pair (1, 33..255); 0 = off
 enum : unsigned { GAUSS_FUSED = 1, GAUSS_SEPARABLE = 2 };
+// camera blur modes (bsb_set_blur_mode): the reference's Gaussian of the whole camera frame, or the masked Gaussian
+enum { BLUR_PLAIN = 0, BLUR_MASKED = 1 };
 BSB_HD int gauss_class(int k) { return k == 0 ? 0 : (k >= 3 && k <= 31) ? (int)GAUSS_FUSED : (int)GAUSS_SEPARABLE; }
 // camera frames in their wire format: YUYV or NV12 (InFmt), `pitch` bytes per row, `stride` per frame, NV12's UV plane
 // at byte `uv`
@@ -332,8 +334,19 @@ bool gauss_tables_ready();
 // the call may need, so a captured launch replays for any strengths within them.  cam.p non-null: `frames` is first
 // filled, for the blurred frames only, from the camera frames.  dst_yuyv / dst_nv12 (may be null): the blurred frames'
 // YUYV / NV12 (W*H*2 / W*H*3/2 bytes per frame; W even, NV12 also H even).
+// Masked camera blur (bsb_set_blur_mode): frame b of src blurred at strength ks[b] (k_all when ks is null; 0 = not
+// blurred) with every tap weighted by frame b of `mask` (W x H bytes, mstride apart) and normalised by the blurred mask,
+// into frame b of dst (and its YUYV / NV12 for the fused class, as launch_gauss_frames).  tmp: n*H*W row sums of the row /
+// column class.  False if the per-device tap tables could not be allocated.
+bool launch_masked_gauss(cudaStream_t s, int n, const uint8_t* src, size_t spitch, size_t sstride, const uint8_t* mask, size_t mstride,
+                         const int* ks, int k_all, unsigned classes, uint4* tmp, uint8_t* dst, size_t dpitch, size_t dstride, int W, int H,
+                         uint8_t* yuyv = nullptr, uint8_t* nv12 = nullptr);
+// the masked frames of a sources call: ks (DEVICE [n]) their strengths, ks_all every blurred frame's (plain or masked),
+// classes the masked launch classes the call may need
+struct MaskedFrames { const int* ks; const int* ks_all; unsigned classes; const uint8_t* mask; size_t mstride; uint4* tmp; };
+// mf non-null: ks names the frames of the plain Gaussian only, and the frames of mf are blurred by launch_masked_gauss
 bool launch_gauss_frames(cudaStream_t s, int n, const GaussSrc& cam, const int* ks, unsigned classes, uint8_t* frames, uint16_t* tmp,
-                         uint8_t* dst, uint8_t* dst_yuyv, uint8_t* dst_nv12, int W, int H);
+                         uint8_t* dst, uint8_t* dst_yuyv, uint8_t* dst_nv12, int W, int H, const MaskedFrames* mf = nullptr);
 // app/deepseg.cc:667-673: cv::flip on n packed frames
 void launch_flip_u8c3(cudaStream_t s, int n, const uint8_t* src, size_t sstride, uint8_t* dst, size_t dstride, int W, int H, bool flip_h, bool flip_v);
 // app/deepseg.cc:667-681 in one launch, the tail of a call whose frames are mirrored or resized outside the post kernel:

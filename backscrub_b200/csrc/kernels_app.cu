@@ -188,6 +188,28 @@ BSB_D void gauss_fused_bc(uint8_t* P, uint16_t* Ht, const GaussFast& g, int rows
   }
 }
 
+// Stage D's YUYV / NV12 of a tw x th output tile O (GF_TW * 3 bytes per row) at (x0, y0) of frame b: yuyv / nv12 (may
+// be null; W even, NV12 also H even) are [n] W*H*2 / W*H*3/2-byte frames
+BSB_D void gauss_tile_video(const uint8_t* O, int tw, int th, int x0, int y0, int W, int H, int b, uint8_t* yuyv, uint8_t* nv12, int tid) {
+  const int np = tw / 2;                                        // pixel pairs per tile row (x0 and W are even)
+  const size_t npix = (size_t)W * H;
+  if (nv12) {                                                   // tile rows start even, th is even (H even)
+    uint8_t* f = nv12 + (size_t)b * (npix * 3 / 2);
+    for (int i = tid; i < (th / 2) * np; i += 256) {
+      const int rp = i / np, j = i - rp * np;
+      const unsigned w0 = yuyv_pair_word(O + (2 * rp) * (GF_TW * 3) + 6 * j), w1 = yuyv_pair_word(O + (2 * rp + 1) * (GF_TW * 3) + 6 * j);
+      const int y = y0 + 2 * rp, x = x0 + 2 * j;
+      nv12_block(w0, w1, f + (size_t)y * W + x, W, f + npix + (size_t)(y >> 1) * W + x);
+    }
+  } else if (yuyv) {
+    unsigned* f = reinterpret_cast<unsigned*>(yuyv + (size_t)b * npix * 2);
+    for (int i = tid; i < th * np; i += 256) {
+      const int row = i / np, j = i - row * np;
+      f[((size_t)(y0 + row) * W + x0) / 2 + j] = yuyv_pair_word(O + row * (GF_TW * 3) + 6 * j);
+    }
+  }
+}
+
 // yuyv / nv12 (may be null; W even, NV12 also H even): [n] W*H*2 / W*H*3/2-byte frames that receive the blurred frame's
 // YUYV / NV12, written from the output tile in stage D
 __global__ void __launch_bounds__(256) k_gauss_fused(const uint8_t* src, size_t spitch, size_t sstride, uint8_t* dst, size_t dpitch,
@@ -260,23 +282,7 @@ __global__ void __launch_bounds__(256) k_gauss_fused(const uint8_t* src, size_t 
       out[(size_t)row * dpitch + l] = O[row * (GF_TW * 3) + l];
     }
   }
-  const int np = tw / 2;                                        // pixel pairs per tile row (x0 and W are even)
-  const size_t npix = (size_t)W * H;
-  if (nv12) {                                                   // tile rows start even, th is even (H even)
-    uint8_t* f = nv12 + (size_t)b * (npix * 3 / 2);
-    for (int i = tid; i < (th / 2) * np; i += 256) {
-      const int rp = i / np, j = i - rp * np;
-      const unsigned w0 = yuyv_pair_word(O + (2 * rp) * (GF_TW * 3) + 6 * j), w1 = yuyv_pair_word(O + (2 * rp + 1) * (GF_TW * 3) + 6 * j);
-      const int y = y0 + 2 * rp, x = x0 + 2 * j;
-      nv12_block(w0, w1, f + (size_t)y * W + x, W, f + npix + (size_t)(y >> 1) * W + x);
-    }
-  } else if (yuyv) {
-    unsigned* f = reinterpret_cast<unsigned*>(yuyv + (size_t)b * npix * 2);
-    for (int i = tid; i < th * np; i += 256) {
-      const int row = i / np, j = i - row * np;
-      f[((size_t)(y0 + row) * W + x0) / 2 + j] = yuyv_pair_word(O + row * (GF_TW * 3) + 6 * j);
-    }
-  }
+  gauss_tile_video(O, tw, th, x0, y0, W, H, b, yuyv, nv12, tid);
 }
 
 // The same YUYV / NV12 for the frames of the row / column class (ks[b] in it), from the blurred BGR frames.  One
@@ -378,19 +384,193 @@ bool launch_gauss_blur(cudaStream_t s, int n, const uint8_t* src, size_t spitch,
   return launch_gauss_classes(s, n, src, spitch, sstride, nullptr, g.k, (unsigned)gauss_class(g.k), tmp, dst, dpitch, dstride, W, H);
 }
 
+// ---------------------------------------------------------------------------
+// Masked camera blur (include/backscrub_b200.h, bsb_set_blur_mode): the Gaussian of the camera frame C weighted by the
+// frame's W x H mask M, normalised by the Gaussian of M:
+//   rows: h_c = sum_j q[j]*M*C_c   (< 2^24)      g = sum_j q[j]*M   (< 2^16)
+//   cols: N_c = sum_i q[i]*h_c     (< 2^32)      D = sum_i q[i]*g   (< 2^24)
+//   B_c = D > 0 ? (N_c + (D >> 1)) / D : C_c
+// All sums are exact integers, so tap order is free.  The same two launch classes as the plain Gaussian: a fused tile
+// kernel for 3..31, a row / column pair for 1 and 33..255; mask: [n] frames of W x H bytes, mstride apart.
+// ---------------------------------------------------------------------------
+BSB_D uint8_t masked_div(unsigned num, unsigned den, uint8_t c) { return den ? (uint8_t)((num + (den >> 1)) / den) : c; }
+
+// Fused class: one block = 64 x 32 output pixels (dynamic shared memory, mgauss_fused_smem):
+//   A  the reflected (32+2r) x (64+2r) patch as four 16-bit planes M*B, M*G, M*R, M,
+//   B  their row sums (32-bit, the row's 64 outputs contiguous),
+//   C  column sums and the division into the interleaved output tile (over plane 0, which B no longer reads),
+//   D  write out, and the tile's YUYV / NV12 (stage D of k_gauss_fused).
+constexpr int MG_PW = GF_TW + 2 * GF_MAXR + 2, MG_PLANE = GF_RM * MG_PW, MG_HPLANE = GF_RM * GF_TW;
+constexpr size_t MG_SMEM = 4 * MG_PLANE * sizeof(uint16_t) + 4 * MG_HPLANE * sizeof(unsigned);
+
+__global__ void __launch_bounds__(256) k_mgauss_fused(const uint8_t* src, size_t spitch, size_t sstride, const uint8_t* mask, size_t mstride,
+                                                      uint8_t* dst, size_t dpitch, size_t dstride, int W, int H, const GaussTables* T,
+                                                      int k_all, const int* ks, uint8_t* yuyv, uint8_t* nv12) {
+  BSB_DYN_SMEM(smem_raw);
+  __shared__ unsigned q[2 * GF_MAXR + 1];
+  uint16_t* P = reinterpret_cast<uint16_t*>(smem_raw);
+  unsigned* Hs = reinterpret_cast<unsigned*>(smem_raw + 4 * MG_PLANE * sizeof(uint16_t));
+  const int tid = threadIdx.x;
+  const int x0 = blockIdx.x * GF_TW, y0 = blockIdx.y * GF_TH, b = blockIdx.z;
+  const int k = ks ? ks[b] : k_all;
+  if (gauss_class(k) != GAUSS_FUSED) return;
+  const int r = k >> 1;
+  const int tw = min(GF_TW, W - x0), th = min(GF_TH, H - y0);
+  const int rows = GF_TH + 2 * r, cols = GF_TW + 2 * r;
+  const uint8_t* frame = src + (size_t)b * sstride;
+  const uint8_t* mf = mask + (size_t)b * mstride;
+  if (tid < k) q[tid] = T->taps[(k - 1) >> 1].q[tid];
+  // ---- A ----
+  for (int i = tid; i < rows * cols; i += 256) {
+    const int row = i / cols, col = i - row * cols;
+    const int sy = bsb_reflect101(y0 + row - r, H), sx = bsb_reflect101(x0 + col - r, W);
+    const unsigned m = mf[(size_t)sy * W + sx];
+    const uint8_t* sp = frame + (size_t)sy * spitch + (size_t)sx * 3;
+    uint16_t* pp = P + row * MG_PW + col;
+    pp[0] = (uint16_t)(m * sp[0]); pp[MG_PLANE] = (uint16_t)(m * sp[1]); pp[2 * MG_PLANE] = (uint16_t)(m * sp[2]); pp[3 * MG_PLANE] = (uint16_t)m;
+  }
+  __syncthreads();
+  // ---- B ----
+  for (int i = tid; i < 4 * rows * GF_TW; i += 256) {
+    const int p = i / (rows * GF_TW), rem = i - p * (rows * GF_TW), row = rem / GF_TW, x = rem - row * GF_TW;
+    const uint16_t* pp = P + p * MG_PLANE + row * MG_PW + x;
+    unsigned acc = 0;
+    for (int j = 0; j < k; ++j) acc += q[j] * pp[j];
+    Hs[p * MG_HPLANE + row * GF_TW + x] = acc;
+  }
+  __syncthreads();
+  // ---- C ----
+  uint8_t* O = reinterpret_cast<uint8_t*>(P);                   // [GF_TH][GF_TW * 3]
+  for (int i = tid; i < th * GF_TW; i += 256) {
+    const int y = i / GF_TW, x = i - y * GF_TW;
+    if (x >= tw) continue;
+    const unsigned* hp = Hs + y * GF_TW + x;
+    unsigned n0 = 0, n1 = 0, n2 = 0, d = 0;
+    for (int j = 0; j < k; ++j) {
+      const unsigned w = q[j];
+      n0 += w * hp[0]; n1 += w * hp[MG_HPLANE]; n2 += w * hp[2 * MG_HPLANE]; d += w * hp[3 * MG_HPLANE];
+      hp += GF_TW;
+    }
+    const uint8_t* cp = frame + (size_t)(y0 + y) * spitch + (size_t)(x0 + x) * 3;
+    uint8_t* op = O + y * (GF_TW * 3) + x * 3;
+    op[0] = masked_div(n0, d, cp[0]); op[1] = masked_div(n1, d, cp[1]); op[2] = masked_div(n2, d, cp[2]);
+  }
+  __syncthreads();
+  // ---- D ----
+  uint8_t* out = dst + (size_t)b * dstride + (size_t)y0 * dpitch + (size_t)x0 * 3;
+  for (int i = tid; i < th * tw * 3; i += 256) {
+    const int row = i / (tw * 3), l = i - row * (tw * 3);
+    out[(size_t)row * dpitch + l] = O[row * (GF_TW * 3) + l];
+  }
+  gauss_tile_video(O, tw, th, x0, y0, W, H, b, yuyv, nv12, tid);
+}
+
+// Row / column class.  Row pass: one block = 256 pixels of one row; tmp receives (h_0, h_1, h_2, g) per pixel.
+__global__ void __launch_bounds__(256) k_mgauss_rows(const uint8_t* src, size_t pitch, size_t frame_stride, const uint8_t* mask, size_t mstride,
+                                                     uint4* tmp, int W, int H, const GaussTables* T, int k_all, const int* ks) {
+  __shared__ uint2 s[GAUSS_TW + 2 * 127];                       // M*B | M*G << 16, M*R | M << 16
+  __shared__ unsigned q[256];
+  const int x0 = blockIdx.x * GAUSS_TW, y = blockIdx.y, b = blockIdx.z;
+  const int k = ks ? ks[b] : k_all;
+  if (gauss_class(k) != GAUSS_SEPARABLE) return;
+  const int r = k >> 1;
+  const int tw = min(GAUSS_TW, W - x0);
+  const uint8_t* row = src + (size_t)b * frame_stride + (size_t)y * pitch;
+  const uint8_t* mrow = mask + (size_t)b * mstride + (size_t)y * W;
+  for (int j = threadIdx.x; j < k; j += blockDim.x) q[j] = T->taps[(k - 1) >> 1].q[j];
+  for (int i = threadIdx.x; i < tw + 2 * r; i += blockDim.x) {
+    const int sx = bsb_reflect101(x0 + i - r, W);
+    const unsigned m = mrow[sx];
+    s[i] = make_uint2(m * row[3 * sx] | (m * row[3 * sx + 1]) << 16, m * row[3 * sx + 2] | m << 16);
+  }
+  __syncthreads();
+  const int x = threadIdx.x;
+  if (x >= tw) return;
+  unsigned h0 = 0, h1 = 0, h2 = 0, g = 0;
+  for (int j = 0; j < k; ++j) {
+    const uint2 v = s[x + j];
+    const unsigned w = q[j];
+    h0 += w * (v.x & 0xffffu); h1 += w * (v.x >> 16); h2 += w * (v.y & 0xffffu); g += w * (v.y >> 16);
+  }
+  tmp[((size_t)b * H + y) * W + x0 + x] = make_uint4(h0, h1, h2, g);
+}
+
+// Column pass: one block = 64 columns x 32 rows, a thread walks 8 rows of one column; the row sums come through L1.
+constexpr int MGC_W = 64, MGC_H = 32;
+
+__global__ void __launch_bounds__(256) k_mgauss_cols(const uint4* tmp, const uint8_t* src, size_t spitch, size_t sstride, uint8_t* dst,
+                                                     size_t dpitch, size_t dstride, int W, int H, const GaussTables* T, int k_all, const int* ks) {
+  __shared__ unsigned q[256];
+  const int b = blockIdx.z;
+  const int k = ks ? ks[b] : k_all;
+  if (gauss_class(k) != GAUSS_SEPARABLE) return;
+  const int r = k >> 1;
+  for (int j = threadIdx.x; j < k; j += blockDim.x) q[j] = T->taps[(k - 1) >> 1].q[j];
+  __syncthreads();
+  const int x = blockIdx.x * MGC_W + threadIdx.x % MGC_W;
+  if (x >= W) return;
+  const uint4* t = tmp + (size_t)b * H * W + x;
+  const int ya = blockIdx.y * MGC_H + (threadIdx.x / MGC_W) * (MGC_H / 4);
+  for (int y = ya; y < min(ya + MGC_H / 4, H); ++y) {
+    unsigned n0 = 0, n1 = 0, n2 = 0, d = 0;
+    for (int j = 0; j < k; ++j) {
+      const uint4 v = __ldg(t + (size_t)bsb_reflect101(y + j - r, H) * W);
+      const unsigned w = q[j];
+      n0 += w * v.x; n1 += w * v.y; n2 += w * v.z; d += w * v.w;
+    }
+    const uint8_t* cp = src + (size_t)b * sstride + (size_t)y * spitch + (size_t)x * 3;
+    uint8_t* op = dst + (size_t)b * dstride + (size_t)y * dpitch + (size_t)x * 3;
+    op[0] = masked_div(n0, d, cp[0]); op[1] = masked_div(n1, d, cp[1]); op[2] = masked_div(n2, d, cp[2]);
+  }
+}
+
+size_t mgauss_fused_smem() { return MG_SMEM; }
+
+bool launch_masked_gauss(cudaStream_t s, int n, const uint8_t* src, size_t spitch, size_t sstride, const uint8_t* mask, size_t mstride,
+                         const int* ks, int k_all, unsigned classes, uint4* tmp, uint8_t* dst, size_t dpitch, size_t dstride, int W, int H,
+                         uint8_t* yuyv, uint8_t* nv12) {
+  const GaussTables* T = gauss_tables();
+  if (!T) return false;
+  if (classes & GAUSS_FUSED) {
+    ensure_dyn_smem(reinterpret_cast<const void*>(k_mgauss_fused), MG_SMEM);
+    const dim3 grid((unsigned)ceil_div(W, GF_TW), (unsigned)ceil_div(H, GF_TH), (unsigned)n);
+    BSB_LAUNCH(k_mgauss_fused, grid, dim3(256), MG_SMEM, s, src, spitch, sstride, mask, mstride, dst, dpitch, dstride, W, H, T, k_all, ks,
+               yuyv, nv12);
+    count_launch();
+  }
+  if (classes & GAUSS_SEPARABLE) {
+    BSB_LAUNCH(k_mgauss_rows, dim3((unsigned)ceil_div(W, GAUSS_TW), (unsigned)H, (unsigned)n), dim3(256), 0, s, src, spitch, sstride, mask,
+               mstride, tmp, W, H, T, k_all, ks);
+    count_launch();
+    BSB_LAUNCH(k_mgauss_cols, dim3((unsigned)ceil_div(W, MGC_W), (unsigned)ceil_div(H, MGC_H), (unsigned)n), dim3(256), 0, s, tmp, src, spitch,
+               sstride, dst, dpitch, dstride, W, H, T, k_all, ks);
+    count_launch();
+  }
+  return true;
+}
+
 bool launch_gauss_frames(cudaStream_t s, int n, const GaussSrc& cam, const int* ks, unsigned classes, uint8_t* frames, uint16_t* tmp,
-                         uint8_t* dst, uint8_t* dst_yuyv, uint8_t* dst_nv12, int W, int H) {
+                         uint8_t* dst, uint8_t* dst_yuyv, uint8_t* dst_nv12, int W, int H, const MaskedFrames* mf) {
   const size_t fbytes = (size_t)W * H * 3;
+  // with masked frames, ks names the frames of the plain kernels and mf->ks_all every blurred frame
+  const int* all = mf ? mf->ks_all : ks;
   if (cam.p) {
     const long blocks = ((long)(W / 2) * H + 255) / 256;
-    BSB_LAUNCH(k_gauss_stage_bgr, dim3((unsigned)blocks, (unsigned)n), dim3(256), 0, s, cam, frames, W, H, ks);
+    BSB_LAUNCH(k_gauss_stage_bgr, dim3((unsigned)blocks, (unsigned)n), dim3(256), 0, s, cam, frames, W, H, all);
     count_launch();
   }
   if (!launch_gauss_classes(s, n, frames, (size_t)W * 3, fbytes, ks, 0, classes, tmp, dst, (size_t)W * 3, fbytes, W, H, dst_yuyv, dst_nv12))
     return false;
-  if ((classes & GAUSS_SEPARABLE) && (dst_yuyv || dst_nv12)) {
+  unsigned sep = classes;
+  if (mf) {
+    if (!launch_masked_gauss(s, n, frames, (size_t)W * 3, fbytes, mf->mask, mf->mstride, mf->ks, 0, mf->classes, mf->tmp, dst, (size_t)W * 3,
+                             fbytes, W, H, dst_yuyv, dst_nv12))
+      return false;
+    sep |= mf->classes;
+  }
+  if ((sep & GAUSS_SEPARABLE) && (dst_yuyv || dst_nv12)) {
     const long blocks = ((long)(W / 2) * ((H + 1) / 2) + 255) / 256;
-    BSB_LAUNCH(k_gauss_slot_yuv, dim3((unsigned)blocks, (unsigned)n), dim3(256), 0, s, dst, fbytes, dst_yuyv, dst_nv12, W, H, ks);
+    BSB_LAUNCH(k_gauss_slot_yuv, dim3((unsigned)blocks, (unsigned)n), dim3(256), 0, s, dst, fbytes, dst_yuyv, dst_nv12, W, H, all);
     count_launch();
   }
   return true;

@@ -265,6 +265,36 @@ BSB_API int bsb_set_source_mask_refine(bsb_ctx* ctx, int source, int sigma);
 /* The range weights R_sigma[d], d = 0..255, of strength sigma 1..255 into w[256] (host only).  Out of range or a null w
  * returns 0 with a bsb_last_error() message. */
 BSB_API int bsb_mask_refine_weights(int sigma, int* w);
+/* Camera blur mode.  A camera-blur frame is one whose background is its own blurred camera frame: in a plain call, no
+ * context image or ring, no live background, bgblur k > 0, the filter on, and a call that blends (a composite or video
+ * output); in a sources call, a frame whose effect blurs its camera frame (bsb_set_source_effect without an image).
+ * BSB_BLUR_PLAIN (the default) blurs the whole camera frame, person included, as the reference does
+ * (app/deepseg.cc:652-658); the person's colours are then smeared into the background around them, a halo about k/2
+ * pixels wide around the outline.  BSB_BLUR_MASKED leaves the person out of the background blur: for such a frame, with C
+ * its camera frame as the composite reads it (BGR; YUYV / NV12 after the fused path's conversion), M its W x H mask
+ * exactly as the call writes it (refined, held, 255 outside roidim), q the 8.8 taps of bsb_gaussian_taps(k), r = k >> 1
+ * and rho the BORDER_REFLECT_101 index,
+ *   h_c(x,y) = sum_j q[j] M(rho(x+j-r),y) C_c(rho(x+j-r),y)      (< 2^24)
+ *   g(x,y)   = sum_j q[j] M(rho(x+j-r),y)                         (< 2^16)
+ *   N_c(x,y) = sum_i q[i] h_c(x,rho(y+i-r))                       (< 2^32)
+ *   D(x,y)   = sum_i q[i] g(x,rho(y+i-r))                         (< 2^24)
+ *   B_c(x,y) = D > 0 ? (N_c + (D >> 1)) / D : C_c(x,y)            (uint32)
+ * B takes the place of GaussianBlur(C); the blend with the same M, flip, resize, framing, YUYV / NV12, BGRA and the
+ * camera-blur slots' cached YUYV / NV12 follow as before.  A mask uniform at any v > 0 gives GaussianBlur(C) byte for byte;
+ * k = 1 gives C; D = 0 only where M = 0 at the pixel, whose background then has no weight in the blend.
+ * The mode changes nothing for frames that blend an image (the context image or ring, a source image or ring, a live
+ * background), filter-off frames, calls that blend nothing (BGRA or mask only), bs_maskgen_process and bsb_calcmask_*.
+ * Host state only: each frame's mode reaches the device in a table with the call, so once both kinds of a call have run,
+ * changing the mode replays a captured call (the context's first masked call allocates the mask staging, and the row /
+ * column class's 16 bytes per pixel of row sums, which drops the captured calls once).  A call with no masked camera-blur frame runs exactly the kernels it runs in
+ * plain mode; one with some runs the post kernel once more, mask only, and the masked Gaussian (see README for its cost).
+ * mode: BSB_BLUR_PLAIN or BSB_BLUR_MASKED.  Out of range returns 0 with a bsb_last_error() message and changes nothing. */
+enum { BSB_BLUR_PLAIN = 0, BSB_BLUR_MASKED = 1 };
+BSB_API int bsb_set_blur_mode(bsb_ctx* ctx, int mode);
+/* One source's mode: -1 follows bsb_set_blur_mode (including later changes), else BSB_BLUR_PLAIN or BSB_BLUR_MASKED.
+ * bsb_set_sources resets every source to -1; bsb_reset_source keeps it.  No bsb_set_sources yet, a source id out of range
+ * or a mode out of range returns 0 with a bsb_last_error() message and changes nothing. */
+BSB_API int bsb_set_source_blur_mode(bsb_ctx* ctx, int source, int mode);
 /* Live backgrounds (the reference's `-b` takes any OpenCV source and blends its newest frame every loop iteration,
  * app/deepseg.cc:522-524,648-661): device images the caller already holds (decoded video surfaces, screen captures, a
  * second camera) are resized, blurred and blended inside the call, with no host copy and no launch outside it.
@@ -541,6 +571,8 @@ BSB_API int bsb_convert_nv12_to_bgr(int device, const uint8_t* nv12, uint8_t* bg
 /* cv::GaussianBlur(src, dst, Size(k,k), 0) 8UC3 (app/deepseg.cc:657-658) and its 8.8 fixed-point taps (host only) */
 BSB_API int bsb_gaussian_blur(int device, const uint8_t* src, uint8_t* dst, int width, int height, int ksize);
 BSB_API int bsb_gaussian_taps(int ksize, int* taps);
+/* The masked camera blur B of bsb_set_blur_mode: src 8UC3, mask 8UC1 (any bytes), both width x height */
+BSB_API int bsb_masked_gaussian_blur(int device, const uint8_t* src, const uint8_t* mask, uint8_t* dst, int width, int height, int ksize);
 /* cv::flip(src, dst, code) 8UC3 (app/deepseg.cc:667-673) */
 BSB_API int bsb_flip(int device, const uint8_t* src, uint8_t* dst, int width, int height, int flip_h, int flip_v);
 /* cv::resize(src, dst, Size(dw, dh)) 8UC3 (app/background.cc:178-194) */
